@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- Mpoints/s through the fused view-aggregation forward+backward (BASELINE.json).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 Workload (named in config.workload): the synthetic stress case the metric is quoted on --
@@ -12,10 +12,11 @@ independent batch; the only collective is the NCCL all-reduce of the pool-parame
 (SURVEY 8e: ~160 KB -- the gate gradients the kernels produce live at its head), issued on a side
 stream so that it overlaps the next step's forward.
 
-Timing: a measurement is EXACTLY --steps steps between two CUDA events, bracketed by a barrier and a
-device synchronisation on both sides, max over ranks.  That measurement is repeated (`rounds`, sized
-so that the timed regions add up to >= 2.5 s) and the MEDIAN round is reported; every round, the mean
-and per-rank step statistics are in `consistency`.
+Timing: after --warmup untimed steps, EXACTLY --steps steps run between two CUDA events, bracketed by a
+barrier and a device synchronisation on both sides, max over ranks; per-rank step statistics are in
+`consistency`.  --dump-outputs DIR then writes what the last timed step computed (rank 0) as .npy files:
+out [N, C], gx [V, C] and gcompat [V, G] on a fixed, seeded sample of rows (row ids in *_rows.npy), and the
+gate gradient ggate [2, G] in full; the inputs are seeded, so two builds can be compared output for output.
 
 value : device-resident throughput (inputs in HBM), CUDA events, max over ranks.
 e2e   : the same step through the host-buffer API (deepviewagg_b200.host_api): pinned host inputs
@@ -68,7 +69,7 @@ def emit(obj):
 def parse():
     p = argparse.ArgumentParser()
     p.add_argument("--gpus", type=int, default=1)
-    p.add_argument("--steps", type=int, default=30)
+    p.add_argument("--steps", type=int, default=150)      # ~2.8 s of timed steps on an H100
     p.add_argument("--warmup", type=int, default=5)
     p.add_argument("--impl", default="ours", choices=["ours", "reference"])
     p.add_argument("--points", type=int, default=1_000_000)
@@ -78,7 +79,8 @@ def parse():
     p.add_argument("--dtype", default="f32", choices=["f32", "bf16"])
     p.add_argument("--idx", default="randperm", choices=["randperm", "arange", "none"])
     p.add_argument("--counts", default="uniform", choices=["uniform", "ragged"])
-    p.add_argument("--rounds", type=int, default=0, help="timed repetitions of the K-step region (0 = from a 2.5 s budget)")
+    p.add_argument("--dump-outputs", default="", metavar="DIR",
+                   help="write the last timed step's results (fixed row sample) to DIR/<name>.npy")
     p.add_argument("--sweep", default="", help="comma list of views per point (BASELINE config #5: 8,16,32,64): extra "
                                                "device-resident measurements under roofline_detail.sweep")
     p.add_argument("--no-variant-b", action="store_true", help="skip the variant-B side measurement (QKVBimodalCSRPool: scores "
@@ -102,7 +104,7 @@ def hbm_peak():
         with open(path) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3)"
 
 
 # ---------------------------------------------------------------------------------------------------
@@ -118,7 +120,7 @@ class ClockSampler:
     """SM clocks / throttle reasons of the given GPUs, sampled in-process through NVML from a
     background thread of rank 0 (no nvidia-smi children: at N = 8 eight of them initialising NVML
     inside a sub-second timed window was one of the round-1 scaling suspects).  start() is called
-    >= 2 s before the timed region; mark()/unmark() delimit the samples that count as "under load"."""
+    before the warm-up steps; mark()/unmark() delimit the samples that count as "under load"."""
 
     def __init__(self, gpu_indices, period_s=0.05):
         self.gpus, self.period = list(gpu_indices), period_s
@@ -290,18 +292,52 @@ def workload_config(args, world):
                                  if args.dtype == "f32" else
                                  "bf16 storage, fp32 accumulate: within 1.6e-2 of the tensor's max (2 bf16 ulps) of the fp32 "
                                  "oracle -- reported separately from the 1e-4 fp32 bar"),
-            "l2": "inputs (>16 GB per step) exceed the 126 MB L2; no explicit flush needed"}
+            "l2": "inputs (>16 GB per step) exceed the 50 MB L2; no explicit flush needed"}
 
 
-def ncu_traffic(args):
-    """DRAM bytes per launch measured by ncu for this exact workload (profiles/ncu_traffic.json), or {}."""
-    key = (f"points={args.points} views={args.views} channels={args.channels} groups={args.groups} "
-           f"dtype={args.dtype} idx={args.idx} counts={args.counts}")
+DUMP_SAMPLE_ROWS = 32768     # rows of out / gx / gcompat written by --dump-outputs: 2 x 16 MB at C = 128 fp32 ...
+DUMP_BUDGET_BYTES = 64 << 20  # ... and fewer at wider rows, so that every dump stays within 64 MB
+
+
+def gpu_identity(index):
+    """Name and enforced power limit of the GPU a number was measured on (part of the number)."""
+    info = {"name": torch.cuda.get_device_name(index), "power_limit_w": None}
     try:
-        with open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "profiles", "ncu_traffic.json")) as f:
-            return json.load(f).get(key, {})
-    except (OSError, ValueError):
-        return {}
+        import pynvml as nv
+        nv.nvmlInit()
+        h = nv.nvmlDeviceGetHandleByIndex(index)
+        info["power_limit_w"] = nv.nvmlDeviceGetEnforcedPowerLimit(h) / 1000.0
+    except Exception:
+        try:
+            out = subprocess.run(["nvidia-smi", "-i", str(index), "--query-gpu=power.limit",
+                                  "--format=csv,noheader,nounits"], capture_output=True, text=True, timeout=30)
+            info["power_limit_w"] = float(out.stdout.strip())
+        except Exception:
+            pass
+    return info
+
+
+def dump_outputs(path, plan, ggate):
+    """The last step's results as float32 .npy files; row-wise outputs on a sample fixed by a CPU seed."""
+    import numpy as np
+    os.makedirs(path, exist_ok=True)
+    gen = torch.Generator().manual_seed(2024)
+
+    # per sampled row: out and gx rows (fp32), a gcompat row (fp32), two row ids (float64)
+    per_row = 2 * plan.C * 4 + plan.G * 4 + 2 * 8
+    k_max = min(DUMP_SAMPLE_ROWS, (DUMP_BUDGET_BYTES - 4096) // per_row)
+
+    def rows(n):
+        return torch.randperm(n, generator=gen)[:min(n, k_max)].sort().values
+
+    pr, vr = rows(plan.N), rows(plan.V)
+    arrays = {"out": plan.out[pr.to(plan.device)], "gx": plan.gx[vr.to(plan.device)],
+              "gcompat": plan.gcompat[vr.to(plan.device)], "ggate": ggate}
+    for name, t in arrays.items():
+        np.save(os.path.join(path, name + ".npy"), t.detach().float().cpu().numpy())
+    # row ids above 2^24 are not exact in float32
+    np.save(os.path.join(path, "out_rows.npy"), pr.numpy().astype(np.float64))
+    np.save(os.path.join(path, "gx_rows.npy"), vr.numpy().astype(np.float64))
 
 
 # ---------------------------------------------------------------------------------------------------
@@ -347,15 +383,15 @@ def main():
     plan = ViewAttentionHostPlan(N, V, V, C, G, dtype=tdtype, idx_dtype=idx_dtype, gating=True,
                                  group_scaling=True, device=dev)
     plan.ptr.copy_(ptr)
-    plan.x.copy_(torch.randn(V, C, device=dev, generator=gen).to(tdtype))
+    plan.x.normal_(generator=gen)                    # in place: a [V, C] temporary would double x's footprint
     if args.idx == "randperm":
         plan.idx.copy_(torch.randperm(V, device=dev, generator=gen).int())
     elif args.idx == "arange":
         plan.idx.copy_(torch.arange(V, device=dev).int())
-    plan.compat.copy_(torch.randn(V, G, device=dev, generator=gen))
+    plan.compat.normal_(generator=gen)
     plan.gate[0].fill_(1.0)
     plan.gate[1].fill_(0.0)
-    plan.gout.copy_(torch.randn(N, C, device=dev, generator=gen).to(tdtype))
+    plan.gout.normal_(generator=gen)
     torch.cuda.synchronize()
 
     # ---- the path's only exchange: the pool-parameter gradient bucket (SURVEY 8e) ------------------
@@ -396,76 +432,53 @@ def main():
         if side is not None:
             main_stream.wait_stream(side)
 
-    W_ = max(args.warmup, 3)
+    W_ = args.warmup
+    sampler = ClockSampler(list(range(int(os.environ.get("LOCAL_WORLD_SIZE", str(world))))) if world > 1
+                           else [local]) if rank == 0 else None
+    if sampler is not None:
+        sampler.start()
     for _ in range(W_):
         step()
     drain()
     torch.cuda.synchronize()
 
     K = args.steps
-    # one measurement = exactly K steps; rounds sized so that the timed regions total >= 2.5 s
+    if K < 1:
+        raise SystemExit("--steps must be at least 1")
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    ev = [[torch.cuda.Event(enable_timing=True) for _ in range(3)] for _ in range(K)]
+    if dist is not None:
+        dist.barrier()
+    torch.cuda.synchronize()
+    launches0 = _lib.launch_count()
+    if sampler is not None:
+        sampler.mark()
     e0.record()
-    for _ in range(K):
-        step()
-    drain()
+    for k in range(K):
+        step(ev[k])
+    drain()                                              # the last all-reduces finish inside the region
     e1.record()
     torch.cuda.synchronize()
-    probe_ms = torch.tensor([e0.elapsed_time(e1)], device=dev, dtype=torch.float64)
-    if dist is not None:
-        dist.all_reduce(probe_ms, op=dist.ReduceOp.MAX)
-    rounds = args.rounds if args.rounds > 0 else int(min(40, max(3, -(-2500.0 // float(probe_ms.item())))))
-
-    sampler = ClockSampler(list(range(int(os.environ.get("LOCAL_WORLD_SIZE", str(world))))) if world > 1
-                           else [local]) if rank == 0 else None
     if sampler is not None:
-        sampler.start()
-    # >= 2 s of the same work before the first timed round: the sampler is up, clocks are settled
-    t_pre = time.perf_counter()
-    while time.perf_counter() - t_pre < 2.0:
-        for _ in range(K):
-            step()
-        drain()
-        torch.cuda.synchronize()
-
-    ev = [[[torch.cuda.Event(enable_timing=True) for _ in range(3)] for _ in range(K)] for _ in range(rounds)]
-    round_ms = []
-    launches = 0
-    for r in range(rounds):
-        if dist is not None:
-            dist.barrier()
-        torch.cuda.synchronize()
-        launches0 = _lib.launch_count()
-        if sampler is not None:
-            sampler.mark()
-        e0.record()
-        for k in range(K):
-            step(ev[r][k])
-        drain()                                          # the last all-reduces finish inside the region
-        e1.record()
-        torch.cuda.synchronize()
-        if sampler is not None:
-            sampler.unmark()
-        launches = _lib.launch_count() - launches0
-        if dist is not None:
-            dist.barrier()
-        t = torch.tensor([e0.elapsed_time(e1)], device=dev, dtype=torch.float64)
-        if dist is not None:
-            dist.all_reduce(t, op=dist.ReduceOp.MAX)
-        round_ms.append(float(t.item()))
+        sampler.unmark()
+    launches = _lib.launch_count() - launches0
+    if dist is not None:
+        dist.barrier()
+    t = torch.tensor([e0.elapsed_time(e1)], device=dev, dtype=torch.float64)
+    if dist is not None:
+        dist.all_reduce(t, op=dist.ReduceOp.MAX)
+    elapsed_ms = float(t.item())
     clocks = sampler.stop() if sampler is not None else None
+    if rank == 0 and args.dump_outputs:
+        dump_outputs(args.dump_outputs, plan, plan.ggate)
     pts = torch.tensor([float(N)], device=dev, dtype=torch.float64)
     if dist is not None:
         dist.all_reduce(pts, op=dist.ReduceOp.SUM)
     total_points = float(pts.item())
-    elapsed_ms = statistics.median(round_ms)
     value = total_points * K / (elapsed_ms * 1e-3) / 1e6
 
     # per-rank step statistics (ms, event-timed start of step k -> start of step k+1) so a straggler is named
-    own = []
-    for r in range(rounds):
-        for k in range(K - 1):
-            own.append(ev[r][k][0].elapsed_time(ev[r][k + 1][0]))
+    own = [ev[k][0].elapsed_time(ev[k + 1][0]) for k in range(K - 1)]
     own_t = torch.tensor([min(own), statistics.median(own), max(own)] if own else [0.0, 0.0, 0.0],
                          device=dev, dtype=torch.float64)
     if dist is not None:
@@ -474,32 +487,25 @@ def main():
     else:
         allr = [own_t]
     per_rank = [{"rank": i, "min": float(t[0]), "median": float(t[1]), "max": float(t[2])} for i, t in enumerate(allr)]
-    consistency = {"rounds": rounds, "steps_per_round": K, "round_ms": round_ms,
-                   "timed_region_s": sum(round_ms) * 1e-3,
-                   "mean_ms_per_step": sum(round_ms) / (rounds * K), "median_ms_per_step": elapsed_ms / K,
-                   "min_ms_per_step": min(round_ms) / K, "max_ms_per_step": max(round_ms) / K,
+    consistency = {"steps": K, "timed_region_s": elapsed_ms * 1e-3, "mean_ms_per_step": elapsed_ms / K,
                    "per_rank_step_ms": per_rank,
                    "allreduce": {"elements": n_bucket, "bytes": 4 * n_bucket,
                                  "where": "side stream, overlaps the next step; drained inside the timed region"}
                    if dist is not None else None,
                    "numa": numa_info}
 
-    flat = [e for r in ev for e in r]
-    fwd_ms = statistics.mean(e[0].elapsed_time(e[1]) for e in flat)
-    bwd_ms = statistics.mean(e[1].elapsed_time(e[2]) for e in flat)
+    fwd_ms = statistics.mean(e[0].elapsed_time(e[1]) for e in ev)
+    bwd_ms = statistics.mean(e[1].elapsed_time(e[2]) for e in ev)
     b_fwd, b_bwd = algorithmic_bytes(N, V, C, G, s)
     peak, peak_src = hbm_peak()
     ach_bwd = b_bwd / (bwd_ms * 1e-3) / 1e9
     ach_fwd = b_fwd / (fwd_ms * 1e-3) / 1e9
     ach_step = (b_fwd + b_bwd) / ((fwd_ms + bwd_ms) * 1e-3) / 1e9
-    traffic = ncu_traffic(args)
     roofline = {"bound": "hbm", "kernel": "view_attention_bwd_kernel", "achieved": ach_bwd, "peak": peak,
-                "unit": "GB/s", "frac": ach_bwd / peak, "traffic": traffic.get("view_attention_bwd_kernel"),
-                "traffic_source": traffic.get("source"), "peak_source": peak_src,
+                "unit": "GB/s", "frac": ach_bwd / peak, "peak_source": peak_src,
                 "algorithmic_bytes_per_launch": b_bwd, "ms_per_launch": bwd_ms}
     extra_roof = {
         "fwd": {"kernel": "view_attention_fwd_kernel", "achieved": ach_fwd, "frac": ach_fwd / peak,
-                "traffic": traffic.get("view_attention_fwd_kernel"),
                 "algorithmic_bytes_per_launch": b_fwd, "ms_per_launch": fwd_ms},
         "fwd_plus_bwd": {"achieved": ach_step, "frac": ach_step / peak,
                          "algorithmic_bytes": b_fwd + b_bwd, "ms": fwd_ms + bwd_ms}}
@@ -509,8 +515,6 @@ def main():
     if not args.no_e2e:
         e2e = run_e2e(args, plan, dist, dev, world, N, V, n_bucket)
 
-    if rank == 0 and world == 1 and args.sweep:
-        extra_roof["sweep"] = run_sweep(args, dev, peak, [int(t) for t in args.sweep.split(",") if t])
     if rank == 0 and world == 1 and not args.no_variant_b:
         try:
             extra_roof["variant_b"] = run_variant_b(args, plan, dev, peak, N, V)
@@ -521,6 +525,14 @@ def main():
             extra_roof["modules"] = run_module_workloads(dev, peak)
         except Exception as e:  # the graded line must survive a failure of this side measurement
             extra_roof["modules"] = {"error": f"{type(e).__name__}: {e}"}
+    if rank == 0 and world == 1 and args.sweep:
+        # the main line's plan (~34 GB at 1 M x 32 x 128) is released first: a 64-view sweep point needs ~70 GB
+        del plan
+        torch.cuda.empty_cache()
+        try:
+            extra_roof["sweep"] = run_sweep(args, dev, peak, [int(t) for t in args.sweep.split(",") if t])
+        except Exception as e:
+            extra_roof["sweep"] = {"error": f"{type(e).__name__}: {e}"}
 
     cpu_baseline = None
     if rank == 0 and world == 1 and not args.no_cpu_baseline:
@@ -545,7 +557,7 @@ def main():
             "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": K,
             "warmup": W_, "ms_per_step": elapsed_ms / K, "higher_is_better": True,
             "scaling": "weak", "vs_baseline": None, "dtype": args.dtype, "data": "synthetic",
-            "config": workload_config(args, world), "clocks": clocks, "e2e": e2e,
+            "config": workload_config(args, world), "gpu": gpu_identity(local), "clocks": clocks, "e2e": e2e,
             "gpu_launches": int(launches), "roofline": roofline, "roofline_detail": extra_roof,
             "cpu_baseline": cpu_baseline, "consistency": consistency,
         }
@@ -611,7 +623,10 @@ def run_module_workloads(dev, peak, steps=20, warmup=5):
 
 def run_sweep(args, dev, peak, views_list, steps=10, warmup=3):
     """BASELINE.json config #5: the same fused pair at N points x v views for every v of the sweep (uniform counts,
-    random permutation), device-resident, median over `steps` launches."""
+    random permutation), device-resident, median over `steps` launches.  Runs after the main line's buffers are
+    freed, one sweep point at a time.  Peak device memory of one point at fp32, C = 128 (V = N v): x and grad_x
+    2 x 512 V bytes, idx 4 V, compat and grad_compat 2 x 16 V, randperm temporaries 12 V, [N, C] and [N, G]
+    buffers ~1.1 kB N: 1 M x 64 views = 69.7 GB (64.9 GiB) of the H100's 79.6 GiB."""
     from deepviewagg_b200.host_api import ViewAttentionHostPlan
     tdtype = torch.float32 if args.dtype == "f32" else torch.bfloat16
     s = 4 if args.dtype == "f32" else 2
@@ -623,12 +638,12 @@ def run_sweep(args, dev, peak, views_list, steps=10, warmup=3):
         plan = ViewAttentionHostPlan(N, V, V, C, G, dtype=tdtype, idx_dtype=torch.int32, gating=True, group_scaling=True,
                                      device=dev)
         plan.ptr.copy_(torch.arange(0, V + 1, v, device=dev))
-        plan.x.copy_(torch.randn(V, C, device=dev, generator=gen).to(tdtype))
+        plan.x.normal_(generator=gen)
         plan.idx.copy_(torch.randperm(V, device=dev, generator=gen).int())
-        plan.compat.copy_(torch.randn(V, G, device=dev, generator=gen))
+        plan.compat.normal_(generator=gen)
         plan.gate[0].fill_(1.0)
         plan.gate[1].fill_(0.0)
-        plan.gout.copy_(torch.randn(N, C, device=dev, generator=gen).to(tdtype))
+        plan.gout.normal_(generator=gen)
         fw, bw = [], []
         for i in range(warmup + steps):
             e = [torch.cuda.Event(enable_timing=True) for _ in range(3)]

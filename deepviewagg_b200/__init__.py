@@ -1,4 +1,4 @@
-"""deepviewagg_b200 -- B200 (sm_100a) implementation of DeepViewAgg's multi-view aggregation
+"""deepviewagg_b200 -- H100 (sm_90a) implementation of DeepViewAgg's multi-view aggregation
 hot path behind the reference's torch_points3d/modules/multimodal operator API.
 
 Layout (only what the path needs):

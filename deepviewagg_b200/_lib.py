@@ -92,7 +92,7 @@ _lib = None
 
 
 def build(verbose=False):
-    """Compile libdva_b200.so for sm_100a (nvcc cross-compiles without a GPU)."""
+    """Compile libdva_b200.so for sm_90a (nvcc cross-compiles without a GPU)."""
     out = subprocess.run(["make", "-C", CSRC_DIR, "-j8"], capture_output=True, text=True)
     if verbose or out.returncode != 0:
         print(out.stdout[-4000:])
@@ -149,7 +149,7 @@ def require_cuda(*tensors):
     for t in tensors:
         if t is not None and not t.is_cuda:
             raise RuntimeError(
-                "deepviewagg_b200 operators run on CUDA tensors only (sm_100a kernels, no CPU "
+                "deepviewagg_b200 operators run on CUDA tensors only (sm_90a kernels, no CPU "
                 "fallback); got a tensor on " + str(t.device))
 
 

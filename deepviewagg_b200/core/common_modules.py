@@ -3,7 +3,7 @@
 state_dicts load unchanged: `<mlp>.<i>.0.weight`, `<mlp>.<i>.1.batch_norm.{weight,bias,
 running_mean,running_var,num_batches_tracked}`.
 
-The dense projections go through ops.linear (3xTF32 mma.sync kernels for K, N <= 64, tcgen05
+The dense projections go through ops.linear (3xTF32 mma.sync kernels for K, N <= 64, wgmma
 kernels for wider layers, widths that are not a multiple of 4 zero-padded) -- the only
 tensor-core work on this path; BatchNorm uses batch statistics over ALL rows in training.
 """

@@ -1,4 +1,4 @@
-// Shared device/host helpers for libdva_b200 (sm_100a only).
+// Shared device/host helpers for libdva_b200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -11,7 +11,7 @@
 
 namespace dva {
 
-constexpr int kNumSMs = 148;  // B200: 2 dies x 74 SMs; grids are sized in multiples of this
+constexpr int kNumSMs = 132;  // H100 SXM; grids are sized in multiples of this
 
 // ---- thread-local error string + launch counter (C ABI: dva_last_error), process-wide launch counter (dva_launch_count)
 char* tls_error_buf();

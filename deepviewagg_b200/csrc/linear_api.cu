@@ -1,5 +1,5 @@
 // C ABI of the projection GEMMs of the pool MLPs: dispatch between the skinny mma.sync kernels
-// (skinny_gemm.cu: K, N <= 64) and the hand-written tcgen05 kernels (tc_gemm.cu: everything wider).
+// (skinny_gemm.cu: K, N <= 64) and the hand-written wgmma kernels (tc_gemm.cu: everything wider).
 #include "dva_common.cuh"
 #include <stdlib.h>
 
@@ -18,20 +18,17 @@ extern "C" int dva_tc_dw_gemm(const float* dZ, const float* X, float* D, int64_t
 
 using namespace dva;
 
-// Which family serves a shape.  The skinny mma.sync kernels take every K, N <= 64; measured on the B200
-// (1.28 M rows): 64 -> 64 forward / dX 0.25 / 0.19 ms on the skinny kernels against 0.146 ms on the tcgen05 rows
-// kernel, 32-wide layers on a par (0.07 - 0.08 ms) -> rows kernels (layouts 0, 1) go to tcgen05 when both widths
-// exceed 32 and are multiples of 4; dW (layout 2) likewise since the tcgen05 dW kernel packs its stages (round 2).
-// Round 2: the 32-wide rows GEMMs (N >= 32, K >= 8) go to the tcgen05 kernel too -- on a par as plain GEMMs, but
-// the BatchNorm statistics then come out of its epilogue (module step 6.06 -> 5.92 ms at the S3DIS shape).
-// DVA_TC_NARROW=0 (A/B knob, read once) restores the round-1 routing.
+// Which family serves a shape.  The skinny mma.sync kernels take every K, N <= 64; rows GEMMs (layouts 0, 1)
+// with N >= 32 and K >= 8 go to the wgmma rows kernel, whose epilogue also yields the BatchNorm statistics of the
+// layer; dW (layout 2) goes to the wgmma dW kernel when both widths exceed 32 (all widths multiples of 4).
+// DVA_TC_NARROW=0 (A/B knob, read once) sends the 32-wide rows GEMMs to the skinny kernels as well.
 extern "C" int dva_tc_narrow() {
   static const int v = [] { const char* e = getenv("DVA_TC_NARROW"); return (e && e[0] == '0') ? 0 : 1; }();
   return v;
 }
 static bool use_skinny(int64_t M, int64_t N, int64_t K, int layout) {
   if (!dva_skinny_gemm_supported(M, N, K, layout)) return false;
-  if (layout == 2) return !(N > 32 && K > 32 && N % 4 == 0 && K % 4 == 0);   // 64 x 64: 2 x 155 us here, tcgen05 dW below that
+  if (layout == 2) return !(N > 32 && K > 32 && N % 4 == 0 && K % 4 == 0);
   if (dva_tc_narrow()) return !(N >= 32 && K >= 8 && N % 4 == 0 && K % 4 == 0);
   return !(N > 32 && K > 32 && N % 4 == 0 && K % 4 == 0);
 }

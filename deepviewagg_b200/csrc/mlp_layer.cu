@@ -6,9 +6,8 @@
 //                        dX = dz . W  and  dW += dz^T . x  from the same tile            reads dA, z, x; writes dX
 // Before: BN-apply (2 R + 1 W), dX GEMM (1 R + 1 W), dW GEMM (2 R) = 5 R + 2 W passes and three launches after
 // the reduction; now 3 R + 1 W and one launch.  3xTF32 split operands on mma.sync.m16n8k8 (fp32-grade accuracy,
-// the arithmetic of skinny_gemm.cu).  Measured at 1.28 M x 32 x 32: 0.106 ms inside a training step (inputs partly
-// L2-resident), 0.155 ms cold under ncu, against 0.100 ms of HBM time; the first version, with integer divisions by
-// the run-time row width in the copy loops, took 0.137 / 0.200 ms (issue-bound: 1 500 instructions per tile).
+// the arithmetic of skinny_gemm.cu).  The copy and store loops use a fixed lane -> (row, 16-byte chunk) map: integer
+// divisions by the run-time row width there made an earlier version issue-bound.
 //
 // A WARP is its own pipeline: 16-row tiles (dA, z, x) double-buffered with cp.async in the warp's private shared
 // memory, no CTA-wide barrier inside the loop; the dW accumulators (N x K, 32 .. 64 registers per lane) live in

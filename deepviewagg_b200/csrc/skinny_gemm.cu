@@ -1,9 +1,8 @@
 // Skinny projections of the pool MLPs (base_modules.py:42 -- Linear(bias=False) inside every MLP
 // layer of DeepSetFeat / E_mod / E_mix, pooling.py:239-261, 645-656): [rows, K] x [N, K]^T with
 // K, N <= 64 and millions of rows (one per view).  2*K*N flops against 4*(K+N) bytes per row is
-// ~16 flop/byte at K = N = 32: HBM-bound on the fp32 pipes already, and far too narrow for the
-// 128x64 tcgen05 tiles of mlp_gemm.cu (measured there: 0.50 ms per launch at 1.28 M x 32 x 32,
-// 10x the HBM time).  Exact fp32 FFMA, weights resident in shared memory, every global access a
+// ~16 flop/byte at K = N = 32: HBM-bound on the fp32 pipes already, and too narrow to fill the
+// 128-wide tiles of the wgmma kernels (tc_gemm.cu).  Exact fp32 FFMA, weights resident in shared memory, every global access a
 // coalesced 16-byte vector through a shared staging tile:
 //   layouts 0/1  skinny_rows_mma_kernel : D[M,OUT] = A[M,RED] . Wt[RED,OUT] on mma.sync with 3xTF32
 //                split operands (fp32-grade accuracy); skinny_rows_kernel: the same on the fp32

@@ -8,7 +8,7 @@
 // which materialises >= 4 [V,C] temporaries in the reference.
 //
 // Work decomposition: one warp owns one point (CSR segment) at a time; CTAs are persistent
-// (148 SMs x occupancy) and stride over the points.  A feature row of C channels is split into
+// (kNumSMs x occupancy) and stride over the points.  A feature row of C channels is split into
 // 16-byte chunks; LPR lanes cover one row (LPR*CPL chunks), so a warp reads 32/LPR rows per step
 // with every lane issuing one LDG.128 -- for C=128 fp32 a row is exactly one 512 B warp-wide
 // load, kUnroll of them in flight per lane.  Scores live in the flat (view,group) order of
@@ -605,7 +605,7 @@ static VAConfig choose_config(const VAParams& P, const void* o1, const void* o2,
   return cfg;
 }
 
-// persistent grid: exactly the number of CTAs that are co-resident (148 SMs x occupancy), so the
+// persistent grid: exactly the number of CTAs that are co-resident (kNumSMs x occupancy), so the
 // grid-stride point loop has no second wave; never more CTAs than there are point groups.
 template <typename K>
 static int va_grid(K kern, size_t smem, int64_t N) {
@@ -697,10 +697,11 @@ static std::atomic<int>& va_path() {
   return p;
 }
 
-// auto (measured on B200, tools/bench_shapes.py, profiles/r1_shapes_*.json): the ring kernels win
-// where per-point scalar work dominates -- short segments.  Forward: fewer than
-// DVA_RING_MAX_MEAN_VIEWS views per point on average; backward: additionally rows of at most 128
-// bytes (with wider rows the streaming backward is as fast and needs no shared-memory tiles).
+// auto, chosen with tools/bench_shapes.py on an H100 at a 400 W power limit (1 M-point stress shapes at 8 - 64 views, the shipped-config
+// step shapes at 32 - 512 channels): the ring kernels win where per-point scalar work dominates -- short segments.
+// Forward: at most DVA_RING_MAX_MEAN_VIEWS views per point on average (elsewhere within 1 % of streaming).
+// Backward: short segments with rows of 129 - 512 bytes (e.g. 160 k x ~8 x 64 fp32: 0.310 ms against 0.324 ms for
+// the lane kernel); the lane kernel below takes every other shape.
 #ifndef DVA_RING_MAX_MEAN_VIEWS
 #define DVA_RING_MAX_MEAN_VIEWS 12
 #endif
@@ -711,19 +712,16 @@ static bool use_ring(const VAParams& P, int dtype, bool applicable, bool backwar
   if (path == 2) return true;
   if (P.V > (int64_t)DVA_RING_MAX_MEAN_VIEWS * P.N) return false;
   const size_t esz = dtype == DVA_F32 ? 4 : 2;
-  return !backward || (size_t)P.C * esz <= 128;
+  return !backward || ((size_t)P.C * esz > 128 && (size_t)P.C * esz <= 512);
 }
 
-// backward only: the lane-per-view kernel (view_attention_lane.cu) for short segments, path 3 forces it
-// auto (profiles/r2_shapes_*.json): short segments AND rows of at most 256 bytes -- with 512-byte rows the
-// streaming backward is as fast (1 M x 8 x 128: 1.85 ms vs 1.99 ms)
-static bool use_lane_bwd(const VAParams& P, int dtype, bool applicable) {
+// backward only: the lane-per-view kernel (view_attention_lane.cu), path 3 forces it.  auto: wherever the ring
+// backward is not chosen -- on the H100 (400 W) it is never slower than the streaming backward (within 0.5 %) and 4 - 5 %
+// faster at long segments (1 M x 32 x 128 fp32: 12.80 ms against 13.26 ms)
+static bool use_lane_bwd(const VAParams& P, bool applicable) {
   if (!applicable) return false;
   const int path = va_path().load(std::memory_order_relaxed);
-  if (path == 3) return true;
-  if (path != 0) return false;
-  const size_t esz = dtype == DVA_F32 ? 4 : 2;
-  return P.V <= (int64_t)DVA_RING_MAX_MEAN_VIEWS * P.N && (size_t)P.C * esz <= 256;
+  return path == 0 || path == 3;
 }
 
 }  // namespace dva
@@ -770,7 +768,7 @@ extern "C" int dva_view_attention_set_path(int path) {
 }
 
 extern "C" size_t dva_view_attention_bwd_workspace_bytes(int64_t G) {
-  // one [2,G] partial per CTA of the persistent grid (at most 148 SMs x 8 co-resident CTAs)
+  // one [2,G] partial per CTA of the persistent grid (at most kNumSMs x 8 co-resident CTAs)
   return (size_t)kNumSMs * 8 * 2 * (size_t)(G > 0 ? G : 1) * sizeof(float);
 }
 
@@ -808,10 +806,10 @@ extern "C" int dva_view_attention_bwd(const void* x, const void* idx, int idx_is
   int grid = 1;
   int rc;
   if (dtype != DVA_F32 && dtype != DVA_BF16 && dtype != DVA_F16) return fail(DVA_EINVAL, "view_attention_bwd: unknown dtype");
-  if (use_lane_bwd(P, dtype, va_lane_bwd_applicable(P, dtype))) {
-    rc = va_lane_bwd(P, dtype, &grid, st);
-  } else if (use_ring(P, dtype, va_ring_bwd_applicable(P, dtype), true)) {
+  if (use_ring(P, dtype, va_ring_bwd_applicable(P, dtype), true)) {
     rc = va_ring_bwd(P, dtype, &grid, st);
+  } else if (use_lane_bwd(P, va_lane_bwd_applicable(P, dtype))) {
+    rc = va_lane_bwd(P, dtype, &grid, st);
   } else {
     switch (dtype) {
       case DVA_F32: rc = bwd_typed<float>(P, &grid, st); break;

@@ -393,7 +393,7 @@ static int lane_bwd_launch(const VAParams& P, int* grid_out, cudaStream_t st) {
   if (e != cudaSuccess) return fail((int)e, "va_lane_bwd: cannot reserve shared memory");
   int occ = 0;
   if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, kLaneWarps * 32, smem) != cudaSuccess || occ < 1) occ = 1;
-  if (occ > 8) occ = 8;                                          // gate partials: at most 148 x 8 CTAs
+  if (occ > 8) occ = 8;                                          // gate partials: at most kNumSMs x 8 CTAs
   int64_t grid = (int64_t)kNumSMs * occ;
   const int64_t warps = grid * kLaneWarps;
   int64_t pr = (P.N + warps * 4 - 1) / (warps * 4);              // ~4 ranges per warp: balances ragged counts

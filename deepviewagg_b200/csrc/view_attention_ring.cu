@@ -63,8 +63,9 @@ constexpr uint32_t FULL = 0xffffffffu;
 #endif
 constexpr int kP1Unroll = DVA_RING_P1_UNROLL;   // score loads in flight per lane in the lane-per-point phases
 
-// Batch size (measured, tools/bench_shapes.py): forward likes 16 rows per batch for 128/256-byte
-// rows and more resident warps (2 KB batches) for 64- and 512-byte rows; backward 4 KB throughout.
+// Batch size (chosen with tools/bench_shapes.py on another GPU; the H100 sweep of the dispatch, view_attention.cu,
+// ran with these): forward likes 16 rows per batch for 128/256-byte rows and more resident warps (2 KB batches)
+// for 64- and 512-byte rows; backward 4 KB throughout.
 template <int LPR, bool BWD> struct RingGeom {
   static constexpr int RPI = 32 / LPR;                       // rows per warp step
   static constexpr int RS = LPR * 16;                        // row stride in the ring (bytes)
@@ -871,7 +872,7 @@ bool va_ring_bwd_applicable(const VAParams& P, int dtype) {
   }
 }
 
-// grid = co-resident CTAs (148 SMs x occupancy); PR = points per range (one range per warp when
+// grid = co-resident CTAs (kNumSMs x occupancy); PR = points per range (one range per warp when
 // the problem is large enough, never fewer than 8 points)
 template <typename K>
 static int ring_launch_geometry(K kern, size_t smem, int64_t N, int max_ctas_per_sm, int* grid_out, int* pr_out) {
@@ -908,7 +909,7 @@ static int ring_bwd_launch(const VAParams& P, int* grid_out, cudaStream_t st) {
   const size_t smem = L.total * kRingWarps;
   auto kern = va_ring_bwd_kernel<T, LPR>;
   int grid, pr;
-  if (int rc = ring_launch_geometry(kern, smem, P.N, 8, &grid, &pr)) return rc;   // gate-gradient workspace: 148 x 8 partials
+  if (int rc = ring_launch_geometry(kern, smem, P.N, 8, &grid, &pr)) return rc;   // gate-gradient workspace: kNumSMs x 8 partials
   *grid_out = grid;
   kern<<<grid, kRingWarps * 32, smem, st>>>(P, pr);
   return check_launch("view_attention_bwd(ring)");

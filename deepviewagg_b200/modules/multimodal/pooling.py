@@ -1,4 +1,4 @@
-"""Drop-in mirror of torch_points3d/modules/multimodal/pooling.py on the sm_100a kernels.
+"""Drop-in mirror of torch_points3d/modules/multimodal/pooling.py on the sm_90a kernels.
 
 Same class names, constructor kwargs (unknown kwargs are swallowed: the model factory always
 injects `index`, unet.py:633-636), `forward(x_main, x_mod, x_map, csr_idx)` signatures,

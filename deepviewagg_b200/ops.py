@@ -1,7 +1,7 @@
 """Autograd operators over the C ABI (include/dva_b200.h).
 
 Each function mirrors one operator of the reference's multimodal path (same argument meaning,
-same empty-segment / tie / eps semantics) and is backed ONLY by the sm_100a kernels of
+same empty-segment / tie / eps semantics) and is backed ONLY by the sm_90a kernels of
 libdva_b200.so: CPU tensors or a missing library raise.  Reference citations are relative to the
 reference repository root.
 """
@@ -647,7 +647,7 @@ def batch_norm_act(z, bn, negative_slope=1.0):
 
 
 # --------------------------------------------------------------------------------------------
-# dense projection of the MLP layers on tcgen05 tensor cores (base_modules.py:42)
+# dense projection of the MLP layers on wgmma tensor cores (base_modules.py:42)
 # --------------------------------------------------------------------------------------------
 _GEMM_PRECISION = {"mode": 0}
 
@@ -681,7 +681,7 @@ def _tc_gemm(a, b, layout, n_out):
 
 def tc_gemm_supported(x, weight):
     """True for 2-D CUDA floating-point inputs with at least one row: every such projection runs on
-    this library's kernels (K, N <= 64: skinny kernels, any K / N; otherwise the tcgen05 kernels, whose
+    this library's kernels (K, N <= 64: skinny kernels, any K / N; otherwise the wgmma kernels, whose
     16-byte TMA rows need K and N to be multiples of 4 -- other widths are zero-padded by `linear`)."""
     return bool(x.is_cuda and weight.is_cuda and x.dim() == 2 and x.shape[0] > 0
                 and x.is_floating_point() and weight.is_floating_point())
@@ -828,15 +828,15 @@ class _MLPLayer(torch.autograd.Function):
         return dx, (dw.to(wdt) if ctx.needs_input_grad[1] else None), gw, gb, None, None, None, None, None
 
 
-# The fused backward (3xTF32 on mma.sync) takes 0.106 ms in a step at 1.28 M x 32 x 32 (HBM time: 0.100) against
-# 0.26 - 0.34 ms for the three kernels it replaces, but is no faster than them at K = 64 (0.33 against 0.29 ms),
-# where dX rides the tcgen05 kernel -> layers with K <= 32 only.
+# The fused backward (3xTF32 on mma.sync) replaces three kernels with one pass; at K = 64 it needs 2 CTAs per SM of
+# registers / shared memory and the unfused chain (dX on the wgmma kernel) is used -> layers with K <= 32 only.
+# This cut-off was chosen on another GPU and is not re-measured on the H100 (tools/bench_layer.py measures it).
 _MLP_LAYER_FUSED = {"on": os.environ.get("DVA_MLP_LAYER_FUSED", "1") != "0", "max_k": 32}
 
 
 def linear_bn_act(x, weight, bn, negative_slope=1.0):
     """act(BatchNorm1d(x @ weight.T)): one MLP layer of the pools (base_modules.py:38-48).  In training,
-    when the layer is wide enough for the tcgen05 kernel and has at most 128 output channels, the batch
+    when the layer is wide enough for the wgmma kernel and has at most 128 output channels, the batch
     statistics come out of the GEMM epilogue (2 passes over the activations instead of 3); otherwise
     linear() followed by batch_norm_act()."""
     lib = _lib.load()

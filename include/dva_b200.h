@@ -1,5 +1,5 @@
 /*
- * dva_b200.h -- C ABI of libdva_b200.so: the B200 (sm_100a) multi-view aggregation hot path.
+ * dva_b200.h -- C ABI of libdva_b200.so: the H100 (sm_90a) multi-view aggregation hot path.
  *
  * Every entry point replaces one operator (or a fused chain of operators) on the reference's
  * path  ImageMapping gather -> per-point ragged attention over views -> softmax-weighted reduce
@@ -214,7 +214,7 @@ int dva_neighborhood_features(const float* xyz, const int64_t* neighbors, int km
                               int64_t V, void* stream);
 
 /* ------------------------------------------------------------------------------------------
- * P9  dense projection GEMM of an MLP layer (tcgen05 / TMA / TMEM)
+ * P9  dense projection GEMM of an MLP layer (wgmma / TMA / mbarrier)
  *   replaces the nn.Linear(bias=False) of base_modules.py:42 in every pool MLP.
  *   layout 0: D[M,N] = A[M,K] . B[N,K]^T   (forward,  B = weight [out,in])
  *   layout 1: D[M,N] = A[M,K] . B[K,N]     (backward, dX = dZ . weight)
@@ -224,8 +224,8 @@ int dva_neighborhood_features(const float* xyz, const int64_t* neighbors, int km
  *       kernels -- weights in shared memory, 128-row tiles double-buffered by cp.async, coalesced
  *       16-byte global traffic, 3xTF32 split operands on mma.sync (fp32-grade accuracy, ~1e-6), dW
  *       as per-CTA partials reduced in a fixed order (deterministic);
- *     otherwise the hand-written tcgen05 kernels of csrc/tc_gemm.cu (TMA-fed tcgen05.mma kind::tf32,
- *       TMEM accumulators, 3xTF32 split operands: ~1e-6 of the result's max against fp64; dW as
+ *     otherwise the hand-written wgmma kernels of csrc/tc_gemm.cu (TMA-fed wgmma.mma_async tf32,
+ *       register accumulators, 3xTF32 split operands: ~1e-6 of the result's max against fp64; dW as
  *       per-CTA partial tiles reduced in a fixed order): operands 16-byte aligned, N % 4 == 0 and
  *       K % 4 == 0 (else DVA_EUNSUPPORTED; ops.linear zero-pads such widths).
  *   `precision` is accepted for ABI stability (0 or 1) and ignored: every path is fp32-grade.
@@ -239,12 +239,12 @@ int dva_linear_gemm(const float* A, const float* B, float* D, int64_t M, int64_t
  * P9  Linear with the BatchNorm batch statistics taken in the GEMM epilogue
  *   replaces base_modules.py:42-44 (nn.Linear(bias=False) followed by the statistics half of
  *   FastBatchNorm1d) for the wide layers (E_mod, E_mix, E_main): D[M,n_out] = X[M,k_red] . W[n_out,k_red]^T
- *   by the tcgen05 rows kernel, whose epilogue threads each own one output column and accumulate its
- *   shifted sum / sum of squares while storing; a one-warp-per-column kernel combines the per-CTA
+ *   by the wgmma rows kernel, whose epilogue accumulates each column's shifted sum / sum of squares
+ *   from the accumulator registers while storing (fp64 per CTA in shared memory); a one-warp-per-column kernel combines the per-CTA
  *   partials in fp64 (fixed order) into mean / invstd [n_out] (biased variance) and updates the running
  *   buffers (momentum, unbiased variance) like nn.BatchNorm1d.  The apply half is dva_bn_act_fwd with
  *   training = 0 on these mean / invstd.  supported(): 32 <= n_out <= 128, n_out % 4 == 0, k_red >= 8,
- *   k_red % 4 == 0 (the shapes dva_linear_gemm serves with the tcgen05 rows kernel; with DVA_TC_NARROW=0 in the
+ *   k_red % 4 == 0 (the shapes dva_linear_gemm serves with the wgmma rows kernel; with DVA_TC_NARROW=0 in the
  *   environment only n_out > 32 and k_red > 32, the round-1 routing); else DVA_EUNSUPPORTED.
  * ------------------------------------------------------------------------------------------ */
 int dva_linear_bnstats_supported(int64_t M, int64_t n_out, int64_t k_red);

@@ -1,4 +1,4 @@
-"""GPU parity: the sm_100a kernels (through the C ABI) vs the oracle and vs the committed
+"""GPU parity: the sm_90a kernels (through the C ABI) vs the oracle and vs the committed
 fixtures of the executed reference.  Tolerances: floats <= 1e-4 relative (north_star), integer
 outputs bit-exact.  bf16/fp16 storage is compared against the fp32 oracle at the storage type's
 own precision and reported separately."""
@@ -490,7 +490,7 @@ def test_bn_act_vs_torch(R, C):
 
 
 # ------------------------------------------------------------------------------------------------
-# tcgen05 projection GEMM vs an fp64 matmul
+# wgmma projection GEMM vs an fp64 matmul
 # ------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("M,K,N", [(4096, 128, 128), (1000, 64, 64), (37, 8, 32), (50000, 128, 64), (3000, 512, 512),
                                    (129, 32, 4), (1, 16, 16),

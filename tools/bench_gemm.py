@@ -36,11 +36,11 @@ for (M, K, N) in SHAPES:
     torch.backends.cuda.matmul.allow_tf32 = False
     for mode in ("fp32", "tf32"):
         ops.set_gemm_precision(mode)
-        res[f"dva tcgen05 {mode}"] = (timeit(lambda: ops._tc_gemm(x, w, 0, N)), ops._tc_gemm(x[:4096].contiguous(), w, 0, N).double())
-        res[f"dva tcgen05 dX {mode}"] = (timeit(lambda: ops._tc_gemm(g, w, 1, K)), None)
-        res[f"dva tcgen05 dW {mode}"] = (timeit(lambda: ops._tc_gemm(g, x, 2, K)), None)
+        res[f"dva wgmma {mode}"] = (timeit(lambda: ops._tc_gemm(x, w, 0, N)), ops._tc_gemm(x[:4096].contiguous(), w, 0, N).double())
+        res[f"dva wgmma dX {mode}"] = (timeit(lambda: ops._tc_gemm(g, w, 1, K)), None)
+        res[f"dva wgmma dW {mode}"] = (timeit(lambda: ops._tc_gemm(g, x, 2, K)), None)
     ops.set_gemm_precision("fp32")
-    print(f"M={M} K={K} N={N}: {flops / 1e12:.2f} TFLOP, {byts / 1e9:.1f} GB (HBM floor {byts / 6561.6e9 * 1e3:.2f} ms)")
+    print(f"M={M} K={K} N={N}: {flops / 1e12:.2f} TFLOP, {byts / 1e9:.1f} GB (HBM floor {byts / 3350e9 * 1e3:.2f} ms)")
     for k, (ms, out) in res.items():
         err = "" if out is None else f" relerr {float((out - ref).abs().max() / ref.abs().max()):.1e}"
         print(f"   {k:22s} {ms:8.3f} ms  {flops / ms / 1e9:8.1f} TFLOP/s {byts / ms / 1e6:8.0f} GB/s{err}")

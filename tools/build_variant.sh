@@ -12,7 +12,7 @@ OUT=$ROOT/build_variants; mkdir -p $OUT/obj_$NAME
 OBJS=""
 for f in $FILES; do
   o=$OUT/obj_$NAME/${f%.cu}.o
-  nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -lineinfo -Xcompiler -fPIC --expt-relaxed-constexpr $DEFS -c $CS/$f -o $o
+  nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -lineinfo -Xcompiler -fPIC --expt-relaxed-constexpr $DEFS -c $CS/$f -o $o
   OBJS="$OBJS $o"
 done
 STOCK=""
@@ -21,5 +21,5 @@ for o in $CS/build/*.o; do
   for f in $FILES; do [ "$b" == "${f%.cu}.o" ] && skip=1; done
   [ $skip == 0 ] && STOCK="$STOCK $o"
 done
-nvcc -gencode arch=compute_100a,code=sm_100a -shared -o $OUT/libdva_$NAME.so $OBJS $STOCK -lcudart
+nvcc -gencode arch=compute_90a,code=sm_90a -shared -o $OUT/libdva_$NAME.so $OBJS $STOCK -lcudart
 echo built $OUT/libdva_$NAME.so
