@@ -51,6 +51,12 @@ SIGNATURES = {
                                    _i64, _i64, _i64, _i64, _i32, _i32, _vp]),
     "dva_interp_pool_bwd": (_i32, [_vp, _i32, _vp, _vp, _i32, _vp, _vp, _vp, _i64, _i64, _i64, _i64,
                                    _i64, _i64, _i64, _i64, _i32, _i32, _vp]),
+    "dva_gather_pool_bwd_det_workspace_bytes": (_sz, [_i64, _i64, _i64, _i64]),
+    "dva_gather_pool_bwd_det": (_i32, [_vp, _i32, _vp, _vp, _i32, _vp, _vp, _vp, _i64, _i64, _i64, _i64,
+                                       _i64, _i64, _i32, _i32, _vp, _sz, _vp]),
+    "dva_interp_pool_bwd_det_workspace_bytes": (_sz, [_i64, _i64, _i64, _i64]),
+    "dva_interp_pool_bwd_det": (_i32, [_vp, _i32, _vp, _vp, _i32, _vp, _vp, _vp, _i64, _i64, _i64, _i64,
+                                       _i64, _i64, _i64, _i64, _i32, _i32, _vp, _sz, _vp]),
     "dva_transpose_last2": (_i32, [_vp, _vp, _i64, _i64, _i64, _i32, _vp]),
     "dva_knn_cell_ids": (_i32, [_vp, _vp, _i64, _f32, _f32, _f32, _f32, _i32, _i32, _i32, _vp]),
     "dva_knn_grid": (_i32, [_vp, _vp, _vp, _vp, _i64, _i32, _f32, _f32, _f32, _f32, _i32, _i32, _i32,
@@ -58,6 +64,8 @@ SIGNATURES = {
     "dva_neighborhood_features": (_i32, [_vp, _vp, _i32, _vp, _vp, _vp, _vp, _i32, _f64, _i32, _i32, _vp,
                                          _i64, _i64, _vp]),
     "dva_scatter_add_rows": (_i32, [_vp, _vp, _vp, _i64, _i64, _i64, _i32, _vp]),
+    "dva_scatter_add_rows_det_workspace_bytes": (_sz, [_i64, _i64]),
+    "dva_scatter_add_rows_det": (_i32, [_vp, _vp, _vp, _i64, _i64, _i64, _i32, _vp, _sz, _vp]),
     "dva_mapping_build_workspace_bytes": (_sz, [_i64, _i64]),
     "dva_mapping_build": (_i32, [_vp, _vp, _vp, _i32, _vp, _vp, _vp, _i64, _i64, _i64, _i32, _vp, _vp, _vp, _vp, _vp, _vp,
                                  _vp, _vp, _sz, _vp]),

@@ -13,7 +13,7 @@
 // the feature map is smaller, and every pixel reads 4 bilinear corners of the replicate-padded
 // map.  The fp32 arithmetic follows the reference operation by operation (no FMA contraction),
 // so corner choices, values and therefore max / argmax decisions are identical in fp32.
-#include "dva_common.cuh"
+#include "bucket_sort.cuh"
 
 namespace dva {
 
@@ -513,6 +513,306 @@ extern "C" int dva_interp_pool_bwd(const void* grad_out, int channels_last, cons
                                    int64_t P, int reduce, int dtype, void* stream) {
   return gather_pool_bwd_impl<true>("interp_pool_bwd", grad_out, channels_last, img, pix, pix_is_i16,
                                     aptr, arg, grad_fmap, B, C, H, W, map_w, map_h, Vw, P, reduce, dtype, stream);
+}
+
+// ---------------------------------------------------------------------------------------------
+// Deterministic backward (used under torch.use_deterministic_algorithms): instead of scattering
+// every contribution with fp32 atomics, the contributions are bucketed by map pixel and every map
+// element is summed by one owner in a fixed order.  For element (b, y, x, c):
+//   contributions (p, k): pixel slot p (atomic-CSR order) of view w; k = 0 for the plain gather,
+//     k = 0..3 = corners w00, w01, w10, w11 of bilin_setup for the bilinear path (two corners of one
+//     slot clamped onto the same pixel are two contributions); taken in ascending (p, k);
+//   value: g = float(grad_out[w, c]); mean: __fdiv_rn(g, n_w); max / min: only when n_w == 1 or
+//     arg[w, c] == p; bilinear: __fmul_rn(w_k, value);
+//   sum: acc = +0.0f, acc = __fadd_rn(acc, value) (explicit _rn: no FMA contraction).
+// Index: counting sort of the contribution ids p * K + k by pixel key (b * H + y) * W + x
+// (bucket_sort.cuh: histogram, scan, scatter, per-bucket rank sort), then one pass that stores the
+// view and bilinear weight beside every ordered entry.  The reducers write every element of the map
+// gradient, zeros included.  The result is a pure function of the inputs.
+// ---------------------------------------------------------------------------------------------
+namespace dva {
+namespace det {
+
+// view of every pixel slot (-1: in no view); one warp per view
+__global__ void __launch_bounds__(256)
+slot_views_kernel(const int64_t* __restrict__ aptr, int64_t Vw, int64_t P, int64_t* __restrict__ view_of) {
+  const int lane = threadIdx.x & 31;
+  const int64_t warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+  for (int64_t w = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; w < Vw; w += warps) {
+    const int64_t p0 = max(aptr[w], (int64_t)0), p1 = min(aptr[w + 1], P);
+    for (int64_t p = p0 + lane; p < p1; p += 32) view_of[p] = w;
+  }
+}
+
+// bucket keys of slot p: the map pixel of each of its K contributions (clamped like the forward)
+template <typename PIX, bool INTERP>
+struct PixelKey {
+  const int64_t* view_of; const int64_t* img; const PIX* pix; int64_t B; int H, W; float mw1, mh1;
+  __device__ __forceinline__ void operator()(int64_t p, int64_t (&k)[INTERP ? 4 : 1]) const {
+    const int64_t w = view_of[p];
+    if (w < 0) {
+#pragma unroll
+      for (int j = 0; j < (INTERP ? 4 : 1); ++j) k[j] = -1;
+      return;
+    }
+    const int64_t row0 = clamp_img(img[w], B) * H;
+    const int px = (int)pix[2 * p], py = (int)pix[2 * p + 1];
+    if constexpr (INTERP) {
+      const Bilin q = bilin_setup(px, py, H, W, mw1, mh1);
+      k[0] = (row0 + q.r0) * W + q.c0; k[1] = (row0 + q.r0) * W + q.c1;
+      k[2] = (row0 + q.r1) * W + q.c0; k[3] = (row0 + q.r1) * W + q.c1;
+    } else {
+      k[0] = (row0 + clamp_px(py, H)) * W + clamp_px(px, W);
+    }
+  }
+};
+
+// what the reducers need of an ordered entry: its view and (bilinear) corner weight
+struct Ent { int32_t w; float wt; };
+
+template <typename PIX, bool INTERP>
+__global__ void __launch_bounds__(256)
+describe_entries(const int64_t* __restrict__ sorted, const int64_t* __restrict__ n_entries, int64_t bound,
+                 const int64_t* __restrict__ view_of, const PIX* __restrict__ pix, int H, int W, float mw1,
+                 float mh1, Ent* __restrict__ ent) {
+  const int64_t n = min(*n_entries, bound);
+  for (int64_t e = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; e < n; e += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t cid = sorted[e];
+    const int64_t p = INTERP ? (cid >> 2) : cid;
+    Ent d;
+    d.w = (int32_t)view_of[p];
+    d.wt = 1.f;
+    if constexpr (INTERP) {
+      const Bilin q = bilin_setup((int)pix[2 * p], (int)pix[2 * p + 1], H, W, mw1, mh1);
+      const int k = (int)(cid & 3);
+      d.wt = k == 0 ? q.w00 : (k == 1 ? q.w01 : (k == 2 ? q.w10 : q.w11));
+    }
+    ent[e] = d;
+  }
+}
+
+template <int RED, bool INTERP>
+__device__ __forceinline__ float contrib(float g, int n, float wt) {
+  if (RED == DVA_MEAN) g = __fdiv_rn(g, (float)n);
+  if (INTERP) g = __fmul_rn(wt, g);
+  return g;
+}
+
+// channels-last, whole 16-byte chunks: LPR lanes own the chunks of one map pixel (the sub-warp shape of
+// gather_pool_bwd_cl_kernel), walk its entries in order and gather the grad_out rows of their views
+template <typename T, int LPR, int RED, bool INTERP>
+__global__ void __launch_bounds__(kGpWarps * 32)
+gather_pool_bwd_det_cl_kernel(const T* __restrict__ gout, const int64_t* __restrict__ aptr,
+                              const int64_t* __restrict__ arg, const int64_t* __restrict__ off,
+                              const int64_t* __restrict__ sorted, const Ent* __restrict__ ent,
+                              float* __restrict__ gfmap, int C, int64_t NB) {
+  constexpr int VEC = Vec16<T>::N, RPI = 32 / LPR;
+  const int lane = threadIdx.x & 31, sg = lane / LPR, lir = lane % LPR;
+  const int cv = C / VEC, tiles = (cv + LPR - 1) / LPR;
+  const int64_t items = NB * tiles;
+  const int64_t stride = (int64_t)gridDim.x * kGpWarps * RPI;
+  for (int64_t item = ((int64_t)blockIdx.x * kGpWarps + (threadIdx.x >> 5)) * RPI + sg; item < items; item += stride) {
+    const int64_t q = tiles == 1 ? item : item / tiles;
+    const int ck = (int)(item - q * tiles) * LPR + lir;
+    if (ck >= cv) continue;
+    const int64_t e1 = off[q + 1];
+    float acc[VEC];
+#pragma unroll
+    for (int j = 0; j < VEC; ++j) acc[j] = 0.f;
+    for (int64_t e = off[q]; e < e1; ++e) {
+      const Ent d = ent[e];
+      const int64_t w = d.w;
+      const int n = RED == DVA_SUM ? 1 : (int)(aptr[w + 1] - aptr[w]);
+      float g[VEC];
+      unpack16<T, VEC>(__ldg(reinterpret_cast<const uint4*>(gout + w * C + (int64_t)ck * VEC)), g);
+      bool on[VEC];
+#pragma unroll
+      for (int j = 0; j < VEC; ++j) on[j] = true;
+      if ((RED == DVA_MAX || RED == DVA_MIN) && n >= 2) {
+        const int64_t p = INTERP ? (sorted[e] >> 2) : sorted[e];
+        const int64_t* a = arg + w * C + (int64_t)ck * VEC;
+#pragma unroll
+        for (int j = 0; j < VEC; ++j) on[j] = a[j] == p;
+      }
+#pragma unroll
+      for (int j = 0; j < VEC; ++j)
+        if (on[j]) acc[j] = __fadd_rn(acc[j], contrib<RED, INTERP>(g[j], n, d.wt));
+    }
+    float4* o = reinterpret_cast<float4*>(gfmap + q * C + (int64_t)ck * VEC);
+#pragma unroll
+    for (int j = 0; j < VEC; j += 4) o[j / 4] = make_float4(acc[j], acc[j + 1], acc[j + 2], acc[j + 3]);
+  }
+}
+
+// one thread per map-gradient element: NCHW maps and channels-last rows that are not whole 16-byte chunks
+template <typename T, bool CL, int RED, bool INTERP>
+__global__ void __launch_bounds__(256)
+gather_pool_bwd_det_kernel(const T* __restrict__ gout, const int64_t* __restrict__ aptr,
+                           const int64_t* __restrict__ arg, const int64_t* __restrict__ off,
+                           const int64_t* __restrict__ sorted, const Ent* __restrict__ ent,
+                           float* __restrict__ gfmap, int64_t C, int64_t HW, int64_t total) {
+  for (int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; t < total; t += (int64_t)gridDim.x * blockDim.x) {
+    int64_t q, c;
+    if (CL) {
+      q = t / C; c = t - q * C;
+    } else {                                      // t = (b * C + c) * HW + s  ->  q = b * HW + s
+      const int64_t bc = t / HW, s = t - bc * HW, b = bc / C;
+      c = bc - b * C; q = b * HW + s;
+    }
+    const int64_t e1 = off[q + 1];
+    float acc = 0.f;
+    for (int64_t e = off[q]; e < e1; ++e) {
+      const Ent d = ent[e];
+      const int64_t w = d.w;
+      const int n = RED == DVA_SUM ? 1 : (int)(aptr[w + 1] - aptr[w]);
+      if ((RED == DVA_MAX || RED == DVA_MIN) && n >= 2 && arg[w * C + c] != (INTERP ? (sorted[e] >> 2) : sorted[e]))
+        continue;
+      acc = __fadd_rn(acc, contrib<RED, INTERP>(Cvt<T>::to_f(gout[w * C + c]), n, d.wt));
+    }
+    gfmap[t] = acc;
+  }
+}
+
+struct Workspace {
+  int64_t* view_of;
+  Ent* ent;
+  bk::BucketIndex idx;
+};
+
+static size_t carve(uint8_t* base, int64_t P, int64_t n_entries, int64_t NB, Workspace* w) {
+  size_t o = 0;
+  auto take = [&](size_t bytes) { uint8_t* p = base ? base + o : nullptr; o += bk::align256(bytes); return p; };
+  uint8_t* p;
+  p = take((size_t)(P + 1) * 8); if (w) w->view_of = (int64_t*)p;
+  p = take((size_t)(n_entries + 1) * sizeof(Ent)); if (w) w->ent = (Ent*)p;
+  o += bk::carve_index(base ? base + o : nullptr, n_entries, NB, w ? &w->idx : nullptr);
+  return o;
+}
+
+static size_t workspace_bytes(int64_t B, int64_t H, int64_t W, int64_t P, int K) {
+  if (B < 0 || H < 0 || W < 0 || P < 0) return 0;
+  return carve(nullptr, P, P * K, B * H * W, nullptr) + 256;
+}
+
+template <typename T, typename PIX, bool CL, bool INTERP>
+static int gp_bwd_det(const void* gout, const int64_t* img, const void* pix, const int64_t* aptr,
+                      const int64_t* arg, float* gfmap, int64_t B, int64_t C, int64_t H, int64_t W,
+                      int64_t Vw, int64_t P, float mw1, float mh1, int reduce, void* workspace,
+                      cudaStream_t st) {
+  constexpr int K = INTERP ? 4 : 1;
+  const int64_t NB = B * H * W;
+  Workspace ws;
+  uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(workspace) + 255) & ~(uintptr_t)255);
+  carve(base, P, P * K, NB, &ws);
+  cudaError_t e = cudaMemsetAsync(ws.view_of, 0xff, (size_t)P * 8, st);           // -1: slot in no view
+  if (e != cudaSuccess) return fail((int)e, "gather_pool_bwd_det: memset failed");
+  slot_views_kernel<<<bk::grid_for(Vw * 32), 256, 0, st>>>(aptr, Vw, P, ws.view_of);
+  int rc = check_launch("gp_det_slot_views");
+  if (rc) return rc;
+  const PixelKey<PIX, INTERP> key{ws.view_of, img, (const PIX*)pix, B, (int)H, (int)W, mw1, mh1};
+  if ((rc = bk::build_index<K>(key, P, NB, ws.idx, st))) return rc;
+  describe_entries<PIX, INTERP><<<bk::grid_for(P * K), 256, 0, st>>>(ws.idx.sorted, ws.idx.off + NB, P * K, ws.view_of,
+                                                                      (const PIX*)pix, (int)H, (int)W, mw1, mh1, ws.ent);
+  if ((rc = check_launch("gp_det_describe_entries"))) return rc;
+  const T* g = (const T*)gout;
+  if constexpr (CL) {
+    if (gp_cl_vec_ok<T>(gfmap, gout, C, H, W) && C % 4 == 0) {
+      const int lpr = gp_cl_lpr<T>(C);
+      const int64_t cvv = C / Vec16<T>::N;
+      const int64_t items = NB * ((cvv + lpr - 1) / lpr);
+      const int gridv = gp_cl_grid(items, 32 / lpr, 1);
+#define GD_BV(R, L) gather_pool_bwd_det_cl_kernel<T, L, R, INTERP><<<gridv, kGpWarps * 32, 0, st>>>(g, aptr, arg, ws.idx.off, ws.idx.sorted, ws.ent, gfmap, (int)C, NB)
+#define GD_BVL(R) do { if (lpr == 4) GD_BV(R, 4); else if (lpr == 8) GD_BV(R, 8); else if (lpr == 16) GD_BV(R, 16); else GD_BV(R, 32); } while (0)
+      switch (reduce) {
+        case DVA_SUM: GD_BVL(DVA_SUM); break;
+        case DVA_MEAN: GD_BVL(DVA_MEAN); break;
+        case DVA_MAX: GD_BVL(DVA_MAX); break;
+        case DVA_MIN: GD_BVL(DVA_MIN); break;
+        default: return fail(DVA_EINVAL, "gather_pool_bwd_det: unknown reduce");
+      }
+#undef GD_BVL
+#undef GD_BV
+      return check_launch("gather_pool_bwd_det(cl)");
+    }
+  }
+  const int64_t total = NB * C;
+  const int grid = gp_grid(total);
+#define GD_B(R) gather_pool_bwd_det_kernel<T, CL, R, INTERP><<<grid, 256, 0, st>>>(g, aptr, arg, ws.idx.off, ws.idx.sorted, ws.ent, gfmap, C, H * W, total)
+  switch (reduce) {
+    case DVA_SUM: GD_B(DVA_SUM); break;
+    case DVA_MEAN: GD_B(DVA_MEAN); break;
+    case DVA_MAX: GD_B(DVA_MAX); break;
+    case DVA_MIN: GD_B(DVA_MIN); break;
+    default: return fail(DVA_EINVAL, "gather_pool_bwd_det: unknown reduce");
+  }
+#undef GD_B
+  return check_launch("gather_pool_bwd_det");
+}
+
+}  // namespace det
+}  // namespace dva
+
+template <bool INTERP>
+static int gather_pool_bwd_det_impl(const char* who, const void* grad_out, int channels_last,
+                                    const int64_t* img, const void* pix, int pix_is_i16,
+                                    const int64_t* aptr, const int64_t* arg, float* grad_fmap, int64_t B,
+                                    int64_t C, int64_t H, int64_t W, int64_t map_w, int64_t map_h,
+                                    int64_t Vw, int64_t P, int reduce, int dtype, void* workspace,
+                                    size_t workspace_bytes, void* stream) {
+  if (B < 0 || C < 0 || H < 0 || W < 0 || Vw < 0 || P < 0) return failf(DVA_EINVAL, "%s: negative size", who);
+  if (reduce < DVA_SUM || reduce > DVA_MIN) return failf(DVA_EINVAL, "%s: unknown reduce", who);
+  if (dtype < DVA_F32 || dtype > DVA_F16) return failf(DVA_EINVAL, "%s: unknown dtype", who);
+  const bool work = Vw > 0 && P > 0;
+  if (work && C > 0 && (B < 1 || H < 1 || W < 1)) return failf(DVA_EINVAL, "%s: pixels given but the map is empty", who);
+  if (B * C * H * W == 0) return DVA_OK;
+  if (!grad_fmap) return failf(DVA_EINVAL, "%s: null pointer", who);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (!work) {          // no contribution: the map gradient is all zeros
+    cudaError_t e = cudaMemsetAsync(grad_fmap, 0, (size_t)(B * C * H * W) * 4, st);
+    return e == cudaSuccess ? DVA_OK : failf((int)e, "%s: memset failed", who);
+  }
+  if (!aptr || !grad_out || !img || !pix || !workspace) return failf(DVA_EINVAL, "%s: null pointer", who);
+  if ((reduce == DVA_MAX || reduce == DVA_MIN) && !arg) return failf(DVA_EINVAL, "%s: max/min need arg", who);
+  if (INTERP && (map_w < 2 || map_h < 2 || H > (1 << 24) || W > (1 << 24)))
+    return failf(DVA_EINVAL, "%s: bad map / mapping size", who);
+  if (Vw >= (1ll << 31)) return failf(DVA_EUNSUPPORTED, "%s: more than 2^31 views", who);
+  if (workspace_bytes < det::workspace_bytes(B, H, W, P, INTERP ? 4 : 1))
+    return failf(DVA_EINVAL, "%s: workspace too small", who);
+  const float mw1 = (float)(map_w - 1), mh1 = (float)(map_h - 1);
+  switch (dtype) {
+    case DVA_F32: { using T = float; GP_DISPATCH(det::gp_bwd_det, INTERP, grad_out, img, pix, aptr, arg, grad_fmap, B, C, H, W, Vw, P, mw1, mh1, reduce, workspace, st); }
+    case DVA_BF16: { using T = __nv_bfloat16; GP_DISPATCH(det::gp_bwd_det, INTERP, grad_out, img, pix, aptr, arg, grad_fmap, B, C, H, W, Vw, P, mw1, mh1, reduce, workspace, st); }
+    default: { using T = __half; GP_DISPATCH(det::gp_bwd_det, INTERP, grad_out, img, pix, aptr, arg, grad_fmap, B, C, H, W, Vw, P, mw1, mh1, reduce, workspace, st); }
+  }
+}
+
+extern "C" size_t dva_gather_pool_bwd_det_workspace_bytes(int64_t B, int64_t H, int64_t W, int64_t P) {
+  return det::workspace_bytes(B, H, W, P, 1);
+}
+
+extern "C" int dva_gather_pool_bwd_det(const void* grad_out, int channels_last, const int64_t* img,
+                                       const void* pix, int pix_is_i16, const int64_t* aptr,
+                                       const int64_t* arg, float* grad_fmap, int64_t B, int64_t C,
+                                       int64_t H, int64_t W, int64_t Vw, int64_t P, int reduce,
+                                       int dtype, void* workspace, size_t workspace_bytes, void* stream) {
+  return gather_pool_bwd_det_impl<false>("gather_pool_bwd_det", grad_out, channels_last, img, pix, pix_is_i16,
+                                         aptr, arg, grad_fmap, B, C, H, W, 0, 0, Vw, P, reduce, dtype, workspace,
+                                         workspace_bytes, stream);
+}
+
+extern "C" size_t dva_interp_pool_bwd_det_workspace_bytes(int64_t B, int64_t H, int64_t W, int64_t P) {
+  return det::workspace_bytes(B, H, W, P, 4);
+}
+
+extern "C" int dva_interp_pool_bwd_det(const void* grad_out, int channels_last, const int64_t* img,
+                                       const void* pix, int pix_is_i16, const int64_t* aptr,
+                                       const int64_t* arg, float* grad_fmap, int64_t B, int64_t C,
+                                       int64_t H, int64_t W, int64_t map_w, int64_t map_h, int64_t Vw,
+                                       int64_t P, int reduce, int dtype, void* workspace,
+                                       size_t workspace_bytes, void* stream) {
+  return gather_pool_bwd_det_impl<true>("interp_pool_bwd_det", grad_out, channels_last, img, pix, pix_is_i16,
+                                        aptr, arg, grad_fmap, B, C, H, W, map_w, map_h, Vw, P, reduce, dtype,
+                                        workspace, workspace_bytes, stream);
 }
 
 // ---------------------------------------------------------------------------------------------

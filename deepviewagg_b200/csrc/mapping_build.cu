@@ -6,7 +6,7 @@
 // The reference composes these from lexargsort / lexargunique (composite int64 key -> full sort ->
 // unique), scatter_mean, repeat_interleave and cumsum, with several host synchronisations (.item(), max).
 //
-// Here: items are BUCKETED by point -- the point id is a dense integer in [0, num_points), so the top
+// Here: items are BUCKETED by point (csrc/bucket_sort.cuh) -- the point id is a dense integer in [0, num_points), so the top
 // level of the CSR is a counting sort (histogram + exclusive scan + scatter), not a comparison sort --
 // and each point's handful of items is then ordered by one warp with a rank sort on the key
 // (image, [x, y,] source index).  Runs of equal image inside a point are its views; their pixels follow
@@ -15,130 +15,22 @@
 // is the pair (V, P) of output sizes, written to a device word the caller reads once.
 //
 // HBM-bound integer work: per item ~6 passes of 8..24 bytes; no tensor cores.
-#include "dva_common.cuh"
+#include "bucket_sort.cuh"
 
 namespace dva {
 namespace mb {
 
-constexpr int kScanItems = 2048;          // elements per scan block (256 threads x 8)
-
-// ---- exclusive scan int32 -> int64 (three phases; sizes up to 2^31 blocks of 2048) -------------------
-__global__ void __launch_bounds__(256)
-scan_block_sums(const int32_t* __restrict__ in, int64_t n, int64_t* __restrict__ block_sums) {
-  __shared__ int64_t red[8];
-  const int64_t base = (int64_t)blockIdx.x * kScanItems;
-  int64_t s = 0;
-  for (int k = 0; k < 8; ++k) {
-    const int64_t i = base + k * 256 + threadIdx.x;
-    if (i < n) s += in[i];
-  }
-  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    int64_t t = 0;
-    for (int w = 0; w < 8; ++w) t += red[w];
-    block_sums[blockIdx.x] = t;
-  }
-}
-
-// single CTA: exclusive scan of the block sums in place; total -> sums[n_blocks]
-__global__ void __launch_bounds__(1024)
-scan_of_sums(int64_t* __restrict__ sums, int64_t n_blocks) {
-  __shared__ int64_t warp_tot[32];
-  __shared__ int64_t carry_s;
-  if (threadIdx.x == 0) carry_s = 0;
-  __syncthreads();
-  for (int64_t base = 0; base < n_blocks; base += 1024) {
-    const int64_t i = base + threadIdx.x;
-    const int64_t v = i < n_blocks ? sums[i] : 0;
-    int64_t inc = v;
-    for (int o = 1; o < 32; o <<= 1) {
-      const int64_t t = __shfl_up_sync(0xffffffffu, inc, o);
-      if ((threadIdx.x & 31) >= o) inc += t;
-    }
-    if ((threadIdx.x & 31) == 31) warp_tot[threadIdx.x >> 5] = inc;
-    __syncthreads();
-    if (threadIdx.x < 32) {
-      int64_t w = warp_tot[threadIdx.x], wi = w;
-      for (int o = 1; o < 32; o <<= 1) {
-        const int64_t t = __shfl_up_sync(0xffffffffu, wi, o);
-        if (threadIdx.x >= o) wi += t;
-      }
-      warp_tot[threadIdx.x] = wi - w;                  // exclusive prefix of the warp totals
-    }
-    __syncthreads();
-    const int64_t carry = carry_s;
-    if (i < n_blocks) sums[i] = carry + warp_tot[threadIdx.x >> 5] + inc - v;
-    __syncthreads();
-    if (threadIdx.x == 1023) carry_s = carry + warp_tot[31] + inc;
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) sums[n_blocks] = carry_s;
-}
-
-__global__ void __launch_bounds__(256)
-scan_apply(const int32_t* __restrict__ in, int64_t n, const int64_t* __restrict__ block_offsets,
-           int64_t* __restrict__ out /* [n + 1] */) {
-  __shared__ int64_t warp_tot[8];
-  const int64_t base = (int64_t)blockIdx.x * kScanItems + (int64_t)threadIdx.x * 8;
-  int32_t v[8];
-  int64_t s = 0;
-#pragma unroll
-  for (int k = 0; k < 8; ++k) { v[k] = (base + k < n) ? in[base + k] : 0; s += v[k]; }
-  int64_t inc = s;
-  for (int o = 1; o < 32; o <<= 1) {
-    const int64_t t = __shfl_up_sync(0xffffffffu, inc, o);
-    if ((threadIdx.x & 31) >= o) inc += t;
-  }
-  if ((threadIdx.x & 31) == 31) warp_tot[threadIdx.x >> 5] = inc;
-  __syncthreads();
-  int64_t pre = block_offsets[blockIdx.x] + inc - s;
-  for (int w = 0; w < (threadIdx.x >> 5); ++w) pre += warp_tot[w];
-#pragma unroll
-  for (int k = 0; k < 8; ++k) {
-    if (base + k < n) out[base + k] = pre;
-    pre += v[k];
-  }
-  if (blockIdx.x == gridDim.x - 1 && threadIdx.x == 0) out[n] = block_offsets[gridDim.x];
-}
-
-static int exclusive_scan(const int32_t* in, int64_t n, int64_t* out, int64_t* block_sums, cudaStream_t st) {
-  // out[0..n] = exclusive prefix sums of in[0..n), out[n] = total.  block_sums: ceil(n / 2048) + 1 words
-  if (n == 0) {
-    cudaError_t e = cudaMemsetAsync(out, 0, 8, st);
-    return e == cudaSuccess ? DVA_OK : fail((int)e, "scan: memset failed");
-  }
-  const int64_t nb = (n + kScanItems - 1) / kScanItems;
-  scan_block_sums<<<(unsigned)nb, 256, 0, st>>>(in, n, block_sums);
-  int rc = check_launch("scan_block_sums");
-  if (rc) return rc;
-  scan_of_sums<<<1, 1024, 0, st>>>(block_sums, nb);
-  if ((rc = check_launch("scan_of_sums"))) return rc;
-  scan_apply<<<(unsigned)nb, 256, 0, st>>>(in, n, block_sums, out);
-  return check_launch("scan_apply");
-}
-
-// ---- bucketing -----------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256)
-count_points(const int64_t* __restrict__ point, int64_t n, int64_t num_points, int32_t* __restrict__ cnt,
-             int32_t* __restrict__ status) {
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+// point id of an item as its bucket key; out-of-range ids set status bit 0 (reported to the host with the
+// sizes) and drop the item
+struct PointKey {
+  const int64_t* point; int64_t num_points; int32_t* status;
+  __device__ __forceinline__ void operator()(int64_t i, int64_t (&k)[1]) const {
     const int64_t p = point[i];
-    if (p < 0 || p >= num_points) { atomicOr(status, 1); continue; }     // reported to the host with the sizes
-    atomicAdd(cnt + p, 1);
+    const bool ok = p >= 0 && p < num_points;
+    if (!ok && status) atomicOr(status, 1);
+    k[0] = ok ? p : -1;
   }
-}
-
-__global__ void __launch_bounds__(256)
-scatter_items(const int64_t* __restrict__ point, int64_t n, int64_t num_points, const int64_t* __restrict__ off,
-              int32_t* __restrict__ cursor, int64_t* __restrict__ bucket) {
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
-    const int64_t p = point[i];
-    if (p < 0 || p >= num_points) continue;
-    bucket[off[p] + atomicAdd(cursor + p, 1)] = i;       // arbitrary order inside the bucket; ordered next
-  }
-}
+};
 
 template <typename PIX> struct PixIO;
 template <> struct PixIO<int16_t> { static __device__ __forceinline__ void ld(const void* p, int64_t i, int& x, int& y) { const short2 v = reinterpret_cast<const short2*>(p)[i]; x = v.x; y = v.y; }
@@ -149,8 +41,7 @@ template <> struct PixIO<int64_t> { static __device__ __forceinline__ void ld(co
                                     static __device__ __forceinline__ void st(void* p, int64_t i, int x, int y) { reinterpret_cast<longlong2*>(p)[i] = make_longlong2(x, y); } };
 
 // key of an item inside its point: (image, [x, y]) then the source index (stability)
-struct Key { int64_t a; int64_t src; };
-__device__ __forceinline__ bool key_less(const Key& u, const Key& v) { return u.a < v.a || (u.a == v.a && u.src < v.src); }
+using bk::Key;
 
 template <typename PIX>
 __device__ __forceinline__ Key make_key(const int64_t* image, const void* pix, int64_t src, bool by_pixel) {
@@ -174,23 +65,8 @@ order_points(const int64_t* __restrict__ image, const void* __restrict__ pix, co
     const int64_t b0 = off[p], L = off[p + 1] - b0;
     if (L == 0) { if (lane == 0) { n_views[p] = 0; n_pix[p] = 0; } continue; }
     // ---- rank sort (stable through the source index) ----
-    if (L <= 32) {
-      Key mine; mine.a = 0; mine.src = 0;
-      if (lane < L) mine = make_key<PIX>(image, pix, bucket[b0 + lane], dedupe != 0);
-      int rank = 0;
-      for (int j = 0; j < (int)L; ++j) {
-        Key o; o.a = __shfl_sync(0xffffffffu, mine.a, j); o.src = __shfl_sync(0xffffffffu, mine.src, j);
-        rank += key_less(o, mine) ? 1 : 0;
-      }
-      if (lane < L) sorted[b0 + rank] = mine.src;
-    } else {
-      for (int64_t i = lane; i < L; i += 32) {
-        const Key mine = make_key<PIX>(image, pix, bucket[b0 + i], dedupe != 0);
-        int64_t rank = 0;
-        for (int64_t j = 0; j < L; ++j) rank += key_less(make_key<PIX>(image, pix, bucket[b0 + j], dedupe != 0), mine) ? 1 : 0;
-        sorted[b0 + rank] = mine.src;
-      }
-    }
+    bk::warp_rank_sort(bucket, sorted, b0, L, lane,
+                       [&](int64_t s) { return make_key<PIX>(image, pix, s, dedupe != 0); });
     __syncwarp();
     // ---- flags and counts over the ordered bucket ----
     int nv = 0, np = 0;
@@ -304,11 +180,8 @@ view_cat_sorting_kernel(const int64_t* const* __restrict__ ptrs, const int64_t* 
   }
 }
 
-static inline int grid_for(int64_t total, int per_block = 256) {
-  int64_t blocks = (total + per_block - 1) / per_block;
-  const int64_t cap = (int64_t)kNumSMs * 16;
-  return (int)(blocks > cap ? cap : (blocks < 1 ? 1 : blocks));
-}
+using bk::grid_for;
+using bk::align256;
 
 struct Workspace {
   int32_t *cnt, *cursor, *n_views, *n_pix, *status;
@@ -316,12 +189,10 @@ struct Workspace {
   uint8_t* flags;
 };
 
-static size_t align256(size_t v) { return (v + 255) & ~(size_t)255; }
-
 static size_t carve(uint8_t* base, int64_t n, int64_t N, Workspace* w) {
   size_t o = 0;
   auto take = [&](size_t bytes) { uint8_t* p = base ? base + o : nullptr; o += align256(bytes); return p; };
-  const int64_t nb = (N + kScanItems - 1) / kScanItems + 2;
+  const int64_t nb = bk::scan_block_words(N);
   uint8_t* p;
   p = take((size_t)(N + 1) * 4); if (w) w->cnt = (int32_t*)p;
   p = take((size_t)(N + 1) * 4); if (w) w->cursor = (int32_t*)p;
@@ -370,12 +241,14 @@ extern "C" int dva_mapping_build(const int64_t* point_ids, const int64_t* image_
   if (e != cudaSuccess) return fail((int)e, "mapping_build: memset failed");
   int rc;
   if (n_items > 0) {
-    mb::count_points<<<mb::grid_for(n_items), 256, 0, st>>>(point_ids, n_items, num_points, w.cnt, w.status);
+    bk::count_keys<1><<<mb::grid_for(n_items), 256, 0, st>>>(mb::PointKey{point_ids, num_points, w.status}, n_items,
+                                                             num_points, w.cnt);
     if ((rc = check_launch("mb_count_points"))) return rc;
   }
-  if ((rc = mb::exclusive_scan(w.cnt, num_points, w.off, w.block_sums, st))) return rc;
+  if ((rc = bk::exclusive_scan(w.cnt, num_points, w.off, w.block_sums, st))) return rc;
   if (n_items > 0) {
-    mb::scatter_items<<<mb::grid_for(n_items), 256, 0, st>>>(point_ids, n_items, num_points, w.off, w.cursor, w.bucket);
+    bk::scatter_keys<1><<<mb::grid_for(n_items), 256, 0, st>>>(mb::PointKey{point_ids, num_points, nullptr}, n_items,
+                                                               num_points, w.off, w.cursor, w.bucket);
     if ((rc = check_launch("mb_scatter_items"))) return rc;
   }
   const int pgrid = mb::grid_for(num_points * 32);
@@ -385,8 +258,8 @@ extern "C" int dva_mapping_build(const int64_t* point_ids, const int64_t* image_
                                                           w.n_pix, num_points, dedupe_pixels)));
     if ((rc = check_launch("mb_order_points"))) return rc;
   }
-  if ((rc = mb::exclusive_scan(w.n_views, num_points, view_ptr, w.block_sums, st))) return rc;
-  if ((rc = mb::exclusive_scan(w.n_pix, num_points, w.pix_ptr, w.block_sums, st))) return rc;
+  if ((rc = bk::exclusive_scan(w.n_views, num_points, view_ptr, w.block_sums, st))) return rc;
+  if ((rc = bk::exclusive_scan(w.n_pix, num_points, w.pix_ptr, w.block_sums, st))) return rc;
   if (num_points > 0 && n_items > 0) {
     MB_PIX((mb::emit_points<PIX><<<pgrid, 256, 0, st>>>(image_ids, pixels, feat, feat_row, feat_on, (int)F, w.off, w.sorted,
                                                          w.flags, view_ptr, w.pix_ptr, num_points, images_out, atomic_ptr,

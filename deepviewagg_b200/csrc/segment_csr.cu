@@ -7,7 +7,7 @@
 // columns, so every row read/write is a coalesced 16-byte-per-lane access, and the reduction
 // order is the sequential order of torch_scatter's CPU kernel (deterministic, first arg-max).
 // These are HBM-bound streaming kernels: bytes = n_items*K*s (read) + n_seg*K*s (write).
-#include "dva_common.cuh"
+#include "bucket_sort.cuh"
 
 namespace dva {
 
@@ -309,6 +309,47 @@ scatter_add_rows_kernel(const T* __restrict__ src, const int64_t* __restrict__ i
   }
 }
 
+// ---- deterministic rows scatter-add (torch.use_deterministic_algorithms) ------------------------------
+// Same result as above up to the summation order, which is fixed here: the source rows are bucketed by
+// destination row (bucket_sort.cuh, stable: ascending v) and the threads of one row's chunks sum them in
+// that order, acc = __fadd_rn(acc, src[v]) from +0.0f.  Every row of dst is written (no pre-zeroing).
+struct RowKey {
+  const int64_t* idx; int64_t R;
+  __device__ __forceinline__ void operator()(int64_t v, int64_t (&k)[1]) const {
+    const int64_t r = idx[v];
+    k[0] = (r < 0 || r >= R) ? -1 : r;
+  }
+};
+
+template <typename T, int VEC>
+__global__ void __launch_bounds__(256)
+scatter_add_rows_det_kernel(const T* __restrict__ src, const int64_t* __restrict__ off,
+                            const int64_t* __restrict__ sorted, float* __restrict__ dst, int64_t R, int64_t C) {
+  const int64_t CV = C / VEC, total = R * CV;
+  for (int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; t < total; t += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t r = t / CV, cv = t - r * CV;
+    const int64_t e1 = off[r + 1];
+    float acc[VEC];
+#pragma unroll
+    for (int j = 0; j < VEC; ++j) acc[j] = 0.f;
+    for (int64_t e = off[r]; e < e1; ++e) {
+      const int64_t v = sorted[e];
+      float f[VEC];
+      if constexpr (VEC == 1) f[0] = Cvt<T>::to_f(src[v * C + cv]);
+      else unpack16<T, VEC>(__ldg(reinterpret_cast<const uint4*>(src + v * C + cv * VEC)), f);
+#pragma unroll
+      for (int j = 0; j < VEC; ++j) acc[j] = __fadd_rn(acc[j], f[j]);
+    }
+    if constexpr (VEC == 1) {
+      dst[r * C + cv] = acc[0];
+    } else {
+      float4* o = reinterpret_cast<float4*>(dst + r * C + cv * VEC);
+#pragma unroll
+      for (int j = 0; j < VEC; j += 4) o[j / 4] = make_float4(acc[j], acc[j + 1], acc[j + 2], acc[j + 3]);
+    }
+  }
+}
+
 // ---- host-side dispatch ---------------------------------------------------------------------
 static inline int grid_for(int64_t total, int threads = 256) {
   int64_t blocks = (total + threads - 1) / threads;
@@ -514,6 +555,47 @@ extern "C" int dva_scatter_add_rows(const void* src, const int64_t* idx, float* 
       scatter_add_rows_kernel<T, 1><<<grid_for(V * C), 256, 0, st>>>((const T*)src, idx, dst, V, R, C);
     }
     return check_launch("scatter_add_rows");
+  });
+  return DVA_OK;
+}
+
+static size_t scatter_rows_det_carve(uint8_t* base, int64_t V, int64_t R, bk::BucketIndex* w) {
+  return bk::carve_index(base, V, R, w);
+}
+
+extern "C" size_t dva_scatter_add_rows_det_workspace_bytes(int64_t V, int64_t R) {
+  if (V < 0 || R < 0) return 0;
+  return scatter_rows_det_carve(nullptr, V, R, nullptr) + 256;
+}
+
+extern "C" int dva_scatter_add_rows_det(const void* src, const int64_t* idx, float* dst, int64_t V, int64_t R,
+                                        int64_t C, int dtype, void* workspace, size_t workspace_bytes,
+                                        void* stream) {
+  if (V < 0 || R < 0 || C < 0) return fail(DVA_EINVAL, "scatter_add_rows_det: negative size");
+  if (dtype < DVA_F32 || dtype > DVA_F16) return fail(DVA_EINVAL, "scatter_add_rows_det: unknown dtype");
+  if (R == 0 || C == 0) return DVA_OK;
+  if (!dst) return fail(DVA_EINVAL, "scatter_add_rows_det: null pointer");
+  cudaStream_t st = (cudaStream_t)stream;
+  if (V == 0) {          // nothing scattered: all rows are zero
+    const cudaError_t e = cudaMemsetAsync(dst, 0, (size_t)(R * C) * 4, st);
+    return e == cudaSuccess ? DVA_OK : fail((int)e, "scatter_add_rows_det: memset failed");
+  }
+  if (!src || !idx || !workspace) return fail(DVA_EINVAL, "scatter_add_rows_det: null pointer");
+  if (workspace_bytes < dva_scatter_add_rows_det_workspace_bytes(V, R))
+    return fail(DVA_EINVAL, "scatter_add_rows_det: workspace too small");
+  bk::BucketIndex w;
+  uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(workspace) + 255) & ~(uintptr_t)255);
+  scatter_rows_det_carve(base, V, R, &w);
+  int rc = bk::build_index<1>(RowKey{idx, R}, V, R, w, st);
+  if (rc) return rc;
+  DVA_DISPATCH_DTYPE(dtype, {
+    constexpr int VEC = Vec16<T>::N;
+    if (C % VEC == 0 && aligned16(src) && aligned16(dst)) {
+      scatter_add_rows_det_kernel<T, VEC><<<grid_for(R * (C / VEC)), 256, 0, st>>>((const T*)src, w.off, w.sorted, dst, R, C);
+    } else {
+      scatter_add_rows_det_kernel<T, 1><<<grid_for(R * C), 256, 0, st>>>((const T*)src, w.off, w.sorted, dst, R, C);
+    }
+    return check_launch("scatter_add_rows_det");
   });
   return DVA_OK;
 }

@@ -228,10 +228,20 @@ def segment_softmax_csr(src, csr_idx, eps=1e-12, scaling=False):
 # fused view attention (modules.py:518 + pooling.py:285-300 / 515-530)
 # --------------------------------------------------------------------------------------------
 def _scatter_add_rows(src, idx, n_rows):
-    """fp32 [n_rows, C] with dst[idx[v]] += src[v] (dva_scatter_add_rows)."""
+    """fp32 [n_rows, C] with dst[idx[v]] += src[v] (dva_scatter_add_rows).  Under
+    torch.use_deterministic_algorithms(True): dva_scatter_add_rows_det (every row summed in ascending v)."""
     lib = _lib.load()
     src = src.contiguous()
     V, C = src.shape
+    if torch.are_deterministic_algorithms_enabled():
+        dst = torch.empty((n_rows, C), dtype=torch.float32, device=src.device)
+        ws_bytes = int(lib.dva_scatter_add_rows_det_workspace_bytes(V, n_rows))
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=src.device)
+        with torch.cuda.device(src.device):
+            check(lib.dva_scatter_add_rows_det(ptr(src), ptr(idx.contiguous()), ptr(dst), V, n_rows, C,
+                                               dtype_code(src), ptr(ws), ws_bytes, stream_ptr()),
+                  "dva_scatter_add_rows_det")
+        return dst
     dst = torch.zeros((n_rows, C), dtype=torch.float32, device=src.device)
     with torch.cuda.device(src.device):
         check(lib.dva_scatter_add_rows(ptr(src), ptr(idx.contiguous()), ptr(dst), V, n_rows, C, dtype_code(src),
@@ -511,16 +521,24 @@ class _GatherPool(torch.autograd.Function):
         B, C, H, W, Vw, P, code, cl, shape, dt, mapping_size, via_cl = ctx.cfg
         lib = _lib.load()
         grad_out = grad_out.contiguous()
-        gf = torch.zeros(shape, dtype=torch.float32, device=grad_out.device)
+        # torch.use_deterministic_algorithms(True): the map gradient is reduced per map pixel in a fixed
+        # order (the _det entry points write every element) instead of accumulated with fp32 atomics
+        det = torch.are_deterministic_algorithms_enabled()
+        gf = (torch.empty if det else torch.zeros)(shape, dtype=torch.float32, device=grad_out.device)
         head = (ptr(grad_out), int(cl), ptr(images), ptr(pixels), int(pixels.dtype == torch.int16),
                 ptr(atomic_ptr), ptr(arg), ptr(gf), B, C, H, W)
-        tail = (Vw, P, code, dtype_code(grad_out), stream_ptr())
+        tail = (Vw, P, code, dtype_code(grad_out))
+        msz = () if mapping_size is None else (int(mapping_size[0]), int(mapping_size[1]))
         with torch.cuda.device(grad_out.device):
-            if mapping_size is None:
-                check(lib.dva_gather_pool_bwd(*head, *tail), "dva_gather_pool_bwd")
+            if det:
+                name = "dva_gather_pool_bwd_det" if mapping_size is None else "dva_interp_pool_bwd_det"
+                ws_bytes = int(getattr(lib, name + "_workspace_bytes")(B, H, W, P))
+                ws = torch.empty(ws_bytes, dtype=torch.uint8, device=grad_out.device)
+                check(getattr(lib, name)(*head, *msz, *tail, ptr(ws), ws_bytes, stream_ptr()), name)
+            elif mapping_size is None:
+                check(lib.dva_gather_pool_bwd(*head, *tail, stream_ptr()), "dva_gather_pool_bwd")
             else:
-                check(lib.dva_interp_pool_bwd(*head, int(mapping_size[0]), int(mapping_size[1]), *tail),
-                      "dva_interp_pool_bwd")
+                check(lib.dva_interp_pool_bwd(*head, *msz, *tail, stream_ptr()), "dva_interp_pool_bwd")
         if via_cl:      # gradient of the NCHW input: transpose the channels-last map gradient back
             gf = _transpose_last2(gf, B, H * W, C).view(B, C, H, W)
         return gf.to(dt), None, None, None, None, None, None

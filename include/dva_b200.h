@@ -162,6 +162,22 @@ int dva_gather_pool_bwd(const void* grad_out, int channels_last, const int64_t* 
                         float* grad_fmap, int64_t B, int64_t C, int64_t H, int64_t W, int64_t Vw,
                         int64_t P, int reduce, int dtype, void* stream);
 
+/* Deterministic variant of dva_gather_pool_bwd          replaces the backward of image.py:1285
+ *   (x[feature_map_indexing]) + pooling.py:63 under torch.use_deterministic_algorithms(True).
+ *   grad_fmap is fully written (zeros included; no zero-initialisation needed).  Every element is the
+ *   fp32 sum, from +0.0f, with one round-to-nearest addition per contribution, of the contributions of
+ *   its map pixel in ascending pixel-slot order p: g = grad_out[w, c] of the slot's view w;
+ *   mean: g / n_w (rounded); max / min: only the slot with arg[w, c] == p (any slot when n_w == 1).
+ *   Out-of-range pixels and images are clamped as in the forward.  The result does not depend on
+ *   the launch configuration.  Needs fewer than 2^31 views.
+ *   workspace: dva_gather_pool_bwd_det_workspace_bytes(B, H, W, P) bytes (pixel-bucket index). */
+size_t dva_gather_pool_bwd_det_workspace_bytes(int64_t B, int64_t H, int64_t W, int64_t P);
+int dva_gather_pool_bwd_det(const void* grad_out, int channels_last, const int64_t* img,
+                            const void* pix, int pix_is_i16, const int64_t* aptr, const int64_t* arg,
+                            float* grad_fmap, int64_t B, int64_t C, int64_t H, int64_t W, int64_t Vw,
+                            int64_t P, int reduce, int dtype, void* workspace, size_t workspace_bytes,
+                            void* stream);
+
 /* [B,R,S] -> [B,S,R] layout change (dtype-sized elements), e.g. the reference's NCHW-contiguous
  * feature maps (image.py:1884 indexes them as x[b, :, y, x]) to channels-last and map gradients back,
  * so that dva_gather_pool_* / dva_interp_pool_* can run their 16-byte-chunk channels-last kernels. */
@@ -182,6 +198,19 @@ int dva_interp_pool_bwd(const void* grad_out, int channels_last, const int64_t* 
                         float* grad_fmap, int64_t B, int64_t C, int64_t H, int64_t W,
                         int64_t map_w, int64_t map_h, int64_t Vw, int64_t P, int reduce, int dtype,
                         void* stream);
+
+/* Deterministic variant of dva_interp_pool_bwd          replaces the backward of image.py:1278-1283
+ *   (sparse_interpolation, image.py:105-170) + pooling.py:63 under torch.use_deterministic_algorithms(True).
+ *   As dva_gather_pool_bwd_det with four contributions per slot, in the order (p, k), k = corners
+ *   top-left, top-right, bottom-left, bottom-right; a contribution is the rounded product of the
+ *   corner weight and the value above (two corners clamped onto one pixel stay two contributions).
+ *   workspace: dva_interp_pool_bwd_det_workspace_bytes(B, H, W, P) bytes. */
+size_t dva_interp_pool_bwd_det_workspace_bytes(int64_t B, int64_t H, int64_t W, int64_t P);
+int dva_interp_pool_bwd_det(const void* grad_out, int channels_last, const int64_t* img,
+                            const void* pix, int pix_is_i16, const int64_t* aptr, const int64_t* arg,
+                            float* grad_fmap, int64_t B, int64_t C, int64_t H, int64_t W,
+                            int64_t map_w, int64_t map_h, int64_t Vw, int64_t P, int reduce, int dtype,
+                            void* workspace, size_t workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * N1  neighbourhood-based mapping features (density, occlusion)
@@ -353,6 +382,13 @@ int dva_project_camera(const float* xyz, const float* cam, int camera, float* di
  * (pooling.py:146-150, "no view" = index V). */
 int dva_scatter_add_rows(const void* src, const int64_t* idx, float* dst, int64_t V, int64_t R, int64_t C,
                          int dtype, void* stream);
+/* Deterministic variant of dva_scatter_add_rows          replaces the same two backwards (modules.py:518,
+ *   pooling.py:146-150) under torch.use_deterministic_algorithms(True): dst [R, C] fp32 is fully written;
+ *   row r is the fp32 sum, from +0.0f in ascending v, of src[v] over the v with idx[v] == r.
+ *   workspace: dva_scatter_add_rows_det_workspace_bytes(V, R) bytes (row-bucket index). */
+size_t dva_scatter_add_rows_det_workspace_bytes(int64_t V, int64_t R);
+int dva_scatter_add_rows_det(const void* src, const int64_t* idx, float* dst, int64_t V, int64_t R, int64_t C,
+                             int dtype, void* workspace, size_t workspace_bytes, void* stream);
 
 /* I1 / I4 / I6  native construction of the point -> view -> pixel CSR (csrc/mapping_build.cu)
  *   replaces ImageMapping.from_dense image.py:1728-1795 (lexargsort + unique + cumsum chains) and the

@@ -12,6 +12,7 @@ Shapes follow the S3DIS batch of SURVEY.md Appendix E (4 x 40 k-point spheres, ~
 Everything goes through the public operators (deepviewagg_b200.ops / core.multimodal), i.e. the C ABI.
 """
 import argparse
+import contextlib
 import json
 import os
 import statistics
@@ -51,6 +52,21 @@ class Timer:
         return statistics.median(ts)
 
 
+@contextlib.contextmanager
+def deterministic():
+    """torch.use_deterministic_algorithms(True) without torch's NaN fill of torch.empty, so that a row
+    times the library's kernels rather than the fill."""
+    import torch.utils.deterministic as tud
+    prev, fill = torch.are_deterministic_algorithms_enabled(), tud.fill_uninitialized_memory
+    torch.use_deterministic_algorithms(True)
+    tud.fill_uninitialized_memory = False
+    try:
+        yield
+    finally:
+        torch.use_deterministic_algorithms(prev)
+        tud.fill_uninitialized_memory = fill
+
+
 def ragged_ptr(N, mean, dev, gen, p_empty=0.1):
     counts = torch.poisson(torch.full((N,), float(mean), device=dev), generator=gen).long()
     counts[torch.rand(N, device=dev, generator=gen) < p_empty] = 0
@@ -73,9 +89,13 @@ def main():
     peak = peak_gbs()
     only = set(filter(None, args.only.split(",")))
     lines = []
+    from bench import gpu_identity
+    ident = gpu_identity(0)            # read, not set: the card and power limit are part of every number
+    print(json.dumps({"gpu": ident}), flush=True)
 
     def emit(name, row, ms, bytes_=None, units=None, unit_name=None, note=""):
-        d = {"op": name, "survey_row": row, "ms": round(ms, 4)}
+        d = {"op": name, "survey_row": row, "ms": round(ms, 4), "gpu": ident["name"],
+             "power_limit_w": ident["power_limit_w"]}
         if bytes_ is not None:
             gbs = bytes_ / (ms * 1e-3) / 1e9
             d.update({"algorithmic_bytes": int(bytes_), "gbs": round(gbs, 1), "frac_of_hbm_peak": round(gbs / peak, 3)})
@@ -152,7 +172,38 @@ def main():
                  Pn * Cm * 4 * 3 + fm.numel() * 4 + Pn * (8 + 4 + 8 + 8),
                  note="grad_out read + read-modify-write of the touched map pixels + zero-fill of the "
                       "whole map gradient; fp32 reductions (16-byte red.v4 on the channels-last path)")
+            with deterministic():
+                emit(f"gather_pool_bwd_det_{tag}", "I5+P1",
+                     T(lambda: torch.autograd.grad(out, fr, go, retain_graph=True)),
+                     Pn * Cm * 4 + fm.numel() * 4 + Pn * (8 + 4 + 8 + 8),
+                     note="torch.use_deterministic_algorithms(True): pixel-bucket index (counting sort) + "
+                          "one ordered fp32 sum per map element, whole map gradient written once; "
+                          "fill_uninitialized_memory=False" + ("" if cl else "; NCHW: scalar reducer"))
             del fm, fr, out
+    if want("interp_pool"):
+        # reuse-heavy: a mapping at 4x the map resolution, ~3 pixels per view, 4 bilinear corners per pixel
+        B, Cm, H, W = 16, 64, 64, 128
+        msz = (4 * W, 4 * H)
+        Vn = 400_000
+        iptr = ragged_ptr(Vn, 3, dev, gen, p_empty=0.0)
+        Pn = int(iptr[-1])
+        images = torch.randint(0, B, (Vn,), device=dev, generator=gen)
+        pix = torch.stack([torch.randint(0, msz[0], (Pn,), device=dev, generator=gen),
+                           torch.randint(0, msz[1], (Pn,), device=dev, generator=gen)], 1).to(torch.int16)
+        fm = torch.randn((B, H, W, Cm), device=dev, generator=gen)
+        fr = fm.clone().requires_grad_(True)
+        out = ops.interp_pool(fr, images, pix, iptr, msz, reduce="max", channels_last=True)
+        go = torch.randn_like(out)
+        note = (f"{Pn} pixels at {msz[0]}x{msz[1]} -> {Vn} views (max) from [{B},{H},{W},{Cm}] maps, "
+                f"~{4 * Pn // (B * H * W)} contributions per map pixel")
+        emit("interp_pool_bwd_atomic_nhwc", "I5b+P1", T(lambda: torch.autograd.grad(out, fr, go, retain_graph=True)),
+             Vn * Cm * 4 + fm.numel() * 4 * 3 + Vn * Cm * 8, note=note + "; zero-fill + red.v4 into the map")
+        with deterministic():
+            emit("interp_pool_bwd_det_nhwc", "I5b+P1",
+                 T(lambda: torch.autograd.grad(out, fr, go, retain_graph=True)),
+                 Vn * Cm * 4 + fm.numel() * 4 + Vn * Cm * 8,
+                 note=note + "; deterministic: bucket index + ordered sums; fill_uninitialized_memory=False")
+        del fm, fr, out
 
     # ---- P9 BN + LeakyReLU ------------------------------------------------------------------------
     if want("bn_act"):
