@@ -17,13 +17,22 @@ from . import visibility as visibility_module
 from .image import ImageMapping, SameSettingImageData
 
 
+_METHODS = ('SplattingVisibility', 'DepthBasedVisibility', 'BiasuttiVisibility')
+
+
 class MapImages:
+    """`method` names the visibility model: 'SplattingVisibility' (z-buffer of splats),
+    'BiasuttiVisibility' (depth contrast among the k nearest projections) or
+    'DepthBasedVisibility' (agreement with a depth map: image i reads
+    `images.extras['depth_map'][i]`, a [W_proj, H_proj] float32 map in metres, -1 where empty,
+    e.g. from read_s3dis_depth_map)."""
+
     def __init__(self, method='SplattingVisibility', proj_upscale=None, ref_size=None, use_cuda=True,
                  verbose=False, cylinder=False, **kwargs):
         if not use_cuda:
             raise RuntimeError("deepviewagg_b200.MapImages runs on CUDA only (no CPU fallback)")
-        if method != 'SplattingVisibility':
-            raise NotImplementedError(f"visibility method '{method}' is out of scope (see DESIGN.md)")
+        if method not in _METHODS:
+            raise NotImplementedError(f"unknown visibility method '{method}', expected one of {_METHODS}")
         self.method, self.proj_upscale, self.ref_size = method, proj_upscale, ref_size
         self.verbose, self.cylinder, self.kwargs = verbose, cylinder, kwargs
 
@@ -49,9 +58,20 @@ class MapImages:
         ex = images.extras
         crop_off = images.crop_offsets if images.crop_offsets is not None else \
             torch.zeros((images.num_views, 2), dtype=torch.long)
+        if self.method == 'DepthBasedVisibility':
+            if 'depth_map' not in ex:
+                raise ValueError("MapImages(method='DepthBasedVisibility') needs images.extras['depth_map'], a "
+                                 "[B, W_proj, H_proj] float32 tensor of depth maps at the projection size "
+                                 "(read_s3dis_depth_map(path, img_size=...) reads an S3DIS depth PNG)")
+            dm = ex['depth_map']
+            if tuple(dm.shape) != (images.num_views,) + proj_size:
+                raise ValueError(f"images.extras['depth_map'] has shape {tuple(dm.shape)}, expected "
+                                 f"{(images.num_views,) + proj_size} (one [W_proj, H_proj] map per image)")
         image_ids, point_ids, features, pixels = [], [], [], []
         for i in range(images.num_views):
             kw = {}
+            if self.method == 'DepthBasedVisibility':
+                kw['depth_map'] = ex['depth_map'][i].to(dev, torch.float32)
             if images.opk is not None:
                 kw['img_opk'] = images.opk[i].float()
             if 'extrinsic' in ex:
@@ -110,9 +130,10 @@ def _grid_for(pos, cell_size):
 
 
 def knn_grid(pos, k, cell_size=None, return_dist2=False):
-    """Exact k nearest neighbours (self included) of every point among all points, on CUDA
-    (replaces the KeOps `argKmin` of image.py:504-514).  Squared distances are
-    (dx*dx + dy*dy) + dz*dz in fp32, ties ordered by point index.  Returns neighbors [N,k] int64
+    """Exact k nearest neighbours (self included, 1 <= k <= 128) of every point among all points,
+    on CUDA (replaces the KeOps `argKmin` of image.py:504-514 and visibility.py:1439-1444).
+    Squared distances are (dx*dx + dy*dy) + dz*dz in fp32, ties ordered by point index; points
+    with z = 0 give the exact 2D distance (image-plane search).  Returns neighbors [N,k] int64
     (ascending distance) and optionally the squared distances."""
     from ... import _lib
     from ..._lib import check, ptr, stream_ptr
@@ -122,8 +143,8 @@ def knn_grid(pos, k, cell_size=None, return_dist2=False):
     lib = _lib.load()
     pos = pos.float().contiguous()
     n = pos.shape[0]
-    if not 1 <= k <= 64:
-        raise ValueError("knn_grid: k must be in [1, 64]")
+    if not 1 <= k <= 128:
+        raise ValueError("knn_grid: k must be in [1, 128]")
     if n < k:
         raise ValueError(f"knn_grid: need at least k={k} points, got {n}")
     cell = torch.empty(n, dtype=torch.int64, device=pos.device)
@@ -138,9 +159,18 @@ def knn_grid(pos, k, cell_size=None, return_dist2=False):
     if cell_size is None:
         # start from a volume-uniform guess, then steer towards ~k/6 points per occupied cell
         # (scans are mostly surfaces: occupancy grows with the square of the cell size)
-        ext = (pos.max(dim=0).values - pos.min(dim=0).values).clamp_min(1e-6)
-        cell_size = float((ext.prod() * k / n) ** (1 / 3))
         target = max(2.0, k / 6)
+        ext = pos.max(dim=0).values - pos.min(dim=0).values
+        live = ext > 0
+        dims_live = int(live.sum())
+        if dims_live == 3:
+            cell_size = float((ext.clamp_min(1e-6).prod() * k / n) ** (1 / 3))
+        elif dims_live > 0:
+            # planar (image-plane, z = 0) or collinear set: uniform over the axes that have extent,
+            # ~target points per cell
+            cell_size = float((ext[live].clamp_min(1e-6).prod() * target / n) ** (1 / dims_live))
+        else:
+            cell_size = 1.0                                 # all points coincide: one cell
         for _ in range(3):
             lo, dims, cell_size = assign(cell_size)
             per_cell = n / max(1, int(torch.unique(cell).numel()))

@@ -7,11 +7,18 @@ bit-identical to the numba loops given the same projections.
   camera_projection          <- visibility.py:478-538, 592-623   (equirectangular, pinhole, fisheye)
   visibility_from_splatting  <- visibility.py:1073-1195, 1288-1322
   postprocess_features       <- visibility.py:1548-1582
-  VisibilityModel, SplattingVisibility <- visibility.py:1677-1776
+  read_s3dis_depth_map       <- visibility.py:1328-1358            (host, PIL)
+  visibility_from_depth_map  <- visibility.py:1361-1392
+  k_nn_image_system          <- visibility.py:1396-1460
+  visibility_biasutti        <- visibility.py:1463-1500
+  VisibilityModel, SplattingVisibility, DepthBasedVisibility, BiasuttiVisibility
+                             <- visibility.py:1677-1799
 
 Kernels: csrc/zbuffer.cu through the C ABI (dva_project_equirectangular, dva_project_camera,
-dva_splat_boxes, dva_splat_boxes_from_width, dva_zbuffer_splat).  Compaction of the kept set / winner map is index plumbing (torch.nonzero).
-Depth-map and Biasutti visibility models are out of scope (not used by any shipped config).
+dva_splat_boxes, dva_splat_boxes_from_width, dva_zbuffer_splat) and the exact grid k-NN of
+csrc/knn_features.cu (mapping.knn_grid) for the image-plane neighbours of the Biasutti model.
+Compaction of the kept set / winner map is index plumbing (torch.nonzero); the Biasutti
+contrast and the depth-map test are O(n k) / O(n) gathers and comparisons in torch.
 """
 import ctypes
 
@@ -228,6 +235,99 @@ def visibility_from_splatting(x_proj, y_proj, dist, xyz=None, img_extrinsic=None
     return idx_map[x_pix, y_pix], x_pix, y_pix + int(crop_top)
 
 
+# -------------------------------------------------------------------------------------------------
+# depth-map visibility
+# -------------------------------------------------------------------------------------------------
+def read_s3dis_depth_map(path, img_size=None, empty=-1):
+    """S3DIS depth PNG (16 bit, 1/512 m per unit, 65535 = no depth) -> float32 [W, H] CPU tensor
+    in metres, `empty` where there is no depth (visibility.py:1328-1358).  `img_size` = (W, H)
+    resizes with nearest-neighbour sampling first."""
+    from PIL import Image
+    im = Image.open(path)
+    if img_size is not None:
+        im = im.resize(tuple(int(v) for v in img_size), resample=Image.NEAREST)
+    a = np.array(im).T
+    out = a.astype(np.float32) / np.float32(512)        # exact: v < 2**16, 512 a power of two
+    out[a == 2 ** 16 - 1] = empty
+    return torch.from_numpy(np.ascontiguousarray(out))
+
+
+def visibility_from_depth_map(x_proj, y_proj, dist, depth_map_path=None, img_size=(1024, 512),
+                              depth_threshold=0.05, depth_map=None, **kwargs):
+    """Points whose depth is within `depth_threshold` of the depth map at their pixel
+    -> (indices, x_proj, y_proj) of the kept points, ascending (visibility.py:1361-1392).
+    `depth_map` ([W, H] float32) is used as is; otherwise the S3DIS PNG at `depth_map_path` is read
+    at `img_size`.  The comparison is |d_real - dist| <= depth_threshold in float32 (torch
+    compares an fp32 tensor with a Python float in fp32)."""
+    require_cuda(x_proj, y_proj, dist)
+    assert x_proj.shape[0] == y_proj.shape[0] == dist.shape[0] > 0
+    if depth_map is None:
+        assert depth_map_path is not None, 'Please provide depth_map_path or depth_map.'
+        depth_map = read_s3dis_depth_map(depth_map_path, img_size=img_size, empty=-1)
+    depth_map = depth_map.to(x_proj.device, torch.float32)
+    dist_real = depth_map[x_proj.long(), y_proj.long()]
+    thr = torch.tensor(depth_threshold, dtype=torch.float32, device=x_proj.device)
+    indices = torch.nonzero((dist_real - dist.float()).abs() <= thr, as_tuple=False).view(-1)
+    return indices, x_proj[indices], y_proj[indices]
+
+
+# -------------------------------------------------------------------------------------------------
+# Biasutti visibility
+# -------------------------------------------------------------------------------------------------
+def k_nn_image_system(x_proj, y_proj, k=75, x_margin=None, x_width=None):
+    """[n, k'] int64: the k nearest projections of every projection in the image plane, self
+    included, k' = min(k, search-set size) (visibility.py:1396-1460).  With `x_margin` > 0 and
+    `x_width` > 0 the image wraps around in x: the search set is the n projections, then copies of
+    those with x <= x_margin shifted by +x_width, then copies of those with x >= x_width - x_margin
+    shifted by -x_width; copies are reported as their original index.  Exact search on the GPU grid
+    k-NN (the reference runs a brute-force KeOps argKmin): squared distance dx*dx + dy*dy in fp32,
+    ties by search-set index."""
+    from .mapping import knn_grid
+    require_cuda(x_proj, y_proj)
+    assert x_margin is None or x_width > 0, 'x_margin and x_width must both be provided for image wrapping.'
+    n = x_proj.shape[0]
+    xy = torch.stack((x_proj.float(), y_proj.float()), dim=1)
+    wrap_x = x_margin is not None and x_margin > 0 and x_width is not None and x_width > 0
+    if wrap_x:
+        off = torch.tensor([[float(np.float32(x_width)), 0.0]], dtype=torch.float32, device=xy.device)
+        idx_left = torch.nonzero(x_proj <= x_margin, as_tuple=False).view(-1)
+        idx_right = torch.nonzero(x_proj >= (x_width - x_margin), as_tuple=False).view(-1)
+        search = torch.cat((xy, xy[idx_left] + off, xy[idx_right] - off))
+    else:
+        search = xy
+    m = search.shape[0]
+    kk = min(int(k), m)
+    pos = torch.cat((search, torch.zeros((m, 1), dtype=torch.float32, device=xy.device)), dim=1)
+    neighbors = knn_grid(pos, kk)[:n]
+    if wrap_x and m > n:
+        orig = torch.cat((torch.arange(n, device=xy.device), idx_left, idx_right))
+        neighbors = orig[neighbors]
+    return neighbors
+
+
+def visibility_biasutti(x_proj, y_proj, dist, img_size=None, k=75, margin=None, threshold=None, **kwargs):
+    """Biasutti et al., "Visibility estimation in point clouds with variable density"
+    (visibility.py:1463-1500): alpha = exp(-((d - d_min) / (d_max - d_min))**2) over the k
+    image-plane neighbours, kept where alpha >= threshold -> (indices, x_proj, y_proj) ascending.
+    `threshold=None` is the mean of alpha, summed in float64 and rounded to float32 (the reference
+    takes a float32 mean, a few ulps away).  A point whose neighbours all share one depth gets
+    alpha = NaN (0/0) and is never kept; with the mean threshold, one NaN keeps nothing."""
+    require_cuda(x_proj, y_proj, dist)
+    assert x_proj.shape[0] == y_proj.shape[0] == dist.shape[0] > 0
+    neighbors = k_nn_image_system(x_proj, y_proj, k=k, x_margin=margin, x_width=img_size[0])
+    d = dist.float()
+    dist_nn = d[neighbors]
+    dist_min = dist_nn.min(dim=1).values
+    dist_max = dist_nn.max(dim=1).values
+    alpha = torch.exp(-((d - dist_min) / (dist_max - dist_min)) ** 2)
+    if threshold is None:
+        thr = alpha.double().mean().float()
+    else:
+        thr = torch.tensor(threshold, dtype=torch.float32, device=alpha.device)
+    indices = torch.nonzero(alpha >= thr, as_tuple=False).view(-1)
+    return indices, x_proj[indices], y_proj[indices]
+
+
 def postprocess_features(xyz_to_img, y_proj, dist, linearity, planarity, scattering, normals,
                          img_size=(1024, 512), r_max=30, r_min=0.5, **kwargs):
     """[n,F] viewing-condition features (visibility.py:1548-1582): normalised depth, linearity,
@@ -304,3 +404,28 @@ class SplattingVisibility(VisibilityModel):
 
     def _visibility(self, x_proj, y_proj, dist, xyz, **kwargs):
         return visibility_from_splatting(x_proj, y_proj, dist, xyz, **self.__dict__, **kwargs)
+
+
+class DepthBasedVisibility(VisibilityModel):
+    """visibility.py:1779-1787.  The depth map comes per call: `depth_map` ([W, H] float32
+    tensor) or `depth_map_path` (S3DIS PNG)."""
+
+    def __init__(self, depth_threshold=0.05, **kwargs):
+        super().__init__(**kwargs)
+        self.depth_threshold = depth_threshold
+
+    def _visibility(self, x_proj, y_proj, dist, xyz, **kwargs):
+        return visibility_from_depth_map(x_proj, y_proj, dist, **self.__dict__, **kwargs)
+
+
+class BiasuttiVisibility(VisibilityModel):
+    """visibility.py:1790-1799."""
+
+    def __init__(self, k=75, margin=None, threshold=None, **kwargs):
+        super().__init__(**kwargs)
+        self.k = k
+        self.margin = margin
+        self.threshold = threshold
+
+    def _visibility(self, x_proj, y_proj, dist, xyz, **kwargs):
+        return visibility_biasutti(x_proj, y_proj, dist, **self.__dict__, **kwargs)

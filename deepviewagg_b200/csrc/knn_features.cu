@@ -16,7 +16,10 @@
 
 namespace dva {
 
+// k <= 64 keeps the 64-entry list per thread; 64 < k <= 128 uses a second instantiation with a
+// 128-entry list (same search, twice the local-memory list)
 constexpr int kKnnMax = 64;
+constexpr int kKnnMaxWide = 128;
 constexpr int kKnnMaxShells = 6;   // 13^3 cells; a query still open after that scans all points
 
 __global__ void __launch_bounds__(256)
@@ -35,14 +38,16 @@ __device__ __forceinline__ bool knn_less(float d, int64_t i, float d2, int64_t i
   return d < d2 || (d == d2 && i < i2);
 }
 
-// xyz_s / cell_s / order: points in cell-sorted order (order[j] = original index of sorted slot j)
+// xyz_s / cell_s / order: points in cell-sorted order (order[j] = original index of sorted slot j).
+// Planar inputs (z = 0) give (dx*dx + dy*dy) + 0, the exact 2D squared distance.
+template <int KMAX>
 __global__ void __launch_bounds__(128)
 knn_grid_kernel(const float* __restrict__ xyz_s, const int64_t* __restrict__ cell_s,
                 const int64_t* __restrict__ order, const int64_t* __restrict__ cell_ptr, int64_t n,
                 int k, float ox, float oy, float oz, float cs, int gx, int gy, int gz,
                 int64_t* __restrict__ nbr, float* __restrict__ d2out) {
-  float bd[kKnnMax];
-  int64_t bi[kKnnMax];
+  float bd[KMAX];
+  int64_t bi[KMAX];
   for (int64_t q = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; q < n; q += (int64_t)gridDim.x * blockDim.x) {
     const float px = xyz_s[3 * q], py = xyz_s[3 * q + 1], pz = xyz_s[3 * q + 2];
     const int64_t c = cell_s[q];
@@ -175,11 +180,15 @@ extern "C" int dva_knn_grid(const float* xyz_sorted, const int64_t* cell_sorted,
                             float cell_size, int gx, int gy, int gz, int64_t* neighbors, float* dist2,
                             void* stream) {
   if (n < 0 || gx < 1 || gy < 1 || gz < 1 || !(cell_size > 0.f)) return fail(DVA_EINVAL, "knn_grid: bad sizes");
-  if (k < 1 || k > kKnnMax) return fail(DVA_EUNSUPPORTED, "knn_grid: k must be in [1, 64]");
+  if (k < 1 || k > kKnnMaxWide) return fail(DVA_EUNSUPPORTED, "knn_grid: k must be in [1, 128]");
   if (n == 0) return DVA_OK;
   if (!xyz_sorted || !cell_sorted || !order || !cell_ptr || !neighbors) return fail(DVA_EINVAL, "knn_grid: null pointer");
-  knn_grid_kernel<<<k_grid(n, 128), 128, 0, (cudaStream_t)stream>>>(xyz_sorted, cell_sorted, order, cell_ptr, n, k, ox, oy,
-                                                                     oz, cell_size, gx, gy, gz, neighbors, dist2);
+  if (k <= kKnnMax)
+    knn_grid_kernel<kKnnMax><<<k_grid(n, 128), 128, 0, (cudaStream_t)stream>>>(
+        xyz_sorted, cell_sorted, order, cell_ptr, n, k, ox, oy, oz, cell_size, gx, gy, gz, neighbors, dist2);
+  else
+    knn_grid_kernel<kKnnMaxWide><<<k_grid(n, 128), 128, 0, (cudaStream_t)stream>>>(
+        xyz_sorted, cell_sorted, order, cell_ptr, n, k, ox, oy, oz, cell_size, gx, gy, gz, neighbors, dist2);
   return check_launch("knn_grid");
 }
 

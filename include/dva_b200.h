@@ -220,9 +220,11 @@ int dva_interp_pool_bwd_det(const void* grad_out, int channels_last, const int64
  *   dva_knn_cell_ids : cell[i] = linear cell of point i in a gx x gy x gz grid of `cell_size`
  *                      cubes anchored at (ox,oy,oz) (clamped).  The caller sorts points by cell
  *                      and builds cell_ptr [gx*gy*gz+1] (dva_csr_pointers_from_sorted).
- *   dva_knn_grid     : exact k nearest neighbours (self included), k <= 64, of every point among
- *                      all points; squared distance (dx*dx + dy*dy) + dz*dz in fp32, ties by
- *                      index.  neighbors [n,k] int64 and dist2 [n,k] (nullable) are indexed by
+ *   dva_knn_grid     : exact k nearest neighbours (self included), 1 <= k <= 128 (else
+ *                      DVA_EUNSUPPORTED, nothing launched), of every point among all points;
+ *                      squared distance (dx*dx + dy*dy) + dz*dz in fp32, ties by index.  Planar
+ *                      inputs (z = 0) give the exact 2D squared distance (image-plane k-NN).
+ *                      neighbors [n,k] int64 and dist2 [n,k] (nullable) are indexed by
  *                      ORIGINAL point id, ascending (dist2, id).
  *   dva_neighborhood_features : out [V, nk*(density + occlusion)] fp32 = for every k of the
  *                      ascending klist: density of the view's point ((k+1)/(3.1416 d_k^2)/(1/voxel^2),
