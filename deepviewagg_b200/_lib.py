@@ -92,6 +92,12 @@ SIGNATURES = {
                                            _i64, _f32, _f32, _vp]),
     "dva_project_camera": (_i32, [_vp, _vp, _i32, _vp, _vp, _vp, _vp, _i64, _i64, _i64, _i64, _i64, _f32,
                                   _f32, _vp]),
+    "dva_mapping_image_stats": (_i32, [_vp, _vp, _vp, _i32, _i64, _i64, _i64, _vp, _vp, _vp, _vp]),
+    "dva_center_roll": (_i32, [_vp, _i64, _i32, _i64, _vp, _vp]),
+    "dva_image_remap": (_i32, [_vp, _vp, _i64, _i64, _i64, _i64, _i64, _i64, _i32, _i32, _vp, _vp, _i32, _vp]),
+    "dva_coverage_index_workspace_bytes": (_sz, [_i64, _i64, _i64]),
+    "dva_coverage_index": (_i32, [_vp, _vp, _i64, _i64, _i64, _vp, _vp, _vp, _sz, _vp]),
+    "dva_coverage_pick": (_i32, [_i64, _i64, _i64, _i64, _vp, _vp, _vp, _sz, _vp]),
     "dva_csr_pointers_from_sorted": (_i32, [_vp, _vp, _i64, _i64, _vp]),
     "dva_csr_select_values": (_i32, [_vp, _vp, _vp, _vp, _i64, _i64, _vp]),
 }

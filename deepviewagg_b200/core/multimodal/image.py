@@ -10,7 +10,8 @@ Integer layout is the reference's bit for bit (Appendix B of SURVEY.md): pointer
 int64 [V], atomic CSR pointers int64 [V+1] over pixels intK [P,2] (x, y), features f32 [V,F],
 is_index_value = [True, False(, False)].  Sorting is stable (utils/multimodal.py), so results
 equal the reference up to the order of equal keys.  File loading, cropping/rolling augmentation,
-intrinsics bookkeeping and plotting are out of scope (dataset side).
+intrinsics bookkeeping and plotting are out of scope (dataset side).  Rolling and cropping of loaded
+samples (update_rollings / update_cropping, used by core/multimodal/transforms.py) are kept.
 """
 import copy
 from typing import List
@@ -401,7 +402,7 @@ class SameSettingImageData:
     opaquely in `extras` (same per-image leading dimension) so that image selection stays consistent."""
 
     def __init__(self, pos=None, opk=None, ref_size=(512, 256), proj_upscale=2, downscale=1, crop_size=None,
-                 crop_offsets=None, x=None, mappings=None, num_views=None, **extras):
+                 crop_offsets=None, x=None, mappings=None, num_views=None, rollings=None, **extras):
         self.pos = pos.double() if pos is not None else None
         self.opk = opk.double() if opk is not None else None
         self._num_views = num_views
@@ -415,6 +416,9 @@ class SameSettingImageData:
         self._mappings = None
         self.x = x
         self.mappings = mappings
+        # per-image width rolling wrt ref_size (image.py:553-576); not part of settings_hash (_shared_keys)
+        self.rollings = rollings if rollings is not None else \
+            torch.zeros(self.num_views, dtype=torch.long, device=self.device)
 
     # -- sizes
     @property
@@ -496,12 +500,14 @@ class SameSettingImageData:
         out.extras = dict(self.extras)
         out._x = self._x.clone() if self._x is not None else None
         out._mappings = self._mappings.clone() if self._mappings is not None else None
+        out.rollings = self.rollings.clone()
         return out
 
     def to(self, device):
         out = copy.copy(self)
         mv = lambda t: t.to(device) if isinstance(t, torch.Tensor) else t  # noqa: E731
         out.pos, out.opk, out.crop_offsets = mv(self.pos), mv(self.opk), mv(self.crop_offsets)
+        out.rollings = mv(self.rollings)
         out.extras = {k: mv(v) for k, v in self.extras.items()}
         out._x = mv(self._x)
         out._mappings = self._mappings.to(device) if self._mappings is not None else None
@@ -514,6 +520,7 @@ class SameSettingImageData:
         sel = lambda t: t[idx.to(t.device)] if isinstance(t, torch.Tensor) else t  # noqa: E731
         out = copy.copy(self)
         out.pos, out.opk, out.crop_offsets = sel(self.pos), sel(self.opk), sel(self.crop_offsets)
+        out.rollings = sel(self.rollings)
         out.extras = {k: sel(v) for k, v in self.extras.items()}
         out._num_views = int(idx.shape[0])
         out._x = self._x[idx] if self._x is not None else None
@@ -544,6 +551,56 @@ class SameSettingImageData:
             images.mappings = images.mappings.select_points(idx, mode=mode)
             return images
         raise ValueError(f"Unknown point selection mode '{mode}'.")
+
+    # -- rolling and cropping (image.py:578-628, 688-720)
+    def update_rollings(self, rollings):
+        """Roll `x` and the mappings along the width by `rollings` [B] int64, wrt ref_size: torch.roll
+        semantics, x[..., j] <- x[..., (j - r) mod W], and pixel x -> (x + r) % ref_W in pixel_dtype.  Images
+        are taken as circular along the width; prior cropping or resizing is refused, as in the reference.
+        CUDA containers roll `x` with one dva_image_remap copy.  No synchronisation."""
+        assert self.ref_size[0] == self.img_size[0], \
+            "CenterRoll cannot operate if images and mappings underwent prior cropping or resizing."
+        assert self.crop_size is None or self.crop_size == self.ref_size, \
+            "CenterRoll cannot operate if images and mappings underwent prior cropping or resizing."
+        assert self.downscale is None or self.downscale == 1, \
+            "CenterRoll cannot operate if images and mappings underwent prior cropping or resizing."
+        self.rollings = rollings
+        if self.x is not None:
+            if self.x.is_cuda:
+                self.x = ops.image_remap(self.x, rolls=self.rollings.to(self.x.device))
+            else:
+                self.x = torch.stack([torch.roll(im, int(r), dims=-1) for im, r in zip(self.x, self.rollings.cpu())])
+        if self.mappings is not None:
+            m = self.mappings.clone()
+            m.values[1] = m.values[1].clone()
+            pix = m.pixels.clone()
+            pix_roll = _expand(self.rollings.to(m.device)[m.images], m.values[1].pointers)
+            pix[:, 0] = ((pix[:, 0].long() + pix_roll) % self.ref_size[0]).to(self.pixel_dtype)
+            m.pixels = pix
+            self.mappings = m
+        return self
+
+    def update_cropping(self, crop_size, crop_offsets):
+        """Crop `x` and the mappings to `crop_size` (W, H) at per-image `crop_offsets` [B, 2] (x, y), both
+        wrt the current img_size.  The stored crop_size and crop_offsets are wrt ref_size: scaled by
+        `downscale` and accumulated over successive crops (a crop_offsets of None counts as zeros).  The
+        mappings go through ImageMapping.crop; CUDA containers crop `x` with one dva_image_remap copy.
+        Camera intrinsics are not adjusted: intrinsics bookkeeping belongs to the dataset side.  No
+        synchronisation."""
+        crop_offsets = crop_offsets.long()
+        base = self.crop_offsets if self.crop_offsets is not None else \
+            torch.zeros((self.num_views, 2), dtype=torch.long, device=self.device)
+        self.crop_size = tuple(int(v * self.downscale) for v in crop_size)
+        self.crop_offsets = (base + crop_offsets.to(base.device) * self.downscale).long()
+        if self.x is not None:
+            if self.x.is_cuda:
+                self.x = ops.image_remap(self.x, (crop_size[1], crop_size[0]), offsets=crop_offsets.to(self.x.device))
+            else:
+                self.x = torch.stack([im[:, o[1]:o[1] + crop_size[1], o[0]:o[0] + crop_size[0]]
+                                      for im, o in zip(self.x, crop_offsets.tolist())])
+        if self.mappings is not None:
+            self.mappings = self.mappings.crop(crop_size, crop_offsets)
+        return self
 
     # -- indexing for the pools
     @property
@@ -612,7 +669,7 @@ class SameSettingImageBatch(SameSettingImageData):
             pos=cat([im.pos for im in items]), opk=cat([im.opk for im in items]), ref_size=first.ref_size,
             proj_upscale=first.proj_upscale, downscale=first.downscale, crop_size=first.crop_size,
             crop_offsets=cat([im.crop_offsets for im in items]), num_views=sum(im.num_views for im in items),
-            **extras)
+            rollings=cat([im.rollings for im in items]), **extras)
         batch._x = cat([im.x for im in items])
         batch._mappings = mappings
         batch.__sizes__ = np.array([im.num_views for im in items])

@@ -215,9 +215,12 @@ static size_t carve_index(uint8_t* base, int64_t n_entries, int64_t nb, BucketIn
   return o;
 }
 
-// n_items items of NK entries each -> stable bucket index (w carved by carve_index)
+// n_items items of NK entries each -> stable bucket index in w.sorted (w carved by carve_index).  With
+// order == false the ordering pass is skipped and the caller reads w.bucket, whose order inside a bucket is
+// arbitrary: for uses that treat a bucket as a set.
 template <int NK, typename KeyOf>
-static int build_index(KeyOf key_of, int64_t n_items, int64_t nb, const BucketIndex& w, cudaStream_t st) {
+static int build_index(KeyOf key_of, int64_t n_items, int64_t nb, const BucketIndex& w, cudaStream_t st,
+                       bool order = true) {
   cudaError_t e = cudaMemsetAsync(w.cnt, 0, (size_t)(nb + 1) * 8, st);       // cnt + cursor
   if (e != cudaSuccess) return fail((int)e, "bucket index: memset failed");
   int rc;
@@ -229,6 +232,7 @@ static int build_index(KeyOf key_of, int64_t n_items, int64_t nb, const BucketIn
   if (n_items > 0) {
     scatter_keys<NK><<<grid_for(n_items), 256, 0, st>>>(key_of, n_items, nb, w.off, w.cursor, w.bucket);
     if ((rc = check_launch("bucket_scatter_keys"))) return rc;
+    if (!order) return DVA_OK;
     order_by_id<<<grid_for(nb * 32), 256, 0, st>>>(w.off, w.bucket, w.sorted, nb);
     if ((rc = check_launch("bucket_order_by_id"))) return rc;
   }

@@ -899,3 +899,95 @@ def linear(x, weight):
     else:
         z = _Linear.apply(x, weight)
     return z if z.dtype == out_dtype or out_dtype not in (torch.float16, torch.bfloat16) else z.to(out_dtype)
+
+
+# --------------------------------------------------------------------------------------------
+# image transforms (core/multimodal/transforms.py): integer mapping statistics, CenterRoll cost,
+# feature-map remap, coverage bookkeeping (csrc/image_transforms.cu)
+# --------------------------------------------------------------------------------------------
+_PIX_CODES = {torch.int16: 0, torch.int32: 1, torch.int64: 2}
+
+
+def mapping_image_stats(images, atomic_ptr, pixels, n_img, ref_w=None):
+    """Per image: pixel count [n] int64, bbox [n, 4] int32 (x_min, x_max, y_min, y_max; 0 for an image
+    without pixels) and, with ref_w, the 256-bin occupancy [n, 8] uint32 of the quantised width
+    (core/data_transform/multimodal/image.py:1005).  No synchronisation."""
+    require_cuda(images, atomic_ptr, pixels)
+    if pixels.dtype not in _PIX_CODES:
+        raise TypeError(f"mapping pixels must be int16/int32/int64, got {pixels.dtype}")
+    lib = _lib.load()
+    dev = images.device
+    images, atomic_ptr, pixels = images.long().contiguous(), atomic_ptr.long().contiguous(), pixels.contiguous()
+    count = torch.empty(n_img, dtype=torch.long, device=dev)
+    bbox = torch.empty((n_img, 4), dtype=torch.int32, device=dev)
+    occ = torch.empty((n_img, 8), dtype=torch.int32, device=dev) if ref_w is not None else None
+    with torch.cuda.device(dev):
+        check(lib.dva_mapping_image_stats(ptr(images), ptr(atomic_ptr), ptr(pixels), _PIX_CODES[pixels.dtype],
+                                          int(images.shape[0]), int(n_img), int(ref_w or 0), ptr(count), ptr(bbox),
+                                          ptr(occ), stream_ptr()), "dva_mapping_image_stats")
+    return count, bbox, occ
+
+
+def center_roll(occ, angular_res, ref_w):
+    """Rollings [n] int64 of CenterRoll from the occupancy of mapping_image_stats (image.py:1009-1029)."""
+    require_cuda(occ)
+    lib = _lib.load()
+    out = torch.empty(occ.shape[0], dtype=torch.long, device=occ.device)
+    with torch.cuda.device(occ.device):
+        check(lib.dva_center_roll(ptr(occ.contiguous()), int(occ.shape[0]), int(angular_res), int(ref_w), ptr(out),
+                                  stream_ptr()), "dva_center_roll")
+    return out
+
+
+_REMAP_ELEM = (1, 2, 4)
+
+
+def image_remap(x, out_hw=None, rolls=None, offsets=None, flip=False):
+    """out[b, :, y, x'] = x[b, :, oy_b + y, (ox_b + (flip ? Wo-1-x' : x') - r_b) mod W] in one copy: the
+    per-image torch.roll of update_rollings, the crop of update_cropping and the horizontal flip.  x is
+    [B, C, H, W] of 1, 2 or 4-byte elements, NCHW or channels-last; the output keeps x's memory format.
+    rolls [B] int64, offsets [B, 2] int64 (ox, oy) on x's device.  No synchronisation."""
+    require_cuda(x)
+    if x.dim() != 4 or x.element_size() not in _REMAP_ELEM:
+        raise TypeError(f"image_remap: expected a 4-D tensor of 1, 2 or 4-byte elements, got {tuple(x.shape)} "
+                        f"{x.dtype}")
+    B, C, H, W = x.shape
+    Ho, Wo = (H, W) if out_hw is None else (int(out_hw[0]), int(out_hw[1]))
+    cl = (not x.is_contiguous()) and x.is_contiguous(memory_format=torch.channels_last)
+    fmt = torch.channels_last if cl else torch.contiguous_format
+    x = x.contiguous(memory_format=fmt)
+    out = torch.empty((B, C, Ho, Wo), dtype=x.dtype, device=x.device, memory_format=fmt)
+    rolls = rolls.to(x.device, torch.long).contiguous() if rolls is not None else None
+    offsets = offsets.to(x.device, torch.long).contiguous() if offsets is not None else None
+    lib = _lib.load()
+    with torch.cuda.device(x.device):
+        check(lib.dva_image_remap(ptr(x), ptr(out), B, C, H, W, Ho, Wo, x.element_size(), int(cl), ptr(rolls),
+                                  ptr(offsets), int(bool(flip)), stream_ptr()), "dva_image_remap")
+    return out
+
+
+class CoverageIndex:
+    """Unseen-point counts of PickImagesFromMemoryCredit (image.py:804-867) without the dense
+    bool[n_img, N] table: `gimg` [V] global image id of every view (setting base + local id), `vpoint` [V]
+    its point.  `unseen` [n_img] int32 starts at the view count of every image; pick(g) marks g's points
+    seen and takes every newly seen point off the count of each image that sees it."""
+
+    def __init__(self, gimg, vpoint, n_img, num_points):
+        require_cuda(gimg, vpoint)
+        lib = _lib.load()
+        self.dev = gimg.device
+        self.V, self.n_img, self.N = int(gimg.shape[0]), int(n_img), int(num_points)
+        self.ws_bytes = int(lib.dva_coverage_index_workspace_bytes(self.V, self.n_img, self.N))
+        self.ws = torch.empty(self.ws_bytes, dtype=torch.uint8, device=self.dev)
+        self.unseen = torch.empty(self.n_img, dtype=torch.int32, device=self.dev)
+        self.seen = torch.empty(max(self.N, 1), dtype=torch.int32, device=self.dev)
+        self._gimg, self._vpoint = gimg.long().contiguous(), vpoint.long().contiguous()
+        with torch.cuda.device(self.dev):
+            check(lib.dva_coverage_index(ptr(self._gimg), ptr(self._vpoint), self.V, self.n_img, self.N,
+                                         ptr(self.unseen), ptr(self.seen), ptr(self.ws), self.ws_bytes, stream_ptr()),
+                  "dva_coverage_index")
+
+    def pick(self, g):
+        with torch.cuda.device(self.dev):
+            check(_lib.load().dva_coverage_pick(int(g), self.V, self.n_img, self.N, ptr(self.unseen), ptr(self.seen),
+                                                ptr(self.ws), self.ws_bytes, stream_ptr()), "dva_coverage_pick")

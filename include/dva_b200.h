@@ -417,6 +417,49 @@ int dva_mapping_build(const int64_t* point_ids, const int64_t* image_ids, const 
 int dva_view_cat_sorting(const int64_t* const* ptrs, const int64_t* bases, int64_t S, int64_t N,
                          int64_t* sorting, int64_t* csr_cat, void* stream);
 
+/* T1  per-image mapping statistics (csrc/image_transforms.cu)     replaces the torch_scatter passes of
+ *   PickImagesFromMappingArea, ImageMapping.bounding_boxes (CropImageGroups) and CenterRoll
+ *   (core/data_transform/multimodal/image.py:733-749, :999-1015).  Views v < V: images [V] int64 in
+ *   [0, n_img) (others skipped), atomic_ptr [V + 1], pixels [P, 2] (x, y) int16 / int32 / int64 (pix_code
+ *   0 / 1 / 2).  Outputs: count [n_img] int64 pixels per image; bbox [n_img, 4] int32 = (x_min, x_max,
+ *   y_min, y_max), all 0 for an image without pixels; occ [n_img, 8] uint32 (nullable) = bit q set for
+ *   every q = (int64)(fp32(fp32(x * 256) / ref_w)) & 255 of the image.  Integer atomics only: the result
+ *   does not depend on the launch. */
+int dva_mapping_image_stats(const int64_t* images, const int64_t* atomic_ptr, const void* pixels, int pix_code,
+                            int64_t V, int64_t n_img, int64_t ref_w, int64_t* count, int32_t* bbox, uint32_t* occ,
+                            void* stream);
+
+/* T2  CenterRoll cost                          replaces image.py:1009-1029 on the occupancy of T1.
+ *   Candidate rolls r = 0, s, 2s, .. < 256 with s = 256 / angular_res (integer division); bins (b + r) & 255;
+ *   cost = (w_max - w_min) + int(|fp32(w_max + w_min) / 2 - 128|), first least cost wins;
+ *   rollings [n_img] int64 = (int64)(fp32(r / 256) * ref_w). */
+int dva_center_roll(const uint32_t* occ, int64_t n_img, int angular_res, int64_t ref_w, int64_t* rollings,
+                    void* stream);
+
+/* T3  batched feature-map remap                 replaces the per-image roll / slice / flip loops + torch.cat
+ *   of SameSettingImageData.update_rollings / update_cropping and RandomHorizontalFlip (image.py:605-609,
+ *   :709-714, data_transform image.py:1207-1212).  in [B, C, Hi, Wi], out [B, C, Ho, Wo], both NCHW or both
+ *   channels-last (channels_last != 0), elements of elem_bytes = 1, 2 or 4 bytes moved as raw bytes:
+ *     out[b, c, y, x] = in[b, c, oy_b + y, (ox_b + (flip ? Wo - 1 - x : x) - r_b) mod Wi]
+ *   rolls [B] int64 (nullable: 0), offsets [B, 2] int64 (ox, oy) (nullable: 0).  Rows whose oy_b + y falls
+ *   outside the input are written as zeros. */
+int dva_image_remap(const void* in, void* out, int64_t B, int64_t C, int64_t Hi, int64_t Wi, int64_t Ho, int64_t Wo,
+                    int elem_bytes, int channels_last, const int64_t* rolls, const int64_t* offsets, int flip,
+                    void* stream);
+
+/* T4  coverage bookkeeping of PickImagesFromMemoryCredit      replaces the dense bool[n_img, N] table and
+ *   the per-pick logical_and loop of image.py:804-867.  Views v < V of all settings: gimg [V] = global image id
+ *   in [0, n_img) (setting base + local id), vpoint [V] = point id in [0, N).  dva_coverage_index builds the
+ *   image -> points and point -> images lists in the workspace (dva_coverage_index_workspace_bytes) and sets
+ *   unseen [n_img] int32 = views of every image, seen [N] int32 = 0.  dva_coverage_pick(g): every point p of
+ *   image g with atomicExch(&seen[p], 1) == 0 takes one off unseen[j] of every image j that sees p.  Integer
+ *   counts: the result does not depend on the order.  Total work over all picks <= V. */
+size_t dva_coverage_index_workspace_bytes(int64_t V, int64_t n_img, int64_t N);
+int dva_coverage_index(const int64_t* gimg, const int64_t* vpoint, int64_t V, int64_t n_img, int64_t N,
+                       int32_t* unseen, int32_t* seen, void* workspace, size_t workspace_bytes, void* stream);
+int dva_coverage_pick(int64_t g, int64_t V, int64_t n_img, int64_t N, int32_t* unseen, int32_t* seen,
+                      const void* workspace, size_t workspace_bytes, void* stream);
+
 /* C1  CSR pointers from sorted dense ids     replaces csr.py:158-172 + :197-229
  *   ids [n] int64 sorted ascending, values in [0,num_groups) -> ptr [num_groups+1] int64 with
  *   empty groups inserted (from_dense + insert_empty_groups, image.py:1787-1793). */
