@@ -98,6 +98,9 @@ SIGNATURES = {
     "dva_coverage_index_workspace_bytes": (_sz, [_i64, _i64, _i64]),
     "dva_coverage_index": (_i32, [_vp, _vp, _i64, _i64, _i64, _vp, _vp, _vp, _sz, _vp]),
     "dva_coverage_pick": (_i32, [_i64, _i64, _i64, _i64, _vp, _vp, _vp, _sz, _vp]),
+    "dva_resample_u8": (_i32, [_vp, _vp, _vp, _i64, _i64, _i64, _i64, _i64, _i64, _i64, _vp, _vp, _i64, _i32, _vp,
+                                _vp, _i64, _i32, _vp, _vp]),
+    "dva_nonstatic_mask": (_i32, [_vp, _i64, _i64, _i64, _i64, _vp, _vp]),
     "dva_csr_pointers_from_sorted": (_i32, [_vp, _vp, _i64, _i64, _vp]),
     "dva_csr_select_values": (_i32, [_vp, _vp, _vp, _vp, _i64, _i64, _vp]),
 }

@@ -9,9 +9,10 @@
 Integer layout is the reference's bit for bit (Appendix B of SURVEY.md): pointers int64, images
 int64 [V], atomic CSR pointers int64 [V+1] over pixels intK [P,2] (x, y), features f32 [V,F],
 is_index_value = [True, False(, False)].  Sorting is stable (utils/multimodal.py), so results
-equal the reference up to the order of equal keys.  File loading, cropping/rolling augmentation,
-intrinsics bookkeeping and plotting are out of scope (dataset side).  Rolling and cropping of loaded
-samples (update_rollings / update_cropping, used by core/multimodal/transforms.py) are kept.
+equal the reference up to the order of equal keys.  Intrinsics bookkeeping and plotting are out of scope
+(dataset side).  Rolling and cropping of loaded samples (update_rollings / update_cropping, used by
+core/multimodal/transforms.py) are kept, and so is image loading (read_images / load, image.py:973-1101):
+Pillow on CPU containers, the Pillow-exact resize kernel of csrc/image_resample.cu on CUDA containers.
 """
 import copy
 from typing import List
@@ -399,10 +400,18 @@ class ImageMappingBatch(ImageMapping, CSRBatch):
 class SameSettingImageData:
     """Feature maps `x` [B,C,H,W] of B images sharing one acquisition setting + their mappings
     (image.py:177-1287).  Only the state the aggregation path reads is kept: pose arrays are carried
-    opaquely in `extras` (same per-image leading dimension) so that image selection stays consistent."""
+    opaquely in `extras` (same per-image leading dimension) so that image selection stays consistent.
+    `path` [B] (numpy object array) names the image files read by read_images / load; `mask` [W_proj, H_proj]
+    bool is the projection mask MapImages applies (a shared setting: kept by indexing, clone and to, taken
+    from the first item when batching, and not part of settings_hash, as in the reference)."""
+
+    # decoded native-resolution bytes staged per chunk by the CUDA read_images (S3DIS panoramas are 25 MB each)
+    _READ_CHUNK_BYTES = 256 << 20
 
     def __init__(self, pos=None, opk=None, ref_size=(512, 256), proj_upscale=2, downscale=1, crop_size=None,
-                 crop_offsets=None, x=None, mappings=None, num_views=None, rollings=None, **extras):
+                 crop_offsets=None, x=None, mappings=None, num_views=None, rollings=None, path=None, mask=None,
+                 **extras):
+        self.path = np.array(path, dtype=object).reshape(-1) if path is not None else None
         self.pos = pos.double() if pos is not None else None
         self.opk = opk.double() if opk is not None else None
         self._num_views = num_views
@@ -419,6 +428,8 @@ class SameSettingImageData:
         # per-image width rolling wrt ref_size (image.py:553-576); not part of settings_hash (_shared_keys)
         self.rollings = rollings if rollings is not None else \
             torch.zeros(self.num_views, dtype=torch.long, device=self.device)
+        self._mask = None
+        self.mask = mask
 
     # -- sizes
     @property
@@ -427,7 +438,9 @@ class SameSettingImageData:
             return self.pos.shape[0]
         if self._num_views is not None:
             return self._num_views
-        return self._x.shape[0] if self._x is not None else 0
+        if self._x is not None:
+            return self._x.shape[0]
+        return len(self.path) if self.path is not None else 0
 
     @property
     def num_points(self):
@@ -444,6 +457,26 @@ class SameSettingImageData:
     @property
     def downscale(self):
         return self._downscale
+
+    @property
+    def proj_size(self):
+        """Size (W, H) of the projection map and of the mask: ref_size * proj_upscale (image.py:543-551)."""
+        return tuple(int(v * self.proj_upscale) for v in self.ref_size)
+
+    @property
+    def mask(self):
+        """Projection mask: None or a [W_proj, H_proj] bool tensor (image.py:952-971)."""
+        return self._mask
+
+    @mask.setter
+    def mask(self, mask):
+        if mask is None:
+            self._mask = None
+            return
+        assert mask.dtype == torch.bool, f"Expected a dtype=torch.bool but got dtype={mask.dtype} instead."
+        assert tuple(mask.shape) == self.proj_size, \
+            f"Expected mask of size {self.proj_size} but got {tuple(mask.shape)} instead."
+        self._mask = mask.to(self.device)
 
     @property
     def pixel_dtype(self):
@@ -511,6 +544,7 @@ class SameSettingImageData:
         out.extras = {k: mv(v) for k, v in self.extras.items()}
         out._x = mv(self._x)
         out._mappings = self._mappings.to(device) if self._mappings is not None else None
+        out._mask = mv(self._mask)
         return out
 
     def __getitem__(self, idx):
@@ -525,6 +559,8 @@ class SameSettingImageData:
         out._num_views = int(idx.shape[0])
         out._x = self._x[idx] if self._x is not None else None
         out._mappings = self._mappings.select_images(idx) if self._mappings is not None else None
+        out.path = self.path[idx.cpu().numpy()] if self.path is not None else None
+        out._mask = self._mask.clone() if self._mask is not None else None
         return out
 
     def select_points(self, idx, mode='pick'):
@@ -602,6 +638,86 @@ class SameSettingImageData:
             self.mappings = self.mappings.crop(crop_size, crop_offsets)
         return self
 
+    # -- image loading (image.py:973-1101)
+    def load(self, show_progress=False):
+        """Read the images of `path` into `x` at ref_size with the container's rollings, crop_size, crop_offsets
+        and downscale (image.py:973-989), on the container's device.  See read_images."""
+        crop_offsets = self.crop_offsets if self.crop_offsets is not None else \
+            torch.zeros((self.num_views, 2), dtype=torch.long)
+        self._x = self.read_images(size=self.ref_size, rollings=self.rollings, crop_size=self.crop_size,
+                                   crop_offsets=crop_offsets, downscale=self.downscale,
+                                   show_progress=show_progress).to(self.device)
+        return self
+
+    def read_images(self, idx=None, size=None, rollings=None, crop_size=None, crop_offsets=None, downscale=None,
+                    show_progress=False):
+        """Read the images `path[idx]` as a [B, 3, H, W] uint8 tensor in channels-last memory, as the reference
+        does (image.py:991-1101): decode to RGB, resize to `size` (W, H) with Pillow's default BICUBIC filter,
+        roll every image sideways by `rollings` (out[:, x] = in[:, (x + r) mod W], i.e. torch.roll by -r, the
+        opposite of update_rollings), then crop `crop_size` at `crop_offsets` or, when `downscale` is set,
+        resize that box to int(crop_size / downscale).  A crop box must lie inside the resized image.
+
+        CPU containers run Pillow.  CUDA containers decode on the host and stage runs of consecutive images of
+        one native size (at most _READ_CHUNK_BYTES decoded) in pinned memory, copy them asynchronously and
+        resize / roll / crop them with ops.image_resample and ops.image_remap, bit for bit what Pillow gives.
+        Host work: decoding; no device->host read."""
+        if idx is None:
+            idx = np.arange(self.num_views)
+        elif isinstance(idx, int):
+            idx = np.array([idx])
+        elif isinstance(idx, torch.Tensor):
+            idx = np.asarray(idx.cpu())
+        elif isinstance(idx, slice):
+            idx = np.arange(self.num_views)[idx]
+        idx = np.asarray(idx).reshape(-1)
+        assert self.path is not None and len(self.path) == self.num_views, \
+            "read_images needs one path per image in 'path'."
+        size = tuple(int(v) for v in (size if size is not None else self.img_size))
+        if rollings is not None:
+            assert rollings.dtype == torch.int64, f"Expected dtype=torch.int64 but got dtype={rollings.dtype} instead."
+            assert rollings.shape[0] == idx.shape[0], \
+                f"Expected tensor of shape {idx.shape[0]} but got {rollings.shape[0]} instead."
+        else:
+            rollings = torch.zeros(idx.shape[0], dtype=torch.long)
+        assert bool(crop_size) == bool(crop_offsets is not None), \
+            "If either 'crop_size' or 'crop_offsets' is specified, both must be specified."
+        if crop_size is not None:
+            crop_size = tuple(int(v) for v in crop_size)
+            assert len(crop_size) == 2, f"Expected len(crop_size)=2 but got {len(crop_size)} instead."
+            assert all(a <= b for a, b in zip(crop_size, size)), \
+                f"Expected crop_size to be smaller than size but got size={size} and crop_size={crop_size} instead."
+            assert crop_offsets.dtype == torch.int64, \
+                f"Expected dtype=torch.int64 but got dtype={crop_offsets.dtype} instead."
+            assert tuple(crop_offsets.shape) == (idx.shape[0], 2), \
+                f"Expected tensor of shape {(idx.shape[0], 2)} but got {tuple(crop_offsets.shape)} instead."
+        else:
+            crop_size = size
+            crop_offsets = torch.zeros((idx.shape[0], 2), dtype=torch.long)
+        if downscale is not None:
+            assert downscale >= 1, f"Expected scalar larger than 1 but got {downscale} instead."
+        offsets = crop_offsets.cpu().long()
+        assert bool((offsets >= 0).all()) and bool((offsets + torch.tensor(crop_size) <= torch.tensor(size)).all()), \
+            f"Crop boxes of size {crop_size} must lie inside the {size} images."
+        paths = self.path[idx]
+        if show_progress:
+            from tqdm.auto import tqdm
+            paths = tqdm(paths)
+        end_size = crop_size if downscale is None else tuple(int(v / downscale) for v in crop_size)
+        from PIL import Image
+        if self.device.type == 'cuda':
+            return _read_images_cuda(list(paths), size, rollings.cpu().long(), crop_size, offsets, downscale,
+                                     end_size, self.device, self._READ_CHUNK_BYTES)
+        w, h = crop_size
+        arrays = []
+        for p, r, (left, top) in zip(paths, rollings.cpu().tolist(), offsets.tolist()):
+            im = Image.open(p).convert('RGB').resize(size)
+            if r % size[0]:
+                im = Image.fromarray(np.roll(np.asarray(im), -(r % size[0]), axis=1))
+            box = (left, top, left + w, top + h)
+            im = im.crop(box) if downscale is None else im.resize(end_size, box=box)
+            arrays.append(np.asarray(im))
+        return torch.from_numpy(np.stack(arrays)).permute(0, 3, 1, 2)
+
     # -- indexing for the pools
     @property
     def feature_map_indexing(self):
@@ -643,6 +759,39 @@ class SameSettingImageData:
                 f"device={self.device})")
 
 
+def _read_images_cuda(paths, size, rollings, crop_size, offsets, downscale, end_size, device, chunk_bytes):
+    """CUDA body of SameSettingImageData.read_images: [B, 3, H, W] uint8, channels-last, on `device`."""
+    from PIL import Image
+    n = len(paths)
+    native = [Image.open(p).size for p in paths]            # header only, no decoding
+    out = torch.empty((n, end_size[1], end_size[0], 3), dtype=torch.uint8, device=device)
+    w, h = crop_size
+    rolls = -(rollings % size[0])
+    boxes = torch.cat([offsets, offsets + torch.tensor([[w, h]])], dim=1)
+    i = 0
+    while i < n:
+        W0, H0 = native[i]
+        j = i + 1
+        while j < n and native[j] == (W0, H0) and (j + 1 - i) * W0 * H0 * 3 <= chunk_bytes:
+            j += 1
+        staged = torch.empty((j - i, H0, W0, 3), dtype=torch.uint8, pin_memory=True)
+        for k in range(i, j):
+            staged[k - i].numpy()[...] = np.asarray(Image.open(paths[k]).convert('RGB'))
+        x = staged.to(device, non_blocking=True).permute(0, 3, 1, 2)
+        x = ops.image_resample(x, size)
+        r = rolls[i:j]
+        if downscale is None:
+            x = ops.image_remap(x, (h, w), rolls=ops._pinned_to(r.numpy(), device),
+                                offsets=ops._pinned_to(offsets[i:j].numpy(), device))
+        else:
+            if bool((r != 0).any()):
+                x = ops.image_remap(x, rolls=ops._pinned_to(r.numpy(), device))
+            x = ops.image_resample(x, end_size, boxes=boxes[i:j].float())
+        out[i:j] = x.permute(0, 2, 3, 1)
+        i = j
+    return out.permute(0, 3, 1, 2)
+
+
 class SameSettingImageBatch(SameSettingImageData):
     """image.py:1290-1406."""
 
@@ -670,6 +819,9 @@ class SameSettingImageBatch(SameSettingImageData):
             proj_upscale=first.proj_upscale, downscale=first.downscale, crop_size=first.crop_size,
             crop_offsets=cat([im.crop_offsets for im in items]), num_views=sum(im.num_views for im in items),
             rollings=cat([im.rollings for im in items]), **extras)
+        batch.path = np.concatenate([im.path for im in items]) if all(im.path is not None for im in items) else None
+        # the first item's mask serves the batch: masks computed by NonStaticMask may differ slightly
+        batch._mask = first.mask
         batch._x = cat([im.x for im in items])
         batch._mappings = mappings
         batch.__sizes__ = np.array([im.num_views for im in items])

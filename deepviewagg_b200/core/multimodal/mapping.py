@@ -47,7 +47,9 @@ class MapImages:
             images.crop_size = images.ref_size
         if self.proj_upscale is not None:
             images.proj_upscale = self.proj_upscale
-        proj_size = tuple(int(v * images.proj_upscale) for v in images.ref_size)
+        proj_size = images.proj_size
+        if images.mask is not None:      # points projecting onto a masked pixel neither map nor occlude
+            assert tuple(images.mask.shape) == proj_size
         model = getattr(visibility_module, self.method)(img_size=proj_size, **self.kwargs)
         dev = torch.device(device)
         pos_d = pos.float().to(dev)
@@ -80,6 +82,8 @@ class MapImages:
                 kw['img_intrinsic_pinhole'] = ex['intrinsic_pinhole'][i].float()
             if 'intrinsic_fisheye' in ex:
                 kw['img_intrinsic_fisheye'] = ex['intrinsic_fisheye'][i].float()
+            if images.mask is not None:
+                kw['img_mask'] = images.mask.to(dev)
             out = model(pos_d, images.pos[i].float(), linearity=lin, planarity=pla, scattering=sca, normals=nor,
                         **kw)
             if out['idx'].shape[0] == 0:

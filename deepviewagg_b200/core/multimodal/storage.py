@@ -13,6 +13,11 @@ two-level CSR exactly as the kernels consume them (SURVEY Appendix B):
                     s{s}/pixels     int16|int32 [P,2]
                     s{s}/features   float32 [V,F]   (optional)
                     s{s}/pos, s{s}/opk float64 [B,3] and any per-image extras
+                    s{s}/x          [B,C,H,W] feature maps, raw bytes in their memory layout
+                                    (channels-last maps stored as [B,H,W,C]) (optional)
+                    s{s}/mask       bool [W_proj,H_proj] projection mask (optional)
+
+    image paths, when set, are kept in the JSON header.
 
 Arrays are read back through `numpy.memmap` (no copy, no unpickling) and uploaded with one
 pinned, asynchronous H2D copy each; `load_image_data(..., device='cuda')` therefore costs one
@@ -55,9 +60,17 @@ def save_image_data(path, image_data):
         for key, val in im.extras.items():
             if isinstance(val, torch.Tensor):
                 arrays[pre + "extras/" + key] = _np(val)
-        meta["settings"].append(dict(ref_size=list(im.ref_size), proj_upscale=im.proj_upscale,
-                                     downscale=im.downscale, crop_size=list(im.crop_size),
-                                     num_views=int(im.num_views), has_features=bool(m.has_features)))
+        st = dict(ref_size=list(im.ref_size), proj_upscale=im.proj_upscale, downscale=im.downscale,
+                  crop_size=list(im.crop_size), num_views=int(im.num_views), has_features=bool(m.has_features))
+        if im.x is not None:
+            cl = (not im.x.is_contiguous()) and im.x.is_contiguous(memory_format=torch.channels_last)
+            arrays[pre + "x"] = _np(im.x.permute(0, 2, 3, 1) if cl else im.x)
+            st["x_channels_last"] = bool(cl)
+        if im.mask is not None:
+            arrays[pre + "mask"] = _np(im.mask)
+        if im.path is not None:
+            st["path"] = [str(p) for p in im.path]
+        meta["settings"].append(st)
     offset, table = 0, {}
     for name, a in arrays.items():
         offset = (offset + _ALIGN - 1) // _ALIGN * _ALIGN
@@ -123,5 +136,12 @@ def load_image_data(path, device="cpu", pin=True):
                                   crop_size=tuple(st["crop_size"]), crop_offsets=opt("crop_offsets"),
                                   num_views=st["num_views"], **extras)
         im.mappings = maps
+        if pre + "x" in meta["arrays"]:
+            x = t(pre + "x")
+            im._x = x.permute(0, 3, 1, 2) if st.get("x_channels_last") else x
+        if pre + "mask" in meta["arrays"]:
+            im.mask = t(pre + "mask")
+        if "path" in st:
+            im.path = np.array(st["path"], dtype=object)
         out.append(im)
     return ImageData(out)

@@ -1,7 +1,9 @@
 """Per-sample image transforms with the reference's names, arguments and defaults
 (torch_points3d/core/data_transform/multimodal/image.py), for the chain every shipped dataset config runs
-between loading a sample and the forward pass:
+between loading a sample and the forward pass, and the two that open every config's pre_transform chain
+(LoadImages -> NonStaticMask -> MapImages -> NeighborhoodBasedMappingFeatures):
 
+  LoadImages -> NonStaticMask
   SelectMappingFromPointId -> CenterRoll -> PickImagesFromMappingArea -> CropImageGroups
     -> PickImagesFromMemoryCredit -> JitterMappingFeatures -> RandomHorizontalFlip
 
@@ -98,6 +100,72 @@ class ImageTransform:
     def __repr__(self):
         attr_repr = ', '.join([f'{k}={v}' for k, v in self.__dict__.items()])
         return f'{self.__class__.__name__}({attr_repr})'
+
+
+def _set_ref_size(images, ref_size):
+    """image.py:492-505: a new ref_size resets crop_size."""
+    images.ref_size = tuple(ref_size)
+    images.crop_size = images.ref_size
+
+
+class LoadImages(ImageTransform):
+    """Load the images of `images.path` into `images.x` (image.py:69-102): the given ref_size, crop_size,
+    crop_offsets and downscale are set on the container first, then SameSettingImageData.load reads the images
+    wrt that state.  Syncs: none on the device; the host decodes every image."""
+
+    def __init__(self, ref_size=None, crop_size=None, crop_offsets=None, downscale=None, show_progress=False):
+        self.ref_size = ref_size
+        self.crop_size = crop_size
+        self.crop_offsets = crop_offsets
+        self.downscale = downscale
+        self.show_progress = show_progress
+
+    def _process(self, data, images):
+        if self.ref_size is not None:
+            _set_ref_size(images, self.ref_size)
+        if self.crop_size is not None:
+            images.crop_size = tuple(self.crop_size)
+        if self.crop_offsets is not None:
+            images.crop_offsets = self.crop_offsets
+        if self.downscale is not None:
+            images._downscale = self.downscale
+        if self.show_progress:
+            print("    LoadImages...")
+        images.load(show_progress=self.show_progress)
+        return data, images
+
+
+class NonStaticMask(ImageTransform):
+    """Projection mask of the pixels that are not identical across images (image.py:105-159), e.g. to drop
+    the camera rig or the vehicle body: `n_sample` images drawn with the reference's
+    torch.multinomial(torch.arange(n, dtype=torch.float), n_sample) on the CPU generator are read at
+    proj_size, and a pixel is True when every channel of some drawn image differs from the first drawn one.
+    With fewer than 2 images the mask is all True.  Image 0 has weight 0 in that draw, so it is drawn only
+    after every other image (reproduced as is).  CUDA: read_images + dva_nonstatic_mask; syncs: none on the
+    device."""
+
+    def __init__(self, ref_size=None, proj_upscale=None, n_sample=5):
+        self.ref_size = tuple(ref_size) if ref_size is not None else None
+        self.proj_upscale = proj_upscale
+        self.n_sample = n_sample
+
+    def _process(self, data, images):
+        if self.ref_size is not None:
+            _set_ref_size(images, self.ref_size)
+        if self.proj_upscale is not None:
+            images.proj_upscale = self.proj_upscale
+        n_sample = min(self.n_sample, images.num_views)
+        if n_sample < 2:
+            mask = torch.ones(images.proj_size, dtype=torch.bool)
+        else:
+            idx = torch.multinomial(torch.arange(images.num_views, dtype=torch.float), n_sample)
+            imgs = images.read_images(idx=idx, size=images.proj_size)
+            if imgs.is_cuda:
+                mask = ops.nonstatic_mask(imgs)
+            else:
+                mask = (imgs[1:] != imgs[:1]).all(dim=1).any(dim=0).t().contiguous()
+        images.mask = mask
+        return data, images
 
 
 class SelectMappingFromPointId(ImageTransform):

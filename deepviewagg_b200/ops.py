@@ -8,6 +8,7 @@ reference repository root.
 import math
 import os
 
+import numpy as np
 import torch
 
 # torch.amp integration (SURVEY 8b "Autograd / AMP / recompute"): every autograd.Function's forward is
@@ -991,3 +992,129 @@ class CoverageIndex:
         with torch.cuda.device(self.dev):
             check(_lib.load().dva_coverage_pick(int(g), self.V, self.n_img, self.N, ptr(self.unseen), ptr(self.seen),
                                                 ptr(self.ws), self.ws_bytes, stream_ptr()), "dva_coverage_pick")
+
+
+# --------------------------------------------------------------------------------------------
+# image loading (SameSettingImageData.read_images, NonStaticMask): Pillow-exact resize and the
+# non-static pixel mask (csrc/image_resample.cu)
+# --------------------------------------------------------------------------------------------
+_PRECISION_BITS = 32 - 8 - 2
+
+
+def _bicubic(x):
+    """Pillow's bicubic_filter (a = -0.5) in float64, with its evaluation order."""
+    a = -0.5
+    x = np.abs(x)
+    near = ((a + 2.0) * x - (a + 3.0)) * x * x + 1
+    far = (((x - 5) * x + 8) * x - 4) * a
+    return np.where(x < 1.0, near, np.where(x < 2.0, far, 0.0))
+
+
+def resample_axis_tables(in_size, in0, in1, out_size):
+    """Pillow's precompute_coeffs + normalize_coeffs_8bpc for one axis and one box [in0, in1) (C floats):
+    bounds [out, 2] int32 (first source index, count) and weights [out, ksize] int32 scaled by 2^22.  Every
+    float64 operation is a separate numpy ufunc call, so nothing is fused or reassociated, and the weight sum
+    is taken sequentially in source order."""
+    span = float(np.float32(in1) - np.float32(in0))             # float subtraction, then (double)
+    scale = span / out_size
+    filterscale = max(scale, 1.0)
+    support = 2.0 * filterscale
+    ksize = int(math.ceil(support)) * 2 + 1
+    center = float(np.float32(in0)) + (np.arange(out_size, dtype=np.float64) + 0.5) * scale
+    xmin = np.maximum(np.trunc(center - support + 0.5).astype(np.int64), 0)
+    xmax = np.minimum(np.trunc(center + support + 0.5).astype(np.int64), in_size) - xmin
+    j = np.arange(ksize, dtype=np.int64)
+    w = _bicubic(((j[None, :] + xmin[:, None]) - center[:, None] + 0.5) * (1.0 / filterscale))
+    w = np.where(j[None, :] < xmax[:, None], w, 0.0)
+    ww = np.zeros(out_size, dtype=np.float64)
+    for k in range(ksize):
+        ww = ww + w[:, k]
+    w = np.where(ww[:, None] != 0.0, w / np.where(ww == 0.0, 1.0, ww)[:, None], w)
+    scaled = w * float(1 << _PRECISION_BITS)
+    k32 = np.trunc(np.where(w < 0, -0.5 + scaled, 0.5 + scaled)).astype(np.int32)
+    return np.stack([xmin, xmax], axis=1).astype(np.int32), k32
+
+
+def _pinned_to(a, device):
+    t = torch.from_numpy(np.ascontiguousarray(a)).pin_memory()
+    return t.to(device, non_blocking=True)
+
+
+def image_resample(src, size, boxes=None):
+    """PIL.Image.resize(size, box=box) with the BICUBIC filter, bit for bit, on a batch of uint8 images of one
+    size: `src` is a [B, C, H, W] uint8 CUDA tensor (any memory format; channels-last avoids a copy) or a list of
+    [C, H, W] ones; `size` = (W_out, H_out); `boxes` None (the whole image), (x0, y0, x1, y1) for every image or
+    [B, 4] per image, as C floats.  Returns [B, C, H_out, W_out] uint8 in channels-last memory, the layout of
+    torch.from_numpy(np.stack(arrays)).permute(0, 3, 1, 2).  The coefficient tables are built on the host and
+    uploaded from pinned memory: no synchronisation, unless `boxes` is a CUDA tensor (one device->host read)."""
+    if isinstance(src, (list, tuple)):
+        src = torch.stack(list(src))
+    require_cuda(src)
+    if src.dim() != 4 or src.dtype != torch.uint8:
+        raise TypeError(f"image_resample: expected a [B, C, H, W] uint8 tensor, got {tuple(src.shape)} {src.dtype}")
+    B, C, Hi, Wi = (int(v) for v in src.shape)
+    Wo, Ho = int(size[0]), int(size[1])
+    if Wo < 1 or Ho < 1:
+        raise ValueError(f"image_resample: output size must be positive, got {tuple(size)}")
+    bx = np.broadcast_to(np.asarray([0, 0, Wi, Hi] if boxes is None else
+                                    (boxes.cpu().numpy() if isinstance(boxes, torch.Tensor) else boxes),
+                                    dtype=np.float32), (B, 4))
+    if (bx[:, 0] < 0).any() or (bx[:, 1] < 0).any() or (bx[:, 2] > Wi).any() or (bx[:, 3] > Hi).any():
+        raise ValueError("image_resample: box can't exceed original image size")
+    if (bx[:, 2] <= bx[:, 0]).any() or (bx[:, 3] <= bx[:, 1]).any():
+        raise ValueError("image_resample: box can't be empty")
+    nhwc = src.permute(0, 2, 3, 1).contiguous()
+    out = torch.empty((B, Ho, Wo, C), dtype=torch.uint8, device=src.device)
+    # Pillow runs a pass only when that axis changes; an identity pass reproduces the input exactly, so one
+    # batch-wide decision per axis gives every image Pillow's bytes
+    need_h = bool(((bx[:, 0] != 0) | (bx[:, 2] != Wo)).any()) or Wo != Wi
+    need_v = bool(((bx[:, 1] != 0) | (bx[:, 3] != Ho)).any()) or Ho != Hi
+    if B == 0 or not (need_h or need_v):
+        out.copy_(nhwc)
+        return out.permute(0, 3, 1, 2)
+    shared = bool((bx == bx[:1]).all())
+    rows = bx[:1] if shared else bx
+
+    def tables(n_in, c0, c1, n_out):
+        per = [resample_axis_tables(n_in, r[c0], r[c1], n_out) for r in rows]
+        k = max(t[1].shape[1] for t in per)
+        coef = np.zeros((len(per), n_out, k), dtype=np.int32)
+        for i, t in enumerate(per):
+            coef[i, :, :t[1].shape[1]] = t[1]
+        return np.stack([t[0] for t in per]), coef
+
+    xb, xc = tables(Wi, 0, 2, Wo)
+    yb, yc = tables(Hi, 1, 3, Ho)
+    yfirst, T = None, Ho
+    if need_h and need_v:
+        first = yb[:, 0, 0].copy()
+        T = int((yb[:, -1, 0] + yb[:, -1, 1] - first).max())
+        yb[:, :, 0] -= first[:, None]
+        yfirst = np.broadcast_to(first, (B,)).astype(np.int32)
+    dev = src.device
+    tmp = torch.empty((B, T, Wo, C), dtype=torch.uint8, device=dev) if (need_h and need_v) else None
+    d = lambda a: _pinned_to(a, dev)  # noqa: E731
+    xb_d, xc_d = (d(xb), d(xc)) if need_h else (None, None)
+    yb_d, yc_d = (d(yb), d(yc)) if need_v else (None, None)
+    yf_d = d(yfirst) if yfirst is not None else None
+    lib = _lib.load()
+    with torch.cuda.device(dev):
+        check(lib.dva_resample_u8(ptr(nhwc), ptr(tmp), ptr(out), B, Hi, Wi, C, Ho, Wo, T, ptr(xb_d), ptr(xc_d),
+                                  int(xc.shape[2]), int(not shared), ptr(yb_d), ptr(yc_d), int(yc.shape[2]),
+                                  int(not shared), ptr(yf_d), stream_ptr()), "dva_resample_u8")
+    return out.permute(0, 3, 1, 2)
+
+
+def nonstatic_mask(imgs):
+    """[W, H] bool: True where every channel of some image i >= 1 differs from image 0 (NonStaticMask,
+    data_transform image.py:139-154).  `imgs` [n, C, H, W] uint8 CUDA, n >= 2.  No synchronisation."""
+    require_cuda(imgs)
+    if imgs.dim() != 4 or imgs.dtype != torch.uint8 or imgs.shape[0] < 2:
+        raise TypeError(f"nonstatic_mask: expected [n >= 2, C, H, W] uint8, got {tuple(imgs.shape)} {imgs.dtype}")
+    n, C, H, W = (int(v) for v in imgs.shape)
+    nhwc = imgs.permute(0, 2, 3, 1).contiguous()
+    mask = torch.empty((W, H), dtype=torch.bool, device=imgs.device)
+    lib = _lib.load()
+    with torch.cuda.device(imgs.device):
+        check(lib.dva_nonstatic_mask(ptr(nhwc), n, H, W, C, ptr(mask), stream_ptr()), "dva_nonstatic_mask")
+    return mask

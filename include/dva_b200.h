@@ -460,6 +460,26 @@ int dva_coverage_index(const int64_t* gimg, const int64_t* vpoint, int64_t V, in
 int dva_coverage_pick(int64_t g, int64_t V, int64_t n_img, int64_t N, int32_t* unseen, int32_t* seen,
                       const void* workspace, size_t workspace_bytes, void* stream);
 
+/* I1  Pillow-exact image resize                 replaces PIL.Image.resize(size, box=...) (BICUBIC, 8 bits) of
+ *   SameSettingImageData.read_images (image.py:1061, :1093).  in [B, Hi, Wi, C] uint8 (channels-last, 1 <= C <= 4),
+ *   out [B, Ho, Wo, C] uint8.  Tables from the caller: bounds [n_out, 2] int32 = (first source index, count) and
+ *   coef [n_out, k] int32 weights scaled by 2^22 (Pillow's precompute_coeffs + normalize_coeffs_8bpc), shared by
+ *   all images or per image (x_per_image / y_per_image: [B, n_out, ...]).  Horizontal pass (xcoef non-null):
+ *   tmp[b, t, x] over source rows yfirst[b] + t, t < T (rows >= Hi skipped; yfirst nullable: 0); the vertical
+ *   bounds are then relative to yfirst[b].  Vertical pass (ycoef non-null) reads tmp [B, T, Wo, C], or `in`
+ *   when there is no horizontal pass (Wo == Wi); with no vertical pass the horizontal one writes `out` (T == Ho).
+ *   Every sum starts at 2^21, accumulates in int32, is shifted right by 22 and clamped to [0, 255] (uint8
+ *   between the passes, as Pillow clips).  Integer only: the result does not depend on the launch. */
+int dva_resample_u8(const uint8_t* in, uint8_t* tmp, uint8_t* out, int64_t B, int64_t Hi, int64_t Wi, int64_t C,
+                    int64_t Ho, int64_t Wo, int64_t T, const int32_t* xbounds, const int32_t* xcoef, int64_t kx,
+                    int x_per_image, const int32_t* ybounds, const int32_t* ycoef, int64_t ky, int y_per_image,
+                    const int32_t* yfirst, void* stream);
+
+/* I2  non-static pixel mask                     replaces the per-image comparison loop of NonStaticMask
+ *   (data_transform image.py:139-154).  imgs [n, H, W, C] uint8 channels-last, n >= 2; mask [W, H] bytes 0 / 1 (a torch.bool buffer):
+ *     mask[x, y] = OR over i >= 1 of AND over c of (imgs[i, y, x, c] != imgs[0, y, x, c]) */
+int dva_nonstatic_mask(const uint8_t* imgs, int64_t n, int64_t H, int64_t W, int64_t C, uint8_t* mask, void* stream);
+
 /* C1  CSR pointers from sorted dense ids     replaces csr.py:158-172 + :197-229
  *   ids [n] int64 sorted ascending, values in [0,num_groups) -> ptr [num_groups+1] int64 with
  *   empty groups inserted (from_dense + insert_empty_groups, image.py:1787-1793). */
