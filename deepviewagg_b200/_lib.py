@@ -101,6 +101,10 @@ SIGNATURES = {
     "dva_resample_u8": (_i32, [_vp, _vp, _vp, _i64, _i64, _i64, _i64, _i64, _i64, _i64, _vp, _vp, _i64, _i32, _vp,
                                 _vp, _i64, _i32, _vp, _vp]),
     "dva_nonstatic_mask": (_i32, [_vp, _i64, _i64, _i64, _i64, _vp, _vp]),
+    "dva_color_jitter_u8_workspace_bytes": (_sz, [_i64]),
+    "dva_color_jitter_u8": (_i32, [_vp, _vp, _i64, _i64, _i64, _i32, _i32, _i32, _f32, _f32, _f32, _f32, _f32, _f32,
+                                   _vp, _sz, _vp]),
+    "dva_image_to_float": (_i32, [_vp, _i32, _vp, _i64, _i64, _i64, _i64, _i32] + [_f32] * 8 + [_vp]),
     "dva_csr_pointers_from_sorted": (_i32, [_vp, _vp, _i64, _i64, _vp]),
     "dva_csr_select_values": (_i32, [_vp, _vp, _vp, _vp, _i64, _i64, _vp]),
 }

@@ -4,19 +4,20 @@ between loading a sample and the forward pass, and the two that open every confi
 (LoadImages -> NonStaticMask -> MapImages -> NeighborhoodBasedMappingFeatures):
 
   LoadImages -> NonStaticMask
-  SelectMappingFromPointId -> CenterRoll -> PickImagesFromMappingArea -> CropImageGroups
-    -> PickImagesFromMemoryCredit -> JitterMappingFeatures -> RandomHorizontalFlip
+  ToImageData -> SelectMappingFromPointId -> CenterRoll -> PickImagesFromMappingArea -> CropImageGroups
+    -> PickImagesFromMemoryCredit -> JitterMappingFeatures -> ColorJitter -> RandomHorizontalFlip
+    -> ToFloatImage -> Normalize
 
 Every transform is called as `data, images = T(data, images)`.  `data` is duck-typed: the mapping key is an
 attribute (`data.mapping_index`) and the point count is `data.num_nodes` or `data.pos.shape[0]`, so a PyG
 `Data` and a `types.SimpleNamespace` both work.  Containers on CUDA run the kernels of
-csrc/image_transforms.cu (no fallback); containers on the CPU (data-loader workers) run a torch restatement
-of the same arithmetic.  Both give the reference's result bit for bit, including its random draws: the
-draws are made on the CPU generators (torch and numpy) exactly as the reference makes them.
+csrc/image_transforms.cu and csrc/image_color.cu (no fallback); containers on the CPU (data-loader workers) run
+a torch restatement of the same arithmetic.  Both give the reference's result bit for bit, including its random
+draws: the draws are made on the CPU generators (torch and numpy) exactly as the reference makes them.  The one
+exception is ColorJitter's contrast mean, which is exact here (see ColorJitter).
 
-Each docstring lists the host synchronisations of the CUDA path.  Intrinsics are not adjusted, `rollings`
-are not persisted by storage.py, and ColorJitter / ToFloatImage / Normalize are plain element-wise ops that
-apply to `images.x` directly.
+Each docstring lists the host synchronisations of the CUDA path.  Intrinsics are not adjusted and `rollings`
+are not persisted by storage.py.  The colour transforms keep the memory format of `images.x`.
 """
 import copy
 
@@ -462,4 +463,135 @@ class RandomHorizontalFlip(ImageTransform):
                 pix[:, 0] = width - 1 - pix[:, 0]
                 m.pixels = pix
                 images.mappings = m
+        return data, images
+
+
+class ToImageData(ImageTransform):
+    """Wrap a SameSettingImageData into ImageData([images]) (image.py:64-68).  An ImageData input comes back as
+    the same settings in one flat ImageData."""
+
+    def _process(self, data, images):
+        return data, ImageData([images])
+
+
+def _jitter_range(value, name):
+    """torchvision ColorJitter._check_input for a scalar: [max(0, 1 - v), 1 + v], None (no draw, no op) when v == 0"""
+    if value < 0:
+        raise ValueError(f"If {name} is a single number, it must be non negative.")
+    lo, hi = max(1.0 - float(value), 0.0), 1.0 + float(value)
+    return None if lo == hi == 1.0 else (lo, hi)
+
+
+def _gray_u8(x):
+    """torchvision rgb_to_grayscale on [B, 3, H, W] uint8: (0.2989 r + 0.587 g) + 0.114 b in fp32, truncated"""
+    r, g, b = x.unbind(dim=-3)
+    return (0.2989 * r + 0.587 * g + 0.114 * b).to(torch.uint8).unsqueeze(-3)
+
+
+def _blend_u8(img, other, ratio):
+    """torchvision _blend for uint8: fp32(ratio) * img + fp32(1 - ratio) * other, clamped to [0, 255], truncated"""
+    return (ratio * img + (1.0 - ratio) * other).clamp(0, 255).to(torch.uint8)
+
+
+def color_jitter_torch(x, ops_seq):
+    """torch restatement of dva_color_jitter_u8 (the CPU path; on CUDA tensors the multi-pass chain a user would
+    write): the ops of `ops_seq` ((name, factor) in the drawn order) on a [B, 3, H, W] uint8 tensor, with the
+    exact contrast mean fp32(float64(S) / float64(H W)) of the integer grayscale sum S.  Keeps x's memory format."""
+    fmt = ops._memory_format(x)
+    HW = x.shape[-1] * x.shape[-2]
+    for name, f in ops_seq:
+        if name == "brightness":
+            x = _blend_u8(x, torch.zeros_like(x), f)
+        elif name == "saturation":
+            x = _blend_u8(x, _gray_u8(x), f)
+        else:
+            s = _gray_u8(x).sum(dim=(1, 2, 3), dtype=torch.int64).double()
+            mean = (s / torch.full_like(s, float(HW))).float().view(-1, 1, 1, 1)      # true division on any device
+            x = _blend_u8(x, mean, f)
+    return x.contiguous(memory_format=fmt)
+
+
+class ColorJitter(ImageTransform):
+    """Randomly change the brightness, contrast and saturation of `images.x` (image.py:1249-1259), restating
+    torchvision's ColorJitter without depending on it.  Ranges are [max(0, 1 - v), 1 + v] (off when v == 0);
+    the draw is torchvision's get_params on the CPU default generator: torch.randperm(4), then one
+    uniform_(lo, hi) each for brightness, contrast and saturation, in that order, for the ones that are on.  The
+    ops run in the drawn order with torchvision's uint8 arithmetic (fp32 blends truncated to uint8 after every
+    op).  Each setting of an ImageData gets its own draw; a setting without images consumes its draw too.
+
+    `images.x` must be [B, 3, H, W] uint8 (ColorJitter comes before ToFloatImage in every config).  One
+    deliberate difference: the contrast mean is float32(float64(S) / float64(H W)) of the exact integer sum S of
+    the grayscale bytes, where torchvision's fp32 torch.mean depends on the reduction order and may be an ulp
+    away; a pixel can then differ by 1 where its blend value lies within that shift of an integer.
+    CUDA: dva_color_jitter_u8 (one pass, or two with contrast).  Syncs: none."""
+
+    def __init__(self, brightness=0, contrast=0, saturation=0):
+        self.brightness = brightness
+        self.contrast = contrast
+        self.saturation = saturation
+        self._ranges = (_jitter_range(brightness, "brightness"), _jitter_range(contrast, "contrast"),
+                        _jitter_range(saturation, "saturation"))
+
+    def get_params(self):
+        """(fn_idx [4] int64, [(name, factor) of the active ops in the drawn order])"""
+        fn_idx = torch.randperm(4)
+        factors = [None if r is None else float(torch.empty(1).uniform_(r[0], r[1])) for r in self._ranges]
+        names = ("brightness", "contrast", "saturation")
+        return fn_idx, [(names[i], factors[i]) for i in fn_idx.tolist() if i < 3 and factors[i] is not None]
+
+    def _process(self, data, images):
+        x = images.x
+        if x is None or x.dim() != 4 or x.shape[1] != 3 or x.dtype != torch.uint8:
+            got = None if x is None else (tuple(x.shape), x.dtype)
+            raise TypeError(f"ColorJitter expects images.x as a [B, 3, H, W] uint8 tensor, got {got}")
+        _, seq = self.get_params()
+        if x.shape[0] == 0 or len(seq) == 0:
+            return data, images
+        images.x = ops.color_jitter_u8(x, seq) if x.is_cuda else color_jitter_torch(x, seq)
+        return data, images
+
+    def __repr__(self):
+        return (f"{self.__class__.__name__}(brightness={self.brightness}, contrast={self.contrast}, "
+                f"saturation={self.saturation})")
+
+
+class ToFloatImage(ImageTransform):
+    """[0, 255] uint8 images to [0, 1] fp32: x.float() / 255 with true division, as on the CPU
+    (image.py:1221-1232); loads the images first when `x` is None.  CUDA: dva_image_to_float, for uint8 or
+    fp32 `x` (a CUDA division by a Python scalar would multiply by the reciprocal).  Syncs: none."""
+
+    def _process(self, data, images):
+        if images.x is None:
+            images.load()
+        x = images.x
+        if x.is_cuda:
+            images.x = ops.image_to_float(x)
+        else:
+            images.x = (x.float() / 255).contiguous(memory_format=ops._memory_format(x))
+        return data, images
+
+
+class Normalize(ImageTransform):
+    """(x - mean_c) / std_c with true division (image.py:1271-1282): torchvision's normalize, sub_(mean).div_(std)
+    with [C, 1, 1] tensors of x's dtype.  Non-float `x` raises a TypeError, as in torchvision.  CUDA:
+    dva_image_to_float with the statistics passed by value, fp32 `x` with 1 to 4 channels.  Syncs: none."""
+
+    def __init__(self, mean=[0.485, 0.456, 0.406], std=[0.229, 0.224, 0.225]):
+        self.mean = mean
+        self.std = std
+
+    def _process(self, data, images):
+        x = images.x
+        if x is None or not torch.is_floating_point(x):
+            raise TypeError(f"Input tensor should be a float tensor. Got {None if x is None else x.dtype}.")
+        if x.is_cuda and x.dtype != torch.float32:
+            raise TypeError(f"Normalize on CUDA runs on float32 images, got {x.dtype}")
+        std = torch.as_tensor(self.std, dtype=x.dtype)
+        if (std == 0).any():
+            raise ValueError(f"std evaluated to zero after conversion to {x.dtype}, leading to division by zero.")
+        if x.is_cuda:
+            images.x = ops.image_to_float(x, self.mean, self.std)
+        else:
+            mean = torch.as_tensor(self.mean, dtype=x.dtype).view(-1, 1, 1)
+            images.x = ((x - mean) / std.view(-1, 1, 1)).contiguous(memory_format=ops._memory_format(x))
         return data, images

@@ -1118,3 +1118,78 @@ def nonstatic_mask(imgs):
     with torch.cuda.device(imgs.device):
         check(lib.dva_nonstatic_mask(ptr(nhwc), n, H, W, C, ptr(mask), stream_ptr()), "dva_nonstatic_mask")
     return mask
+
+
+# --------------------------------------------------------------------------------------------
+# colour transforms (ColorJitter, ToFloatImage, Normalize): torchvision's tensor arithmetic
+# (csrc/image_color.cu)
+# --------------------------------------------------------------------------------------------
+_JITTER_CODES = {"brightness": 0, "contrast": 1, "saturation": 2}
+
+
+def _memory_format(x):
+    """channels_last when x is channels-last and not also contiguous (C == 1 or H == W == 1), else contiguous"""
+    cl = (not x.is_contiguous()) and x.is_contiguous(memory_format=torch.channels_last)
+    return torch.channels_last if cl else torch.contiguous_format
+
+
+def color_jitter_u8(x, ops_seq):
+    """torchvision's ColorJitter for drawn factors on a [B, 3, H, W] uint8 CUDA tensor (NCHW or channels-last; the
+    output keeps x's memory format).  `ops_seq`: the active ops in the drawn order, as (name, factor) pairs with
+    name in 'brightness' / 'contrast' / 'saturation'.  The contrast mean is exact (csrc/image_color.cu).  No
+    synchronisation."""
+    require_cuda(x)
+    if x.dim() != 4 or x.shape[1] != 3 or x.dtype != torch.uint8:
+        raise TypeError(f"color_jitter_u8: expected a [B, 3, H, W] uint8 tensor, got {tuple(x.shape)} {x.dtype}")
+    if len(ops_seq) > 3:
+        raise ValueError("color_jitter_u8: at most three ops")
+    fmt = _memory_format(x)
+    x = x.contiguous(memory_format=fmt)
+    out = torch.empty_like(x, memory_format=fmt)
+    codes, args = 0, []
+    for i, (name, factor) in enumerate(ops_seq):
+        codes |= _JITTER_CODES[name] << (4 * i)
+        args += [float(factor), float(1.0 - float(factor))]   # 1 - ratio in float64, rounded to fp32 by ctypes
+    args += [0.0, 0.0] * (3 - len(ops_seq))
+    B, _, H, W = (int(v) for v in x.shape)
+    lib = _lib.load()
+    ws_bytes = int(lib.dva_color_jitter_u8_workspace_bytes(B))
+    ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=x.device)
+    with torch.cuda.device(x.device):
+        check(lib.dva_color_jitter_u8(ptr(x), ptr(out), B, H, W, int(fmt == torch.channels_last), len(ops_seq), codes,
+                                      *args, ptr(ws), ws_bytes, stream_ptr()), "dva_color_jitter_u8")
+    return out
+
+
+def image_to_float(x, mean=None, std=None):
+    """(x - mean_c) / std_c in fp32 with true division on a [B, C, H, W] CUDA tensor, 1 <= C <= 4, NCHW or
+    channels-last (kept).  x uint8 with mean = std = None is ToFloatImage (x.float() / 255 as on the CPU); x fp32
+    with per-channel mean / std (sequences of C floats, or of 1 for all channels) is Normalize.  The statistics are
+    rounded to fp32 and passed by value: no copy to the device, no synchronisation."""
+    require_cuda(x)
+    if x.dim() != 4 or x.dtype not in (torch.uint8, torch.float32):
+        raise TypeError(f"image_to_float: expected a [B, C, H, W] uint8 or float32 tensor, got {tuple(x.shape)} "
+                        f"{x.dtype}")
+    C = int(x.shape[1])
+    if not 1 <= C <= 4:
+        raise TypeError(f"image_to_float: 1 to 4 channels, got {C}")
+    if mean is None:
+        mean, std = [0.0], [255.0]
+
+    def per_channel(v, what):
+        v = [float(a) for a in (v.tolist() if isinstance(v, torch.Tensor) else v)]
+        if len(v) == 1:
+            v = v * C
+        if len(v) != C:
+            raise ValueError(f"image_to_float: {what} has {len(v)} values for {C} channels")
+        return v + [1.0] * (4 - C)
+    m, s = per_channel(mean, "mean"), per_channel(std, "std")
+    fmt = _memory_format(x)
+    x = x.contiguous(memory_format=fmt)
+    out = torch.empty(x.shape, dtype=torch.float32, device=x.device, memory_format=fmt)
+    B, _, H, W = (int(v) for v in x.shape)
+    lib = _lib.load()
+    with torch.cuda.device(x.device):
+        check(lib.dva_image_to_float(ptr(x), int(x.dtype == torch.uint8), ptr(out), B, C, H, W,
+                                     int(fmt == torch.channels_last), *m, *s, stream_ptr()), "dva_image_to_float")
+    return out

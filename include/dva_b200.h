@@ -480,6 +480,34 @@ int dva_resample_u8(const uint8_t* in, uint8_t* tmp, uint8_t* out, int64_t B, in
  *     mask[x, y] = OR over i >= 1 of AND over c of (imgs[i, y, x, c] != imgs[0, y, x, c]) */
 int dva_nonstatic_mask(const uint8_t* imgs, int64_t n, int64_t H, int64_t W, int64_t C, uint8_t* mask, void* stream);
 
+/* I3  colour jitter on uint8 images             replaces torchvision's ColorJitter.forward as the reference's
+ *   ColorJitter calls it (data_transform image.py:1249-1259), i.e. _functional_tensor.adjust_brightness /
+ *   adjust_contrast / adjust_saturation over _blend and rgb_to_grayscale, for drawn factors (no hue).
+ *   in, out [B, 3, H, W] uint8, both NCHW or both channels-last (channels_last != 0), any H and W.  Ops i < n_ops
+ *   (0 <= n_ops <= 3) in that order, op code i in bits 4i..4i+3 of op_codes (0 brightness, 1 contrast,
+ *   2 saturation, each at most once), factor ratio_i >= 0 and rest_i = fp32(1 - ratio_i) (float64 subtraction).
+ *   Per op and channel, in fp32 without contraction:
+ *     v' = trunc(clamp(ratio * v + rest * o, 0, 255)),  o = 0 (brightness), the pixel's grayscale (saturation),
+ *     or the image's contrast mean;  grayscale = trunc((0.2989 r + 0.587 g) + 0.114 b).
+ *   Contrast mean = fp32(double(S) / double(H W)), S the exact sum of the grayscale bytes of the image after the
+ *   ops before contrast (torchvision's fp32 torch.mean may differ by an ulp).  With contrast, a first pass sums S
+ *   into the workspace (dva_color_jitter_u8_workspace_bytes(B) bytes, zeroed on the stream by the call); the apply
+ *   pass reads it on the device.  Integer sums: the result does not depend on the launch. */
+size_t dva_color_jitter_u8_workspace_bytes(int64_t B);
+int dva_color_jitter_u8(const uint8_t* in, uint8_t* out, int64_t B, int64_t H, int64_t W, int channels_last,
+                        int n_ops, int op_codes, float ratio0, float rest0, float ratio1, float rest1, float ratio2,
+                        float rest2, void* workspace, size_t workspace_bytes, void* stream);
+
+/* I4  ToFloatImage / Normalize                   replaces `images.x.float() / 255` (data_transform
+ *   image.py:1221-1232) and torchvision's _functional_tensor.normalize, `sub_(mean).div_(std)` with fp32
+ *   [C, 1, 1] tensors, as the reference's Normalize calls it (:1271-1282).  in [B, C, H, W] uint8 (in_u8 != 0)
+ *   or fp32, out [B, C, H, W] fp32, both NCHW or both channels-last, 1 <= C <= 4:
+ *     out = (fp32(in) - m_c) / s_c   with true division (ToFloatImage: m_c = 0, s_c = 255).
+ *   The channel statistics are passed by value (unused ones ignored): no copy to the device. */
+int dva_image_to_float(const void* in, int in_u8, float* out, int64_t B, int64_t C, int64_t H, int64_t W,
+                       int channels_last, float m0, float m1, float m2, float m3, float s0, float s1, float s2,
+                       float s3, void* stream);
+
 /* C1  CSR pointers from sorted dense ids     replaces csr.py:158-172 + :197-229
  *   ids [n] int64 sorted ascending, values in [0,num_groups) -> ptr [num_groups+1] int64 with
  *   empty groups inserted (from_dense + insert_empty_groups, image.py:1787-1793). */
