@@ -166,6 +166,24 @@ def stream_ptr(device=None):
     return ctypes.c_void_p(torch.cuda.current_stream(device).cuda_stream)
 
 
+def launch(name, device, *args):
+    """Run the entry point `name` on `device`'s current stream, raising like check().
+
+    Every entry point that launches work takes its stream last; it is appended here.  Tensors are
+    passed as their device pointer and None as NULL.  `args` holds every tensor, temporaries made in
+    the caller's argument list included, until the call returns: a temporary freed before the call
+    would hand its block to the next one, and two arguments would alias."""
+    fn = getattr(load(), name)
+    with torch.cuda.device(device):
+        check(fn(*[ptr(a) if isinstance(a, torch.Tensor) else a for a in args], stream_ptr()), name)
+
+
+def workspace(nbytes, device):
+    """Scratch buffer of at least `nbytes` bytes, passed on as (ws, ws.numel()).  Never empty, so its
+    pointer is never NULL, which most entry points reject even when they need no scratch."""
+    return torch.empty(max(int(nbytes), 1), dtype=torch.uint8, device=device)
+
+
 def require_cuda(*tensors):
     for t in tensors:
         if t is not None and not t.is_cuda:

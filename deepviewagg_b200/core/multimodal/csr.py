@@ -20,11 +20,8 @@ def pointers_from_sorted(ids, num_groups):
     ids = ids.long().contiguous()
     n = ids.numel()
     if ids.is_cuda:
-        lib = _lib.load()
         ptr = torch.empty(num_groups + 1, dtype=torch.long, device=ids.device)
-        with torch.cuda.device(ids.device):
-            _lib.check(lib.dva_csr_pointers_from_sorted(_lib.ptr(ids), _lib.ptr(ptr), n, num_groups,
-                                                        _lib.stream_ptr()), "dva_csr_pointers_from_sorted")
+        _lib.launch("dva_csr_pointers_from_sorted", ids.device, ids, ptr, n, num_groups)
         return ptr
     return torch.searchsorted(ids, torch.arange(num_groups + 1, dtype=torch.long))
 
@@ -35,12 +32,9 @@ def select_values(pointers, sel):
     pn = torch.cat([torch.zeros(1, dtype=torch.long, device=pointers.device), torch.cumsum(sizes, 0)])
     n_new = int(pn[-1].item())
     if pointers.is_cuda:
-        lib = _lib.load()
         val = torch.empty(n_new, dtype=torch.long, device=pointers.device)
-        p, s = pointers.contiguous(), sel.contiguous()
-        with torch.cuda.device(pointers.device):
-            _lib.check(lib.dva_csr_select_values(_lib.ptr(p), _lib.ptr(s), _lib.ptr(pn), _lib.ptr(val),
-                                                 s.numel(), n_new, _lib.stream_ptr()), "dva_csr_select_values")
+        _lib.launch("dva_csr_select_values", pointers.device, pointers.contiguous(), sel.contiguous(), pn, val,
+                    sel.numel(), n_new)
         return pn, val
     val = torch.arange(n_new) - pn[:-1].repeat_interleave(sizes) + pointers[sel].repeat_interleave(sizes)
     return pn, val

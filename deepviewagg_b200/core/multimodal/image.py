@@ -33,7 +33,6 @@ def _native_mapping_build(point_ids, image_ids, pixels, features, num_points, fe
     point's items with a warp rank sort on (image[, x, y], source index), cut views / dedupe pixels,
     average the view features -- all on the current stream, ONE device->host read (the output sizes).
     Returns an ImageMapping."""
-    lib = _lib.load()
     dev = point_ids.device
     n = int(point_ids.shape[0])
     if pixels.dtype not in _PIX_CODES:
@@ -50,18 +49,14 @@ def _native_mapping_build(point_ids, image_ids, pixels, features, num_points, fe
     pixels_out = torch.empty_like(pixels)
     feat_out = torch.empty((n, F), dtype=torch.float32, device=dev) if feat is not None else None
     counts = torch.empty(3, dtype=torch.long, device=dev)
-    ws_bytes = int(lib.dva_mapping_build_workspace_bytes(n, num_points))
-    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+    ws = _lib.workspace(_lib.load().dva_mapping_build_workspace_bytes(n, num_points), dev)
     if feat_on is not None:
         feat_on = feat_on.to(torch.uint8).contiguous()
     if feat_row is not None:
         feat_row = feat_row.long().contiguous()
-    with torch.cuda.device(dev):
-        _lib.check(lib.dva_mapping_build(
-            _lib.ptr(point_ids), _lib.ptr(image_ids), _lib.ptr(pixels), _PIX_CODES[pixels.dtype], _lib.ptr(feat),
-            _lib.ptr(feat_row), _lib.ptr(feat_on), F, n, int(num_points), int(bool(dedupe)), _lib.ptr(view_ptr),
-            _lib.ptr(images_out), _lib.ptr(atomic_ptr), _lib.ptr(pixels_out), _lib.ptr(feat_out), None,
-            _lib.ptr(counts), _lib.ptr(ws), ws_bytes, _lib.stream_ptr()), "dva_mapping_build")
+    _lib.launch("dva_mapping_build", dev, point_ids, image_ids, pixels, _PIX_CODES[pixels.dtype], feat, feat_row,
+                feat_on, F, n, int(num_points), int(bool(dedupe)), view_ptr, images_out, atomic_ptr, pixels_out,
+                feat_out, None, counts, ws, ws.numel())
     V, P, status = counts.tolist()                           # the only synchronisation
     if status != 0:
         raise IndexError("from_dense: point ids outside [0, num_points)")
@@ -916,7 +911,6 @@ class ImageData:
     def _view_cat_native(self):
         """(sorting, csr_cat) in closed form (dva_view_cat_sorting): every setting's views are already
         grouped by point, so a view's slot in the merged order is a sum of pointers -- no sort."""
-        lib = _lib.load()
         ptrs = [im.view_csr_indexing.contiguous() for im in self]
         N = int(ptrs[0].numel()) - 1
         sizes = [int(im.mappings.images.shape[0]) if im.mappings is not None else 0 for im in self]
@@ -928,10 +922,8 @@ class ImageData:
         table = torch.tensor([p.data_ptr() for p in ptrs] + bases, dtype=torch.long).to(dev)
         sorting = torch.empty(tot, dtype=torch.long, device=dev)
         csr_cat = torch.empty(N + 1, dtype=torch.long, device=dev)
-        with torch.cuda.device(dev):
-            _lib.check(lib.dva_view_cat_sorting(_lib.ptr(table), table.data_ptr() + 8 * len(ptrs), len(ptrs), N,
-                                                _lib.ptr(sorting), _lib.ptr(csr_cat), _lib.stream_ptr()),
-                       "dva_view_cat_sorting")
+        _lib.launch("dva_view_cat_sorting", dev, table, table.data_ptr() + 8 * len(ptrs), len(ptrs), N, sorting,
+                    csr_cat)
         return sorting, csr_cat
 
     @property

@@ -139,12 +139,10 @@ def knn_grid(pos, k, cell_size=None, return_dist2=False):
     Squared distances are (dx*dx + dy*dy) + dz*dz in fp32, ties ordered by point index; points
     with z = 0 give the exact 2D distance (image-plane search).  Returns neighbors [N,k] int64
     (ascending distance) and optionally the squared distances."""
-    from ... import _lib
-    from ..._lib import check, ptr, stream_ptr
+    from ..._lib import launch
     from .csr import pointers_from_sorted
     if not pos.is_cuda:
         raise RuntimeError("knn_grid runs on CUDA tensors only (no CPU fallback)")
-    lib = _lib.load()
     pos = pos.float().contiguous()
     n = pos.shape[0]
     if not 1 <= k <= 128:
@@ -155,9 +153,7 @@ def knn_grid(pos, k, cell_size=None, return_dist2=False):
 
     def assign(cs):
         lo, dims, cs = _grid_for(pos, cs)
-        with torch.cuda.device(pos.device):
-            check(lib.dva_knn_cell_ids(ptr(pos), ptr(cell), n, lo[0], lo[1], lo[2], cs, dims[0], dims[1], dims[2],
-                                       stream_ptr(pos.device)), "dva_knn_cell_ids")
+        launch("dva_knn_cell_ids", pos.device, pos, cell, n, lo[0], lo[1], lo[2], cs, dims[0], dims[1], dims[2])
         return lo, dims, cs
 
     if cell_size is None:
@@ -187,10 +183,8 @@ def knn_grid(pos, k, cell_size=None, return_dist2=False):
     xyz_s = pos[order].contiguous()
     nbr = torch.empty((n, k), dtype=torch.int64, device=pos.device)
     d2 = torch.empty((n, k), dtype=torch.float32, device=pos.device) if return_dist2 else None
-    with torch.cuda.device(pos.device):
-        check(lib.dva_knn_grid(ptr(xyz_s), ptr(cell_s), ptr(order), ptr(cell_ptr), n, k, lo[0], lo[1], lo[2],
-                               cell_size, dims[0], dims[1], dims[2], ptr(nbr), ptr(d2), stream_ptr(pos.device)),
-              "dva_knn_grid")
+    launch("dva_knn_grid", pos.device, xyz_s, cell_s, order, cell_ptr, n, k, lo[0], lo[1], lo[2], cell_size, dims[0],
+           dims[1], dims[2], nbr, d2)
     return (nbr, d2) if return_dist2 else nbr
 
 
@@ -215,8 +209,7 @@ class NeighborhoodBasedMappingFeatures:
     def __call__(self, pos, images: SameSettingImageData, device='cuda', neighbors=None):
         """pos [N,3] (row i = point i of `images.mappings`); returns `images` with the new columns
         appended to `images.mappings.features` (on the mappings' device)."""
-        from ... import _lib
-        from ..._lib import check, ptr, stream_ptr
+        from ..._lib import launch
         assert images.mappings is not None
         maps = images.mappings
         in_device = maps.pointers.device
@@ -235,12 +228,8 @@ class NeighborhoodBasedMappingFeatures:
         width = nk * (int(self.compute_density) + int(self.compute_occlusion))
         out = torch.empty((V, width), dtype=torch.float32, device=dev)
         klist = torch.tensor(self.k_list, dtype=torch.int32, device=dev)
-        lib = _lib.load()
-        with torch.cuda.device(dev):
-            check(lib.dva_neighborhood_features(ptr(xyz), ptr(neighbors), kmax, ptr(vptr), ptr(img), ptr(view_point),
-                                                ptr(klist), nk, float(self.voxel), int(self.compute_density),
-                                                int(self.compute_occlusion), ptr(out), n, V, stream_ptr(dev)),
-                  "dva_neighborhood_features")
+        launch("dva_neighborhood_features", dev, xyz, neighbors, kmax, vptr, img, view_point, klist, nk,
+               float(self.voxel), int(self.compute_density), int(self.compute_occlusion), out, n, V)
         out = out.to(in_device)
         maps.features = out if not maps.has_features else torch.cat([maps.features, out], dim=1)
         return images

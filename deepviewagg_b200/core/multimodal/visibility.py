@@ -20,13 +20,10 @@ csrc/knn_features.cu (mapping.knn_grid) for the image-plane neighbours of the Bi
 Compaction of the kept set / winner map is index plumbing (torch.nonzero); the Biasutti
 contrast and the depth-map test are O(n k) / O(n) gathers and comparisons in torch.
 """
-import ctypes
-
 import numpy as np
 import torch
 
-from ... import _lib
-from ..._lib import check, ptr, require_cuda, stream_ptr
+from ..._lib import launch, require_cuda
 
 _PINHOLE_CAMERAS = ("scannet", "kitti360_perspective")
 
@@ -87,7 +84,6 @@ def camera_projection(xyz, img_xyz, img_opk=None, img_intrinsic_pinhole=None, im
     (visibility.py:478-538).  Cameras: s3dis_equirectangular, scannet, kitti360_perspective,
     kitti360_fisheye."""
     require_cuda(xyz)
-    lib = _lib.load()
     dev = xyz.device
     xyz = xyz.float().contiguous()
     n = xyz.shape[0]
@@ -97,32 +93,28 @@ def camera_projection(xyz, img_xyz, img_opk=None, img_intrinsic_pinhole=None, im
     y_proj = torch.empty(n, dtype=torch.float64, device=dev)
     keep = torch.empty(n, dtype=torch.uint8, device=dev)
     cam_xyz = _host_f32(img_xyz, 3)
-    with torch.cuda.device(dev):
-        if camera == 's3dis_equirectangular':
-            rot = pose_to_rotation_matrix(img_opk if img_opk is not None else np.zeros(3, np.float32))
-            pose = torch.from_numpy(np.concatenate([cam_xyz, rot.numpy().reshape(-1)])).to(dev)
-            check(lib.dva_project_equirectangular(ptr(xyz), ptr(pose), ptr(dist), ptr(x_proj), ptr(y_proj),
-                                                  ptr(keep), n, W, H, int(crop_top), int(crop_bottom),
-                                                  float(r_min), float(r_max), stream_ptr()),
-                  "dva_project_equirectangular")
-        elif camera in _PINHOLE_CAMERAS or camera == 'kitti360_fisheye':
-            A, t0, t1 = _camera_transform(camera, img_extrinsic)
-            intr = np.zeros(8, np.float32)
-            if camera == 'kitti360_fisheye':
-                intr[:7] = _host_f32(img_intrinsic_fisheye, 7)
-                code = 3
-            else:
-                K = img_intrinsic_pinhole.detach().cpu().numpy() if isinstance(img_intrinsic_pinhole, torch.Tensor) \
-                    else np.asarray(img_intrinsic_pinhole)
-                K = np.asarray(K, dtype=np.float32)
-                intr[:4] = [K[0, 0], K[1, 1], K[0, 2], K[1, 2]]
-                code = 1
-            cam = torch.from_numpy(np.concatenate([cam_xyz, A.reshape(-1), t0, t1, intr]).astype(np.float32)).to(dev)
-            check(lib.dva_project_camera(ptr(xyz), ptr(cam), code, ptr(dist), ptr(x_proj), ptr(y_proj), ptr(keep),
-                                         n, W, H, int(crop_top), int(crop_bottom), float(r_min), float(r_max),
-                                         stream_ptr()), "dva_project_camera")
+    if camera == 's3dis_equirectangular':
+        rot = pose_to_rotation_matrix(img_opk if img_opk is not None else np.zeros(3, np.float32))
+        pose = torch.from_numpy(np.concatenate([cam_xyz, rot.numpy().reshape(-1)])).to(dev)
+        launch("dva_project_equirectangular", dev, xyz, pose, dist, x_proj, y_proj, keep, n, W, H, int(crop_top),
+               int(crop_bottom), float(r_min), float(r_max))
+    elif camera in _PINHOLE_CAMERAS or camera == 'kitti360_fisheye':
+        A, t0, t1 = _camera_transform(camera, img_extrinsic)
+        intr = np.zeros(8, np.float32)
+        if camera == 'kitti360_fisheye':
+            intr[:7] = _host_f32(img_intrinsic_fisheye, 7)
+            code = 3
         else:
-            raise ValueError(f"unknown camera '{camera}'")
+            K = img_intrinsic_pinhole.detach().cpu().numpy() if isinstance(img_intrinsic_pinhole, torch.Tensor) \
+                else np.asarray(img_intrinsic_pinhole)
+            K = np.asarray(K, dtype=np.float32)
+            intr[:4] = [K[0, 0], K[1, 1], K[0, 2], K[1, 2]]
+            code = 1
+        cam = torch.from_numpy(np.concatenate([cam_xyz, A.reshape(-1), t0, t1, intr]).astype(np.float32)).to(dev)
+        launch("dva_project_camera", dev, xyz, cam, code, dist, x_proj, y_proj, keep, n, W, H, int(crop_top),
+               int(crop_bottom), float(r_min), float(r_max))
+    else:
+        raise ValueError(f"unknown camera '{camera}'")
     if img_mask is not None:  # field_of_view_cpu: img_mask[floor(x), floor(y)] (visibility.py:428-434)
         assert tuple(img_mask.shape) == (W, H), \
             f'Expected img_mask to be a torch.BoolTensor of shape img_size={img_size} but got size={img_mask.shape}.'
@@ -135,7 +127,6 @@ def camera_projection(xyz, img_xyz, img_opk=None, img_intrinsic_pinhole=None, im
 
 def _project_raw(xyz, camera, img_extrinsic, intr8, code):
     """x_proj, y_proj of every row of xyz (no filtering) through dva_project_camera."""
-    lib = _lib.load()
     dev, n = xyz.device, xyz.shape[0]
     A, t0, t1 = _camera_transform(camera, img_extrinsic)
     cam = torch.from_numpy(np.concatenate([np.zeros(3, np.float32), A.reshape(-1), t0, t1, intr8])
@@ -144,9 +135,7 @@ def _project_raw(xyz, camera, img_extrinsic, intr8, code):
     xp = torch.empty(n, dtype=torch.float64, device=dev)
     yp = torch.empty(n, dtype=torch.float64, device=dev)
     keep = torch.empty(n, dtype=torch.uint8, device=dev)
-    with torch.cuda.device(dev):
-        check(lib.dva_project_camera(ptr(xyz), ptr(cam), code, ptr(d), ptr(xp), ptr(yp), ptr(keep), n, 1 << 20,
-                                     1 << 20, 0, 0, 0.0, 1e30, stream_ptr()), "dva_project_camera")
+    launch("dva_project_camera", dev, xyz, cam, code, d, xp, yp, keep, n, 1 << 20, 1 << 20, 0, 0, 0.0, 1e30)
     return xp, yp
 
 
@@ -157,7 +146,6 @@ def fisheye_splat_boxes(x_proj, y_proj, xyz, img_extrinsic, img_intrinsic_fishey
     a point and the projection of the top of its voxel (xyz + [0, 0, swell * voxel / 2]); NB the
     reference takes `dist = norm(xyz)` of the ABSOLUTE coordinates here (:900), reproduced."""
     require_cuda(x_proj, y_proj, xyz)
-    lib = _lib.load()
     xyz = xyz.float().contiguous()
     m = xyz.shape[0]
     # norm_cpu: float32, squares summed left to right (a device-side reduction may associate otherwise)
@@ -170,11 +158,8 @@ def fisheye_splat_boxes(x_proj, y_proj, xyz, img_extrinsic, img_intrinsic_fishey
     xt, yt = _project_raw(top, camera, img_extrinsic, intr, 3)
     width = 2 * torch.sqrt((x_proj.double() - xt) ** 2 + (y_proj.double() - yt) ** 2)
     splat = torch.empty((m, 4), dtype=torch.int32, device=xyz.device)
-    with torch.cuda.device(xyz.device):
-        check(lib.dva_splat_boxes_from_width(ptr(x_proj.double().contiguous()), ptr(y_proj.double().contiguous()),
-                                             ptr(width.contiguous()), ptr(splat), m, int(img_size[0]),
-                                             int(img_size[1]), int(crop_top), int(crop_bottom), stream_ptr()),
-              "dva_splat_boxes_from_width")
+    launch("dva_splat_boxes_from_width", xyz.device, x_proj.double().contiguous(), y_proj.double().contiguous(),
+           width.contiguous(), splat, m, int(img_size[0]), int(img_size[1]), int(crop_top), int(crop_bottom))
     return splat
 
 
@@ -182,7 +167,6 @@ def splat_boxes(x_proj, y_proj, dist, img_intrinsic_pinhole=None, img_size=(1024
                 crop_bottom=0, voxel=0.02, k_swell=1.0, d_swell=1000, camera='s3dis_equirectangular'):
     """[m,4] int32 (x_a, x_b, y_a, y_b) like *_splat_cpu (visibility.py:630-704, 761-827)."""
     require_cuda(x_proj, y_proj, dist)
-    lib = _lib.load()
     m = x_proj.shape[0]
     splat = torch.empty((m, 4), dtype=torch.int32, device=x_proj.device)
     if camera == 's3dis_equirectangular':
@@ -192,13 +176,9 @@ def splat_boxes(x_proj, y_proj, dist, img_intrinsic_pinhole=None, img_size=(1024
         fx, fy = float(img_intrinsic_pinhole[0][0]), float(img_intrinsic_pinhole[1][1])
     else:
         raise NotImplementedError(f"camera='{camera}' has no CUDA splat kernel yet")
-    D = ctypes.c_double
-    with torch.cuda.device(x_proj.device):
-        check(lib.dva_splat_boxes(ptr(x_proj.double().contiguous()), ptr(y_proj.double().contiguous()),
-                                  ptr(dist.float().contiguous()), ptr(splat), m, int(img_size[0]),
-                                  int(img_size[1]), int(crop_top), int(crop_bottom), D(float(voxel)),
-                                  D(float(k_swell)), D(float(d_swell)), cam, D(fx), D(fy), stream_ptr()),
-              "dva_splat_boxes")
+    launch("dva_splat_boxes", x_proj.device, x_proj.double().contiguous(), y_proj.double().contiguous(),
+           dist.float().contiguous(), splat, m, int(img_size[0]), int(img_size[1]), int(crop_top), int(crop_bottom),
+           float(voxel), float(k_swell), float(d_swell), cam, fx, fy)
     return splat
 
 
@@ -210,7 +190,6 @@ def visibility_from_splatting(x_proj, y_proj, dist, xyz=None, img_extrinsic=None
     [x, y] winner map).  Ties go to the lowest point index; `exact` keeps splat centres only."""
     require_cuda(x_proj, y_proj, dist)
     assert x_proj.shape[0] == y_proj.shape[0] == dist.shape[0] > 0
-    lib = _lib.load()
     dev = x_proj.device
     W, H = int(img_size[0]), int(img_size[1])
     Hc = H - int(crop_top) - int(crop_bottom)
@@ -226,10 +205,8 @@ def visibility_from_splatting(x_proj, y_proj, dist, xyz=None, img_extrinsic=None
     zbuf = torch.empty(W * Hc, dtype=torch.int64, device=dev)       # uint64 keys
     idx_map = torch.empty((W, Hc), dtype=torch.int64, device=dev)
     seen = torch.empty(m, dtype=torch.uint8, device=dev) if exact else None
-    with torch.cuda.device(dev):
-        check(lib.dva_zbuffer_splat(ptr(splat), ptr(d), ptr(xp), ptr(yp), ptr(zbuf), ptr(idx_map), ptr(seen), m,
-                                    W, H, int(crop_top), int(crop_bottom), int(bool(exact)), stream_ptr()),
-              "dva_zbuffer_splat")
+    launch("dva_zbuffer_splat", dev, splat, d, xp, yp, zbuf, idx_map, seen, m, W, H, int(crop_top), int(crop_bottom),
+           int(bool(exact)))
     pix = torch.nonzero(idx_map >= 0, as_tuple=False)
     x_pix, y_pix = pix[:, 0], pix[:, 1]
     return idx_map[x_pix, y_pix], x_pix, y_pix + int(crop_top)

@@ -14,7 +14,7 @@ direction at a time).  Every step still moves all of its inputs and results.
 import torch
 
 from . import _lib
-from ._lib import check, ptr, stream_ptr
+from ._lib import launch
 
 
 class ViewAttentionHostPlan:
@@ -22,7 +22,6 @@ class ViewAttentionHostPlan:
                  group_scaling=True, eps=1e-12, device="cuda"):
         self.N, self.V, self.R, self.C, self.G = N, V, R, C, G
         self.dtype, self.group_scaling, self.eps, self.gating = dtype, group_scaling, eps, gating
-        self.lib = _lib.load()
         d = torch.device(device)
         self.device = d
         e = lambda shape, dt: torch.empty(shape, dtype=dt, device=d)  # noqa: E731
@@ -39,31 +38,26 @@ class ViewAttentionHostPlan:
         self.gx = e((V, C), dtype)
         self.gcompat = e((V, G), torch.float32)
         self.ggate = e((2, G), torch.float32) if gating else None
-        self.ws_bytes = int(self.lib.dva_view_attention_bwd_workspace_bytes(G)) if gating else 0
-        self.ws = e((max(self.ws_bytes, 1),), torch.uint8)
+        # the workspace holds the gate-gradient partials; without gating the kernel does not read it
+        self.ws = _lib.workspace(_lib.load().dva_view_attention_bwd_workspace_bytes(G) if gating else 0, d)
         self.dcode = _lib.DTYPE_CODES[dtype]
 
     # -- device-resident pieces (bench.py's `value` times exactly these two calls) ---------------
     def forward_device(self, save_att=None):
         gw = self.gate[0] if self.gating else None
         gb = self.gate[1] if self.gating else None
-        check(self.lib.dva_view_attention_fwd(
-            ptr(self.x), ptr(self.idx), int(self.idx is not None and self.idx.dtype == torch.int64),
-            ptr(self.compat), ptr(self.ptr), ptr(gw), ptr(gb), ptr(self.out), ptr(save_att),
-            ptr(self.seg_max), ptr(self.seg_den), ptr(self.seg_arg), self.N, self.V, self.R, self.C,
-            self.G, int(self.group_scaling), float(self.eps), self.dcode, stream_ptr(self.device)),
-            "dva_view_attention_fwd")
+        launch("dva_view_attention_fwd", self.device, self.x, self.idx,
+               int(self.idx is not None and self.idx.dtype == torch.int64), self.compat, self.ptr, gw, gb, self.out,
+               save_att, self.seg_max, self.seg_den, self.seg_arg, self.N, self.V, self.R, self.C, self.G,
+               int(self.group_scaling), float(self.eps), self.dcode)
 
     def backward_device(self):
         gw = self.gate[0] if self.gating else None
         gb = self.gate[1] if self.gating else None
-        check(self.lib.dva_view_attention_bwd(
-            ptr(self.x), ptr(self.idx), int(self.idx is not None and self.idx.dtype == torch.int64),
-            ptr(self.compat), ptr(self.ptr), ptr(gw), ptr(gb), ptr(self.gout), ptr(self.seg_max),
-            ptr(self.seg_den), ptr(self.seg_arg), ptr(self.gx), ptr(self.gcompat), ptr(self.ggate), 0,
-            self.N, self.V, self.R, self.C, self.G, int(self.group_scaling), self.dcode,
-            ptr(self.ws) if self.gating else None, self.ws_bytes, stream_ptr(self.device)),
-            "dva_view_attention_bwd")
+        launch("dva_view_attention_bwd", self.device, self.x, self.idx,
+               int(self.idx is not None and self.idx.dtype == torch.int64), self.compat, self.ptr, gw, gb, self.gout,
+               self.seg_max, self.seg_den, self.seg_arg, self.gx, self.gcompat, self.ggate, 0, self.N, self.V,
+               self.R, self.C, self.G, int(self.group_scaling), self.dcode, self.ws, self.ws.numel())
 
     # -- host-buffer call ---------------------------------------------------------------------------
     def host_buffers(self, pin=True):

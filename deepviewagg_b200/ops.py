@@ -5,6 +5,7 @@ same empty-segment / tie / eps semantics) and is backed ONLY by the sm_90a kerne
 libdva_b200.so: CPU tensors or a missing library raise.  Reference citations are relative to the
 reference repository root.
 """
+import contextlib
 import math
 import os
 
@@ -23,7 +24,7 @@ _fwd_f32 = torch.amp.custom_fwd(device_type="cuda", cast_inputs=torch.float32)
 _bwd = torch.amp.custom_bwd(device_type="cuda")
 
 from . import _lib
-from ._lib import DTYPE_CODES, REDUCE_CODES, check, dtype_code, ptr, require_cuda, stream_ptr
+from ._lib import DTYPE_CODES, REDUCE_CODES, dtype_code, launch, require_cuda
 
 
 def _as_2d(src):
@@ -52,7 +53,6 @@ class _SegmentCSR(torch.autograd.Function):
     @_fwd
     def forward(ctx, src, csr_idx, reduce):
         require_cuda(src, csr_idx)
-        lib = _lib.load()
         code = REDUCE_CODES[reduce]
         shape = src.shape
         s2 = _as_2d(src)
@@ -65,9 +65,7 @@ class _SegmentCSR(torch.autograd.Function):
         arg = None
         if code in (2, 3):
             arg = torch.empty((n_seg, K), dtype=torch.int64, device=src.device)
-        with torch.cuda.device(src.device):
-            check(lib.dva_segment_csr_fwd(ptr(s2), ptr(csr_idx), ptr(out), ptr(arg), n_seg, n_items,
-                                          K, code, dtype_code(s2), stream_ptr()), "dva_segment_csr_fwd")
+        launch("dva_segment_csr_fwd", src.device, s2, csr_idx, out, arg, n_seg, n_items, K, code, dtype_code(s2))
         ctx.code, ctx.n_items, ctx.in_shape = code, n_items, shape
         ctx.save_for_backward(csr_idx, arg)
         return out
@@ -77,14 +75,11 @@ class _SegmentCSR(torch.autograd.Function):
     @torch.autograd.function.once_differentiable
     def backward(ctx, grad_out):
         csr_idx, arg = ctx.saved_tensors
-        lib = _lib.load()
         g2 = _as_2d(grad_out)
         n_seg, K = g2.shape
         gsrc = torch.empty(ctx.in_shape, dtype=g2.dtype, device=g2.device)
-        with torch.cuda.device(g2.device):
-            check(lib.dva_segment_csr_bwd(ptr(g2), ptr(csr_idx), ptr(arg), ptr(gsrc), n_seg,
-                                          ctx.n_items, K, ctx.code, dtype_code(g2), stream_ptr()),
-                  "dva_segment_csr_bwd")
+        launch("dva_segment_csr_bwd", g2.device, g2, csr_idx, arg, gsrc, n_seg, ctx.n_items, K, ctx.code,
+               dtype_code(g2))
         return gsrc, None, None
 
 
@@ -104,16 +99,13 @@ def segment_csr(src, indptr, out=None, reduce="sum"):
 def segment_csr_arg(src, indptr, reduce="max"):
     """(values, first-arg rows) like torch_scatter.segment_max_csr; arg = n_items when empty."""
     require_cuda(src, indptr)
-    lib = _lib.load()
     s2 = _as_2d(src)
     indptr = _check_csr(indptr, src.device)
     n_seg, n_items, K = indptr.numel() - 1, s2.shape[0], s2.shape[1]
     out = torch.empty((n_seg, K), dtype=src.dtype, device=src.device)
     arg = torch.empty((n_seg, K), dtype=torch.int64, device=src.device)
-    with torch.cuda.device(src.device):
-        check(lib.dva_segment_csr_fwd(ptr(s2), ptr(indptr), ptr(out), ptr(arg), n_seg, n_items, K,
-                                      REDUCE_CODES[reduce], dtype_code(s2), stream_ptr()),
-              "dva_segment_csr_fwd")
+    launch("dva_segment_csr_fwd", src.device, s2, indptr, out, arg, n_seg, n_items, K, REDUCE_CODES[reduce],
+           dtype_code(s2))
     tail = tuple(src.shape[1:])
     return out.view((n_seg,) + tail), arg.view((n_seg,) + tail)
 
@@ -126,14 +118,11 @@ class _GatherCSR(torch.autograd.Function):
     @_fwd
     def forward(ctx, src, csr_idx, n_items):
         require_cuda(src, csr_idx)
-        lib = _lib.load()
         s2 = _as_2d(src)
         csr_idx = _check_csr(csr_idx, src.device)
         n_seg, K = csr_idx.numel() - 1, s2.shape[1]
         out = torch.empty((n_items,) + tuple(src.shape[1:]), dtype=src.dtype, device=src.device)
-        with torch.cuda.device(src.device):
-            check(lib.dva_gather_csr(ptr(s2), ptr(csr_idx), ptr(out), n_seg, n_items, K,
-                                     dtype_code(s2), stream_ptr()), "dva_gather_csr")
+        launch("dva_gather_csr", src.device, s2, csr_idx, out, n_seg, n_items, K, dtype_code(s2))
         ctx.in_shape = src.shape
         ctx.save_for_backward(csr_idx)
         return out
@@ -143,15 +132,12 @@ class _GatherCSR(torch.autograd.Function):
     @torch.autograd.function.once_differentiable
     def backward(ctx, grad_out):
         (csr_idx,) = ctx.saved_tensors
-        lib = _lib.load()
         g2 = _as_2d(grad_out)
         n_items, K = g2.shape
         n_seg = csr_idx.numel() - 1
         gsrc = torch.empty(ctx.in_shape, dtype=g2.dtype, device=g2.device)
-        with torch.cuda.device(g2.device):
-            check(lib.dva_segment_csr_fwd(ptr(g2), ptr(csr_idx), ptr(gsrc), None, n_seg, n_items, K,
-                                          REDUCE_CODES["sum"], dtype_code(g2), stream_ptr()),
-                  "dva_segment_csr_fwd")
+        launch("dva_segment_csr_fwd", g2.device, g2, csr_idx, gsrc, None, n_seg, n_items, K, REDUCE_CODES["sum"],
+               dtype_code(g2))
         return gsrc, None, None
 
 
@@ -184,15 +170,12 @@ class _SegmentSoftmaxCSR(torch.autograd.Function):
     @_fwd
     def forward(ctx, src, csr_idx, eps, scaling):
         require_cuda(src, csr_idx)
-        lib = _lib.load()
         s2 = _as_2d(src)
         csr_idx = _check_csr(csr_idx, src.device)
         n_seg, n_items, K = csr_idx.numel() - 1, s2.shape[0], s2.shape[1]
         out = torch.empty(src.shape, dtype=src.dtype, device=src.device)
-        with torch.cuda.device(src.device):
-            check(lib.dva_segment_softmax_csr_fwd(ptr(s2), ptr(csr_idx), ptr(out), n_seg, n_items, K,
-                                                  float(eps), int(bool(scaling)), dtype_code(s2),
-                                                  stream_ptr()), "dva_segment_softmax_csr_fwd")
+        launch("dva_segment_softmax_csr_fwd", src.device, s2, csr_idx, out, n_seg, n_items, K, float(eps),
+               int(bool(scaling)), dtype_code(s2))
         ctx.scaling, ctx.in_shape = bool(scaling), src.shape
         ctx.save_for_backward(csr_idx, out)
         return out
@@ -202,15 +185,11 @@ class _SegmentSoftmaxCSR(torch.autograd.Function):
     @torch.autograd.function.once_differentiable
     def backward(ctx, grad_out):
         csr_idx, out = ctx.saved_tensors
-        lib = _lib.load()
         g2 = _as_2d(grad_out)
         n_items, K = g2.shape
         gsrc = torch.empty(ctx.in_shape, dtype=g2.dtype, device=g2.device)
-        with torch.cuda.device(g2.device):
-            check(lib.dva_segment_softmax_csr_bwd(ptr(out), ptr(g2), ptr(csr_idx), ptr(gsrc),
-                                                  csr_idx.numel() - 1, n_items, K, int(ctx.scaling),
-                                                  dtype_code(g2), stream_ptr()),
-                  "dva_segment_softmax_csr_bwd")
+        launch("dva_segment_softmax_csr_bwd", g2.device, out, g2, csr_idx, gsrc, csr_idx.numel() - 1, n_items, K,
+               int(ctx.scaling), dtype_code(g2))
         return gsrc, None, None, None
 
 
@@ -231,22 +210,16 @@ def segment_softmax_csr(src, csr_idx, eps=1e-12, scaling=False):
 def _scatter_add_rows(src, idx, n_rows):
     """fp32 [n_rows, C] with dst[idx[v]] += src[v] (dva_scatter_add_rows).  Under
     torch.use_deterministic_algorithms(True): dva_scatter_add_rows_det (every row summed in ascending v)."""
-    lib = _lib.load()
     src = src.contiguous()
     V, C = src.shape
     if torch.are_deterministic_algorithms_enabled():
         dst = torch.empty((n_rows, C), dtype=torch.float32, device=src.device)
-        ws_bytes = int(lib.dva_scatter_add_rows_det_workspace_bytes(V, n_rows))
-        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=src.device)
-        with torch.cuda.device(src.device):
-            check(lib.dva_scatter_add_rows_det(ptr(src), ptr(idx.contiguous()), ptr(dst), V, n_rows, C,
-                                               dtype_code(src), ptr(ws), ws_bytes, stream_ptr()),
-                  "dva_scatter_add_rows_det")
+        ws = _lib.workspace(_lib.load().dva_scatter_add_rows_det_workspace_bytes(V, n_rows), src.device)
+        launch("dva_scatter_add_rows_det", src.device, src, idx.contiguous(), dst, V, n_rows, C, dtype_code(src),
+               ws, ws.numel())
         return dst
     dst = torch.zeros((n_rows, C), dtype=torch.float32, device=src.device)
-    with torch.cuda.device(src.device):
-        check(lib.dva_scatter_add_rows(ptr(src), ptr(idx.contiguous()), ptr(dst), V, n_rows, C, dtype_code(src),
-                                       stream_ptr()), "dva_scatter_add_rows")
+    launch("dva_scatter_add_rows", src.device, src, idx.contiguous(), dst, V, n_rows, C, dtype_code(src))
     return dst
 
 
@@ -260,7 +233,6 @@ class _ViewAttention(torch.autograd.Function):
     def forward(ctx, x, idx, compat, csr_idx, gate_w, gate_b, num_groups, group_scaling, eps,
                 idx_is_permutation):
         require_cuda(x, idx, compat, csr_idx, gate_w, gate_b)
-        lib = _lib.load()
         x = x.contiguous()
         compat = compat.float().contiguous()
         csr_idx = _check_csr(csr_idx, x.device)
@@ -285,12 +257,8 @@ class _ViewAttention(torch.autograd.Function):
         seg_max = torch.empty((N, G), dtype=torch.float32, device=x.device)
         seg_den = torch.empty((N, G), dtype=torch.float32, device=x.device)
         seg_arg = torch.empty((N, G), dtype=torch.int32, device=x.device)
-        with torch.cuda.device(x.device):
-            check(lib.dva_view_attention_fwd(ptr(x), ptr(idx), idx64, ptr(compat), ptr(csr_idx), ptr(gw),
-                                             ptr(gb), ptr(out), ptr(att), ptr(seg_max), ptr(seg_den),
-                                             ptr(seg_arg), N, V, R, C, G, int(bool(group_scaling)),
-                                             float(eps), dtype_code(x), stream_ptr()),
-                  "dva_view_attention_fwd")
+        launch("dva_view_attention_fwd", x.device, x, idx, idx64, compat, csr_idx, gw, gb, out, att, seg_max,
+               seg_den, seg_arg, N, V, R, C, G, int(bool(group_scaling)), float(eps), dtype_code(x))
         ctx.cfg = (N, V, R, C, G, bool(group_scaling), idx64, bool(idx_is_permutation),
                    gate_w.shape if gate_w is not None else None,
                    gate_b.shape if gate_b is not None else None,
@@ -305,22 +273,17 @@ class _ViewAttention(torch.autograd.Function):
     def backward(ctx, grad_out, _ga, _gm):
         x, idx, compat, csr_idx, gw, gb, seg_max, seg_den, seg_arg = ctx.saved_tensors
         N, V, R, C, G, scaling, idx64, is_perm, w_shape, b_shape, w_dtype = ctx.cfg
-        lib = _lib.load()
         grad_out = grad_out.contiguous()
         scatter = int(idx is not None and is_perm and R == V)
         gx_rows = torch.empty((V, C), dtype=x.dtype, device=x.device)
         gcompat = torch.empty((V, G), dtype=torch.float32, device=x.device)
-        ggate, ws, ws_bytes = None, None, 0
+        ggate, ws = None, None                      # the workspace holds the gate-gradient partials only
         if gw is not None:
             ggate = torch.empty((2, G), dtype=torch.float32, device=x.device)
-            ws_bytes = int(lib.dva_view_attention_bwd_workspace_bytes(G))
-            ws = torch.empty(ws_bytes, dtype=torch.uint8, device=x.device)
-        with torch.cuda.device(x.device):
-            check(lib.dva_view_attention_bwd(ptr(x), ptr(idx), idx64, ptr(compat), ptr(csr_idx), ptr(gw),
-                                             ptr(gb), ptr(grad_out), ptr(seg_max), ptr(seg_den),
-                                             ptr(seg_arg), ptr(gx_rows), ptr(gcompat), ptr(ggate),
-                                             scatter, N, V, R, C, G, int(scaling), dtype_code(x), ptr(ws),
-                                             ws_bytes, stream_ptr()), "dva_view_attention_bwd")
+            ws = _lib.workspace(_lib.load().dva_view_attention_bwd_workspace_bytes(G), x.device)
+        launch("dva_view_attention_bwd", x.device, x, idx, idx64, compat, csr_idx, gw, gb, grad_out, seg_max,
+               seg_den, seg_arg, gx_rows, gcompat, ggate, scatter, N, V, R, C, G, int(scaling), dtype_code(x), ws,
+               0 if ws is None else ws.numel())
         if idx is None or scatter:
             gx = gx_rows
         else:  # general (non-injective) gather: accumulate duplicated rows (red.global.add.v4.f32 kernel)
@@ -357,7 +320,6 @@ class _QKScores(torch.autograd.Function):
     @_fwd
     def forward(ctx, keys, queries, csr_idx, num_groups, scale):
         require_cuda(keys, queries, csr_idx)
-        lib = _lib.load()
         k32, q32 = keys.float().contiguous(), queries.float().contiguous()
         csr_idx = _check_csr(csr_idx, keys.device)
         N, V, G = csr_idx.numel() - 1, k32.shape[0], int(num_groups)
@@ -365,9 +327,7 @@ class _QKScores(torch.autograd.Function):
         if k32.shape[1] != G * D or q32.shape != (N, G * D):
             raise ValueError("keys must be [V,G*D] and queries [N,G*D]")
         compat = torch.empty((V, G), dtype=torch.float32, device=keys.device)
-        with torch.cuda.device(keys.device):
-            check(lib.dva_qk_scores_fwd(ptr(k32), ptr(q32), ptr(csr_idx), ptr(compat), N, V, G, D,
-                                        float(scale), stream_ptr()), "dva_qk_scores_fwd")
+        launch("dva_qk_scores_fwd", keys.device, k32, q32, csr_idx, compat, N, V, G, D, float(scale))
         ctx.cfg = (N, V, G, D, float(scale), keys.dtype, queries.dtype)
         ctx.save_for_backward(k32, q32, csr_idx)
         return compat
@@ -378,12 +338,9 @@ class _QKScores(torch.autograd.Function):
     def backward(ctx, gcompat):
         k32, q32, csr_idx = ctx.saved_tensors
         N, V, G, D, scale, kd, qd = ctx.cfg
-        lib = _lib.load()
         gcompat = gcompat.float().contiguous()
         gk, gq = torch.empty_like(k32), torch.empty_like(q32)
-        with torch.cuda.device(k32.device):
-            check(lib.dva_qk_scores_bwd(ptr(k32), ptr(q32), ptr(csr_idx), ptr(gcompat), ptr(gk), ptr(gq),
-                                        N, V, G, D, scale, stream_ptr()), "dva_qk_scores_bwd")
+        launch("dva_qk_scores_bwd", k32.device, k32, q32, csr_idx, gcompat, gk, gq, N, V, G, D, scale)
         return gk.to(kd), gq.to(qd), None, None, None
 
 
@@ -402,17 +359,14 @@ class _HeuristicPool(torch.autograd.Function):
     @_fwd
     def forward(ctx, x_mod, x_map, csr_idx, feat, use_max):
         require_cuda(x_mod, x_map, csr_idx)
-        lib = _lib.load()
         x_mod = x_mod.contiguous()
         m32 = x_map.float().contiguous()
         csr_idx = _check_csr(csr_idx, x_mod.device)
         N, V, C = csr_idx.numel() - 1, x_mod.shape[0], x_mod.shape[1]
         out = torch.empty((N, C), dtype=x_mod.dtype, device=x_mod.device)
         arg = torch.empty((N,), dtype=torch.int64, device=x_mod.device)
-        with torch.cuda.device(x_mod.device):
-            check(lib.dva_heuristic_pool_fwd(ptr(x_mod), ptr(m32), m32.shape[1], int(feat), ptr(csr_idx),
-                                             ptr(out), ptr(arg), N, V, C, int(bool(use_max)),
-                                             dtype_code(x_mod), stream_ptr()), "dva_heuristic_pool_fwd")
+        launch("dva_heuristic_pool_fwd", x_mod.device, x_mod, m32, m32.shape[1], int(feat), csr_idx, out, arg, N,
+               V, C, int(bool(use_max)), dtype_code(x_mod))
         ctx.V = V
         ctx.save_for_backward(arg)
         return out
@@ -437,9 +391,7 @@ def heuristic_pool(x_mod, x_map, csr_idx, feat, mode="max"):
 def _transpose_last2(t, B, R, S):
     """[B,R,S] -> [B,S,R] copy through dva_transpose_last2 (t contiguous)."""
     out = torch.empty_like(t)
-    with torch.cuda.device(t.device):
-        check(_lib.load().dva_transpose_last2(ptr(t), ptr(out), B, R, S, dtype_code(t), stream_ptr()),
-              "dva_transpose_last2")
+    launch("dva_transpose_last2", t.device, t, out, B, R, S, dtype_code(t))
     return out
 
 
@@ -475,7 +427,6 @@ class _GatherPool(torch.autograd.Function):
     @_fwd
     def forward(ctx, fmap, images, pixels, atomic_ptr, reduce, channels_last, mapping_size):
         require_cuda(fmap, images, pixels, atomic_ptr)
-        lib = _lib.load()
         fmap = fmap.contiguous()
         via_cl = False
         if channels_last:
@@ -501,15 +452,13 @@ class _GatherPool(torch.autograd.Function):
             _validate_gather_indices(images, pixels.long(), B, int(lim[0]), int(lim[1]))
         out = torch.empty((Vw, C), dtype=fmap.dtype, device=fmap.device)
         arg = torch.empty((Vw, C), dtype=torch.int64, device=fmap.device) if code in (2, 3) else None
-        head = (ptr(fmap), int(channels_last), ptr(images), ptr(pixels), int(pixels.dtype == torch.int16),
-                ptr(atomic_ptr), ptr(out), ptr(arg), B, C, H, W)
-        tail = (Vw, P, code, dtype_code(fmap), stream_ptr())
-        with torch.cuda.device(fmap.device):
-            if mapping_size is None:
-                check(lib.dva_gather_pool_fwd(*head, *tail), "dva_gather_pool_fwd")
-            else:
-                check(lib.dva_interp_pool_fwd(*head, int(mapping_size[0]), int(mapping_size[1]), *tail),
-                      "dva_interp_pool_fwd")
+        head = (fmap, int(channels_last), images, pixels, int(pixels.dtype == torch.int16), atomic_ptr, out, arg,
+                B, C, H, W)
+        tail = (Vw, P, code, dtype_code(fmap))
+        if mapping_size is None:
+            launch("dva_gather_pool_fwd", fmap.device, *head, *tail)
+        else:
+            launch("dva_interp_pool_fwd", fmap.device, *head, int(mapping_size[0]), int(mapping_size[1]), *tail)
         ctx.cfg = (B, C, H, W, Vw, P, code, bool(channels_last), fmap.shape, fmap.dtype, mapping_size, via_cl)
         ctx.save_for_backward(images, pixels, atomic_ptr, arg)
         return out
@@ -520,26 +469,21 @@ class _GatherPool(torch.autograd.Function):
     def backward(ctx, grad_out):
         images, pixels, atomic_ptr, arg = ctx.saved_tensors
         B, C, H, W, Vw, P, code, cl, shape, dt, mapping_size, via_cl = ctx.cfg
-        lib = _lib.load()
         grad_out = grad_out.contiguous()
+        dev = grad_out.device
         # torch.use_deterministic_algorithms(True): the map gradient is reduced per map pixel in a fixed
         # order (the _det entry points write every element) instead of accumulated with fp32 atomics
         det = torch.are_deterministic_algorithms_enabled()
-        gf = (torch.empty if det else torch.zeros)(shape, dtype=torch.float32, device=grad_out.device)
-        head = (ptr(grad_out), int(cl), ptr(images), ptr(pixels), int(pixels.dtype == torch.int16),
-                ptr(atomic_ptr), ptr(arg), ptr(gf), B, C, H, W)
+        gf = (torch.empty if det else torch.zeros)(shape, dtype=torch.float32, device=dev)
+        head = (grad_out, int(cl), images, pixels, int(pixels.dtype == torch.int16), atomic_ptr, arg, gf, B, C, H, W)
         tail = (Vw, P, code, dtype_code(grad_out))
         msz = () if mapping_size is None else (int(mapping_size[0]), int(mapping_size[1]))
-        with torch.cuda.device(grad_out.device):
-            if det:
-                name = "dva_gather_pool_bwd_det" if mapping_size is None else "dva_interp_pool_bwd_det"
-                ws_bytes = int(getattr(lib, name + "_workspace_bytes")(B, H, W, P))
-                ws = torch.empty(ws_bytes, dtype=torch.uint8, device=grad_out.device)
-                check(getattr(lib, name)(*head, *msz, *tail, ptr(ws), ws_bytes, stream_ptr()), name)
-            elif mapping_size is None:
-                check(lib.dva_gather_pool_bwd(*head, *tail, stream_ptr()), "dva_gather_pool_bwd")
-            else:
-                check(lib.dva_interp_pool_bwd(*head, *msz, *tail, stream_ptr()), "dva_interp_pool_bwd")
+        name = "dva_gather_pool_bwd" if mapping_size is None else "dva_interp_pool_bwd"
+        if det:
+            ws = _lib.workspace(getattr(_lib.load(), name + "_det_workspace_bytes")(B, H, W, P), dev)
+            launch(name + "_det", dev, *head, *msz, *tail, ws, ws.numel())
+        else:
+            launch(name, dev, *head, *msz, *tail)
         if via_cl:      # gradient of the NCHW input: transpose the channels-last map gradient back
             gf = _transpose_last2(gf, B, H * W, C).view(B, C, H, W)
         return gf.to(dt), None, None, None, None, None, None
@@ -570,59 +514,60 @@ def sparse_interpolation_pixels(fmap, images_per_pixel, pixels, mapping_size, ch
 # --------------------------------------------------------------------------------------------
 # fused BatchNorm1d + LeakyReLU over [rows, C] (base_modules.py:38-48, 131-156)
 # --------------------------------------------------------------------------------------------
+@contextlib.contextmanager
+def _fp32_running(running_mean, running_var):
+    """The running buffers as the contiguous fp32 arrays the training kernels update IN PLACE through raw
+    pointers.  A buffer of another dtype or layout (e.g. a module converted with .half()) is staged through an
+    fp32 copy, which is written back when the block ends."""
+    bufs = (running_mean, running_var)
+    staged = tuple(b if b is None or (b.dtype == torch.float32 and b.is_contiguous()) else b.float().contiguous()
+                   for b in bufs)
+    yield staged
+    for buf, tmp in zip(bufs, staged):
+        if tmp is not buf:
+            buf.copy_(tmp)
+
+
+def _bn_apply(z, gamma, beta, mean, invstd, eps, slope):
+    """act(gamma (z - mean) invstd + beta) on given statistics: dva_bn_act_fwd with training = 0, which reads
+    only mean / invstd (also passed for the running buffers it requires) and no workspace."""
+    y = torch.empty_like(z)
+    launch("dva_bn_act_fwd", z.device, z, gamma, beta, mean, mean, mean, invstd, y, z.shape[0], z.shape[1],
+           float(eps), 0.0, float(slope), 0, dtype_code(z), None, 0)
+    return y
+
+
 class _BNAct(torch.autograd.Function):
     @staticmethod
     @_fwd
     def forward(ctx, z, weight, bias, running_mean, running_var, training, momentum, eps, slope,
                 pre_mean=None, pre_invstd=None):
         require_cuda(z, weight, bias, running_mean, running_var)
-        lib = _lib.load()
         z = z.contiguous()
         R, C = z.shape
         dev = z.device
         gamma = weight.detach().float().contiguous() if weight is not None else None
         beta = bias.detach().float().contiguous() if bias is not None else None
-        y = torch.empty_like(z)
-        # batch statistics already taken in the producing GEMM's epilogue (ops.linear_bn_act): apply only;
-        # the backward still differentiates through the batch statistics (ctx keeps training = True)
-        have_stats = training and pre_mean is not None
-        if have_stats:
-            mean, invstd = pre_mean, pre_invstd
-        elif training:
+        if training and pre_mean is None:
             mean = torch.empty(C, dtype=torch.float32, device=dev)
             invstd = torch.empty(C, dtype=torch.float32, device=dev)
+            y = torch.empty_like(z)
+            ws = _lib.workspace(_lib.load().dva_bn_workspace_bytes(R, C), dev)
+            with _fp32_running(running_mean, running_var) as (rm, rv):
+                launch("dva_bn_act_fwd", dev, z, gamma, beta, rm, rv, mean, invstd, y, R, C, float(eps),
+                       float(momentum), float(slope), 1, dtype_code(z), ws, ws.numel())
         else:
-            mean = running_mean.float().contiguous()
-            invstd = torch.rsqrt(running_var.float() + eps).contiguous()
-        ws_bytes = int(lib.dva_bn_workspace_bytes(R, C))
-        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
-        rm = running_mean if (training and running_mean is not None) else None
-        rv = running_var if (training and running_var is not None) else None
-        if not training:
-            rm, rv = running_mean, running_var
-        kernel_training = training and not have_stats
-        if have_stats:
-            rm = rv = mean                     # eval-style call: the kernel only reads mean / invstd
-        # the training kernel updates the running buffers IN PLACE through raw float pointers
-        stage = []
-        for name, buf in (("running_mean", rm), ("running_var", rv)):
-            if have_stats:
-                break
-            if buf is not None and (buf.dtype != torch.float32 or not buf.is_contiguous()):
-                if not training:
-                    raise TypeError(f"{name} must be a contiguous float32 buffer in eval mode")
-                stage.append((name, buf, buf.float().contiguous()))   # e.g. a module converted with .half()
-        for name, _, tmp in stage:
-            if name == "running_mean":
-                rm = tmp
+            if training:
+                # batch statistics already taken in the producing GEMM's epilogue (ops.linear_bn_act): apply only;
+                # the backward still differentiates through the batch statistics (ctx keeps training = True)
+                mean, invstd = pre_mean, pre_invstd
             else:
-                rv = tmp
-        with torch.cuda.device(dev):
-            check(lib.dva_bn_act_fwd(ptr(z), ptr(gamma), ptr(beta), ptr(rm), ptr(rv), ptr(mean), ptr(invstd), ptr(y),
-                                     R, C, float(eps), float(momentum), float(slope), int(bool(kernel_training)),
-                                     dtype_code(z), ptr(ws), ws_bytes, stream_ptr()), "dva_bn_act_fwd")
-        for _, buf, tmp in stage:
-            buf.copy_(tmp)
+                for name, buf in (("running_mean", running_mean), ("running_var", running_var)):
+                    if buf.dtype != torch.float32 or not buf.is_contiguous():
+                        raise TypeError(f"{name} must be a contiguous float32 buffer in eval mode")
+                mean = running_mean.float().contiguous()
+                invstd = torch.rsqrt(running_var.float() + eps).contiguous()
+            y = _bn_apply(z, gamma, beta, mean, invstd, eps, slope)
         ctx.cfg = (R, C, float(slope), bool(training), weight is not None, bias is not None,
                    weight.dtype if weight is not None else None)
         ctx.save_for_backward(z, gamma, beta, mean, invstd)
@@ -634,27 +579,26 @@ class _BNAct(torch.autograd.Function):
     def backward(ctx, dy):
         z, gamma, beta, mean, invstd = ctx.saved_tensors
         R, C, slope, training, has_w, has_b, wdt = ctx.cfg
-        lib = _lib.load()
         dy = dy.contiguous()
         dz = torch.empty_like(z)
         sums = torch.empty((2, C), dtype=torch.float32, device=z.device)
-        ws_bytes = int(lib.dva_bn_workspace_bytes(R, C))
-        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=z.device)
-        with torch.cuda.device(z.device):
-            check(lib.dva_bn_act_bwd(ptr(dy), ptr(z), ptr(gamma), ptr(beta), ptr(mean), ptr(invstd), ptr(dz),
-                                     ptr(sums), R, C, slope, int(training), dtype_code(z), ptr(ws), ws_bytes,
-                                     stream_ptr()), "dva_bn_act_bwd")
+        ws = _lib.workspace(_lib.load().dva_bn_workspace_bytes(R, C), z.device)
+        launch("dva_bn_act_bwd", z.device, dy, z, gamma, beta, mean, invstd, dz, sums, R, C, slope, int(training),
+               dtype_code(z), ws, ws.numel())
         gw = sums[1].to(wdt) if has_w else None
         gb = sums[0].to(wdt) if has_b else None
         return dz, gw, gb, None, None, None, None, None, None, None, None
 
 
-def batch_norm_act(z, bn, negative_slope=1.0):
-    """act(BatchNorm1d(z)) for z [rows, C] with the statistics / running-average semantics of
-    nn.BatchNorm1d (training: batch statistics over all rows, momentum update of the running
-    buffers, num_batches_tracked += 1).  `bn` is the nn.BatchNorm1d holding the parameters;
-    negative_slope = 1 gives plain BatchNorm, 0.2 the MLP layers of the pools."""
-    training = bn.training or (bn.running_mean is None and bn.running_var is None)
+def _uses_batch_stats(bn):
+    """nn.BatchNorm1d normalises with the batch statistics in training and when it keeps no running ones."""
+    return bn.training or (bn.running_mean is None and bn.running_var is None)
+
+
+def _bn_step(bn):
+    """nn.BatchNorm1d's bookkeeping for one forward: num_batches_tracked += 1 in training; returns the running
+    buffers to update (None when not tracked) and the momentum (1 / num_batches_tracked, a cumulative average,
+    when bn.momentum is None)."""
     momentum = 0.0 if bn.momentum is None else bn.momentum
     if bn.training and bn.track_running_stats and bn.num_batches_tracked is not None:
         bn.num_batches_tracked.add_(1)
@@ -662,7 +606,16 @@ def batch_norm_act(z, bn, negative_slope=1.0):
             momentum = 1.0 / float(bn.num_batches_tracked)
     rm = bn.running_mean if bn.track_running_stats else None
     rv = bn.running_var if bn.track_running_stats else None
-    return _BNAct.apply(z, bn.weight, bn.bias, rm, rv, training, momentum, bn.eps, negative_slope)
+    return rm, rv, momentum
+
+
+def batch_norm_act(z, bn, negative_slope=1.0):
+    """act(BatchNorm1d(z)) for z [rows, C] with the statistics / running-average semantics of
+    nn.BatchNorm1d (training: batch statistics over all rows, momentum update of the running
+    buffers, num_batches_tracked += 1).  `bn` is the nn.BatchNorm1d holding the parameters;
+    negative_slope = 1 gives plain BatchNorm, 0.2 the MLP layers of the pools."""
+    rm, rv, momentum = _bn_step(bn)
+    return _BNAct.apply(z, bn.weight, bn.bias, rm, rv, _uses_batch_stats(bn), momentum, bn.eps, negative_slope)
 
 
 # --------------------------------------------------------------------------------------------
@@ -680,7 +633,6 @@ def set_gemm_precision(mode):
 def _tc_gemm(a, b, layout, n_out):
     """layout 0: D[M,n_out] = a[M,K] . b[n_out,K]^T;  1: D[M,n_out] = a[M,K] . b[K,n_out];
     2: D[N,n_out] = a[M,N]^T . b[M,n_out]  -- through dva_linear_gemm."""
-    lib = _lib.load()
     prec = _GEMM_PRECISION["mode"]
     if layout == 2:
         M, N = a.shape
@@ -690,12 +642,34 @@ def _tc_gemm(a, b, layout, n_out):
         M, K = a.shape
         N = n_out
         out = torch.empty((M, N), dtype=torch.float32, device=a.device)
-    ws_bytes = int(lib.dva_linear_gemm_workspace_bytes(M, N, K, layout, prec))
-    ws = torch.empty(max(ws_bytes, 16), dtype=torch.uint8, device=a.device)
-    with torch.cuda.device(a.device):
-        check(lib.dva_linear_gemm(ptr(a), ptr(b), ptr(out), M, N, K, layout, prec, ptr(ws), ws.numel(),
-                                  stream_ptr()), "dva_linear_gemm")
+    ws = _lib.workspace(_lib.load().dva_linear_gemm_workspace_bytes(M, N, K, layout, prec), a.device)
+    launch("dva_linear_gemm", a.device, a, b, out, M, N, K, layout, prec, ws, ws.numel())
     return out
+
+
+def _linear_grads(ctx, gz):
+    """(dX, dW) of z = x @ w.T, each only when its input needs it, from the (x, w) the forward saved."""
+    x, w = ctx.saved_tensors
+    gz = gz.float().contiguous()
+    gx = _tc_gemm(gz, w, 1, w.shape[1]) if ctx.needs_input_grad[0] else None
+    # dW = dZ^T X: [out,in] result reduced over all rows -- stream-K split over the SMs
+    gw = _tc_gemm(gz, x, 2, x.shape[1]) if ctx.needs_input_grad[1] else None
+    return gx, gw
+
+
+def _linear_bnstats(x, w, running_mean, running_var, momentum, eps):
+    """z = x @ w.T (fp32, contiguous) with the batch statistics of z's columns taken in the GEMM epilogue
+    (dva_linear_bnstats_fwd), which also updates the running buffers: returns (z, mean, invstd)."""
+    M, K = x.shape
+    N = w.shape[0]
+    z = torch.empty((M, N), dtype=torch.float32, device=x.device)
+    mean = torch.empty(N, dtype=torch.float32, device=x.device)
+    invstd = torch.empty(N, dtype=torch.float32, device=x.device)
+    ws = _lib.workspace(_lib.load().dva_linear_bnstats_workspace_bytes(N, K), x.device)
+    with _fp32_running(running_mean, running_var) as (rm, rv):
+        launch("dva_linear_bnstats_fwd", x.device, x, w, z, M, N, K, float(eps), float(momentum), mean, invstd, rm,
+               rv, ws, ws.numel())
+    return z, mean, invstd
 
 
 def tc_gemm_supported(x, weight):
@@ -720,12 +694,7 @@ class _Linear(torch.autograd.Function):
     @_bwd
     @torch.autograd.function.once_differentiable
     def backward(ctx, gz):
-        x, w = ctx.saved_tensors
-        gz = gz.float().contiguous()
-        gx = _tc_gemm(gz, w, 1, w.shape[1]) if ctx.needs_input_grad[0] else None
-        # dW = dZ^T X: [out,in] result reduced over all rows -- stream-K split over the SMs
-        gw = _tc_gemm(gz, x, 2, x.shape[1]) if ctx.needs_input_grad[1] else None
-        return gx, gw
+        return _linear_grads(ctx, gz)
 
 
 class _LinearStats(torch.autograd.Function):
@@ -736,31 +705,8 @@ class _LinearStats(torch.autograd.Function):
     @_fwd_f32
     def forward(ctx, x, weight, running_mean, running_var, momentum, eps):
         require_cuda(x, weight)
-        lib = _lib.load()
         x, w = x.float().contiguous(), weight.float().contiguous()
-        M, K = x.shape
-        N = w.shape[0]
-        z = torch.empty((M, N), dtype=torch.float32, device=x.device)
-        mean = torch.empty(N, dtype=torch.float32, device=x.device)
-        invstd = torch.empty(N, dtype=torch.float32, device=x.device)
-        stage = []
-        rm, rv = running_mean, running_var
-        for name, buf in (("m", rm), ("v", rv)):
-            if buf is not None and (buf.dtype != torch.float32 or not buf.is_contiguous()):
-                stage.append((name, buf, buf.float().contiguous()))
-        for name, _, tmp in stage:
-            if name == "m":
-                rm = tmp
-            else:
-                rv = tmp
-        ws_bytes = int(lib.dva_linear_bnstats_workspace_bytes(N, K))
-        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=x.device)
-        with torch.cuda.device(x.device):
-            check(lib.dva_linear_bnstats_fwd(ptr(x), ptr(w), ptr(z), M, N, K, float(eps), float(momentum), ptr(mean),
-                                             ptr(invstd), ptr(rm), ptr(rv), ptr(ws), ws_bytes, stream_ptr()),
-                  "dva_linear_bnstats_fwd")
-        for _, buf, tmp in stage:
-            buf.copy_(tmp)
+        z, mean, invstd = _linear_bnstats(x, w, running_mean, running_var, momentum, eps)
         ctx.save_for_backward(x, w)
         ctx.mark_non_differentiable(mean, invstd)
         return z, mean, invstd
@@ -769,11 +715,7 @@ class _LinearStats(torch.autograd.Function):
     @_bwd
     @torch.autograd.function.once_differentiable
     def backward(ctx, gz, _gm, _gi):
-        x, w = ctx.saved_tensors
-        gz = gz.float().contiguous()
-        gx = _tc_gemm(gz, w, 1, w.shape[1]) if ctx.needs_input_grad[0] else None
-        gw = _tc_gemm(gz, x, 2, x.shape[1]) if ctx.needs_input_grad[1] else None
-        return gx, gw, None, None, None, None
+        return (*_linear_grads(ctx, gz), None, None, None, None)
 
 
 class _MLPLayer(torch.autograd.Function):
@@ -785,39 +727,11 @@ class _MLPLayer(torch.autograd.Function):
     @_fwd_f32
     def forward(ctx, x, weight, gamma, beta, running_mean, running_var, momentum, eps, slope):
         require_cuda(x, weight, gamma, beta)
-        lib = _lib.load()
         x, w = x.float().contiguous(), weight.float().contiguous()
-        M, K = x.shape
-        N = w.shape[0]
-        dev = x.device
-        z = torch.empty((M, N), dtype=torch.float32, device=dev)
-        mean = torch.empty(N, dtype=torch.float32, device=dev)
-        invstd = torch.empty(N, dtype=torch.float32, device=dev)
         g = gamma.detach().float().contiguous() if gamma is not None else None
         b = beta.detach().float().contiguous() if beta is not None else None
-        stage = []
-        rm, rv = running_mean, running_var
-        for name, buf in (("m", rm), ("v", rv)):
-            if buf is not None and (buf.dtype != torch.float32 or not buf.is_contiguous()):
-                stage.append((name, buf, buf.float().contiguous()))
-        for name, _, tmp in stage:
-            if name == "m":
-                rm = tmp
-            else:
-                rv = tmp
-        ws_bytes = max(int(lib.dva_linear_bnstats_workspace_bytes(N, K)), int(lib.dva_bn_workspace_bytes(M, N)))
-        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
-        y = torch.empty_like(z)
-        with torch.cuda.device(dev):
-            check(lib.dva_linear_bnstats_fwd(ptr(x), ptr(w), ptr(z), M, N, K, float(eps), float(momentum), ptr(mean),
-                                             ptr(invstd), ptr(rm), ptr(rv), ptr(ws), ws_bytes, stream_ptr()),
-                  "dva_linear_bnstats_fwd")
-            # apply half: eval-style call on the batch statistics (the kernel only reads mean / invstd)
-            check(lib.dva_bn_act_fwd(ptr(z), ptr(g), ptr(b), ptr(mean), ptr(mean), ptr(mean), ptr(invstd), ptr(y),
-                                     M, N, float(eps), 0.0, float(slope), 0, dtype_code(z), ptr(ws), ws_bytes,
-                                     stream_ptr()), "dva_bn_act_fwd")
-        for _, buf, tmp in stage:
-            buf.copy_(tmp)
+        z, mean, invstd = _linear_bnstats(x, w, running_mean, running_var, momentum, eps)
+        y = _bn_apply(z, g, b, mean, invstd, eps, slope)
         ctx.cfg = (float(slope), gamma is not None, beta is not None,
                    gamma.dtype if gamma is not None else (beta.dtype if beta is not None else None), weight.dtype)
         ctx.save_for_backward(x, w, z, g, b, mean, invstd)
@@ -829,19 +743,15 @@ class _MLPLayer(torch.autograd.Function):
     def backward(ctx, dy):
         x, w, z, g, b, mean, invstd = ctx.saved_tensors
         slope, has_g, has_b, pdt, wdt = ctx.cfg
-        lib = _lib.load()
         M, K = x.shape
         N = w.shape[0]
         dy = dy.float().contiguous()
         dx = torch.empty_like(x) if ctx.needs_input_grad[0] else None
         dw = torch.empty_like(w)
         sums = torch.empty((2, N), dtype=torch.float32, device=x.device)
-        ws_bytes = int(lib.dva_mlp_layer_bwd_workspace_bytes(M, N, K))
-        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=x.device)
-        with torch.cuda.device(x.device):
-            check(lib.dva_mlp_layer_bwd(ptr(dy), ptr(z), ptr(x), ptr(w), ptr(g), ptr(b), ptr(mean), ptr(invstd),
-                                        ptr(dx), ptr(dw), ptr(sums), M, N, K, slope, ptr(ws), ws_bytes, stream_ptr()),
-                  "dva_mlp_layer_bwd")
+        ws = _lib.workspace(_lib.load().dva_mlp_layer_bwd_workspace_bytes(M, N, K), x.device)
+        launch("dva_mlp_layer_bwd", x.device, dy, z, x, w, g, b, mean, invstd, dx, dw, sums, M, N, K, slope, ws,
+               ws.numel())
         gw = sums[1].to(pdt) if has_g else None
         gb = sums[0].to(pdt) if has_b else None
         return dx, (dw.to(wdt) if ctx.needs_input_grad[1] else None), gw, gb, None, None, None, None, None
@@ -861,16 +771,10 @@ def linear_bn_act(x, weight, bn, negative_slope=1.0):
     lib = _lib.load()
     M, K = x.shape
     N = weight.shape[0]
-    training = bn.training or (bn.running_mean is None and bn.running_var is None)
-    if not (training and x.is_cuda and M > 0 and K % 4 == 0 and lib.dva_linear_bnstats_supported(M, N, K)):
+    if not (_uses_batch_stats(bn) and x.is_cuda and M > 0 and K % 4 == 0
+            and lib.dva_linear_bnstats_supported(M, N, K)):
         return batch_norm_act(linear(x, weight), bn, negative_slope=negative_slope)
-    momentum = 0.0 if bn.momentum is None else bn.momentum
-    if bn.training and bn.track_running_stats and bn.num_batches_tracked is not None:
-        bn.num_batches_tracked.add_(1)
-        if bn.momentum is None:
-            momentum = 1.0 / float(bn.num_batches_tracked)
-    rm = bn.running_mean if bn.track_running_stats else None
-    rv = bn.running_var if bn.track_running_stats else None
+    rm, rv, momentum = _bn_step(bn)
     if (_MLP_LAYER_FUSED["on"] and K <= _MLP_LAYER_FUSED["max_k"] and lib.dva_mlp_layer_bwd_supported(M, N, K)
             and torch.is_grad_enabled()
             and (x.requires_grad or weight.requires_grad)):
@@ -916,31 +820,31 @@ def mapping_image_stats(images, atomic_ptr, pixels, n_img, ref_w=None):
     require_cuda(images, atomic_ptr, pixels)
     if pixels.dtype not in _PIX_CODES:
         raise TypeError(f"mapping pixels must be int16/int32/int64, got {pixels.dtype}")
-    lib = _lib.load()
     dev = images.device
     images, atomic_ptr, pixels = images.long().contiguous(), atomic_ptr.long().contiguous(), pixels.contiguous()
     count = torch.empty(n_img, dtype=torch.long, device=dev)
     bbox = torch.empty((n_img, 4), dtype=torch.int32, device=dev)
     occ = torch.empty((n_img, 8), dtype=torch.int32, device=dev) if ref_w is not None else None
-    with torch.cuda.device(dev):
-        check(lib.dva_mapping_image_stats(ptr(images), ptr(atomic_ptr), ptr(pixels), _PIX_CODES[pixels.dtype],
-                                          int(images.shape[0]), int(n_img), int(ref_w or 0), ptr(count), ptr(bbox),
-                                          ptr(occ), stream_ptr()), "dva_mapping_image_stats")
+    launch("dva_mapping_image_stats", dev, images, atomic_ptr, pixels, _PIX_CODES[pixels.dtype], int(images.shape[0]),
+           int(n_img), int(ref_w or 0), count, bbox, occ)
     return count, bbox, occ
 
 
 def center_roll(occ, angular_res, ref_w):
     """Rollings [n] int64 of CenterRoll from the occupancy of mapping_image_stats (image.py:1009-1029)."""
     require_cuda(occ)
-    lib = _lib.load()
     out = torch.empty(occ.shape[0], dtype=torch.long, device=occ.device)
-    with torch.cuda.device(occ.device):
-        check(lib.dva_center_roll(ptr(occ.contiguous()), int(occ.shape[0]), int(angular_res), int(ref_w), ptr(out),
-                                  stream_ptr()), "dva_center_roll")
+    launch("dva_center_roll", occ.device, occ.contiguous(), int(occ.shape[0]), int(angular_res), int(ref_w), out)
     return out
 
 
 _REMAP_ELEM = (1, 2, 4)
+
+
+def _memory_format(x):
+    """channels_last when x is channels-last and not also contiguous (C == 1 or H == W == 1), else contiguous"""
+    cl = (not x.is_contiguous()) and x.is_contiguous(memory_format=torch.channels_last)
+    return torch.channels_last if cl else torch.contiguous_format
 
 
 def image_remap(x, out_hw=None, rolls=None, offsets=None, flip=False):
@@ -954,16 +858,13 @@ def image_remap(x, out_hw=None, rolls=None, offsets=None, flip=False):
                         f"{x.dtype}")
     B, C, H, W = x.shape
     Ho, Wo = (H, W) if out_hw is None else (int(out_hw[0]), int(out_hw[1]))
-    cl = (not x.is_contiguous()) and x.is_contiguous(memory_format=torch.channels_last)
-    fmt = torch.channels_last if cl else torch.contiguous_format
+    fmt = _memory_format(x)
     x = x.contiguous(memory_format=fmt)
     out = torch.empty((B, C, Ho, Wo), dtype=x.dtype, device=x.device, memory_format=fmt)
     rolls = rolls.to(x.device, torch.long).contiguous() if rolls is not None else None
     offsets = offsets.to(x.device, torch.long).contiguous() if offsets is not None else None
-    lib = _lib.load()
-    with torch.cuda.device(x.device):
-        check(lib.dva_image_remap(ptr(x), ptr(out), B, C, H, W, Ho, Wo, x.element_size(), int(cl), ptr(rolls),
-                                  ptr(offsets), int(bool(flip)), stream_ptr()), "dva_image_remap")
+    launch("dva_image_remap", x.device, x, out, B, C, H, W, Ho, Wo, x.element_size(), int(fmt == torch.channels_last),
+           rolls, offsets, int(bool(flip)))
     return out
 
 
@@ -975,23 +876,18 @@ class CoverageIndex:
 
     def __init__(self, gimg, vpoint, n_img, num_points):
         require_cuda(gimg, vpoint)
-        lib = _lib.load()
         self.dev = gimg.device
         self.V, self.n_img, self.N = int(gimg.shape[0]), int(n_img), int(num_points)
-        self.ws_bytes = int(lib.dva_coverage_index_workspace_bytes(self.V, self.n_img, self.N))
-        self.ws = torch.empty(self.ws_bytes, dtype=torch.uint8, device=self.dev)
+        self.ws = _lib.workspace(_lib.load().dva_coverage_index_workspace_bytes(self.V, self.n_img, self.N), self.dev)
         self.unseen = torch.empty(self.n_img, dtype=torch.int32, device=self.dev)
         self.seen = torch.empty(max(self.N, 1), dtype=torch.int32, device=self.dev)
         self._gimg, self._vpoint = gimg.long().contiguous(), vpoint.long().contiguous()
-        with torch.cuda.device(self.dev):
-            check(lib.dva_coverage_index(ptr(self._gimg), ptr(self._vpoint), self.V, self.n_img, self.N,
-                                         ptr(self.unseen), ptr(self.seen), ptr(self.ws), self.ws_bytes, stream_ptr()),
-                  "dva_coverage_index")
+        launch("dva_coverage_index", self.dev, self._gimg, self._vpoint, self.V, self.n_img, self.N, self.unseen,
+               self.seen, self.ws, self.ws.numel())
 
     def pick(self, g):
-        with torch.cuda.device(self.dev):
-            check(_lib.load().dva_coverage_pick(int(g), self.V, self.n_img, self.N, ptr(self.unseen), ptr(self.seen),
-                                                ptr(self.ws), self.ws_bytes, stream_ptr()), "dva_coverage_pick")
+        launch("dva_coverage_pick", self.dev, int(g), self.V, self.n_img, self.N, self.unseen, self.seen, self.ws,
+               self.ws.numel())
 
 
 # --------------------------------------------------------------------------------------------
@@ -1097,11 +993,8 @@ def image_resample(src, size, boxes=None):
     xb_d, xc_d = (d(xb), d(xc)) if need_h else (None, None)
     yb_d, yc_d = (d(yb), d(yc)) if need_v else (None, None)
     yf_d = d(yfirst) if yfirst is not None else None
-    lib = _lib.load()
-    with torch.cuda.device(dev):
-        check(lib.dva_resample_u8(ptr(nhwc), ptr(tmp), ptr(out), B, Hi, Wi, C, Ho, Wo, T, ptr(xb_d), ptr(xc_d),
-                                  int(xc.shape[2]), int(not shared), ptr(yb_d), ptr(yc_d), int(yc.shape[2]),
-                                  int(not shared), ptr(yf_d), stream_ptr()), "dva_resample_u8")
+    launch("dva_resample_u8", dev, nhwc, tmp, out, B, Hi, Wi, C, Ho, Wo, T, xb_d, xc_d, int(xc.shape[2]),
+           int(not shared), yb_d, yc_d, int(yc.shape[2]), int(not shared), yf_d)
     return out.permute(0, 3, 1, 2)
 
 
@@ -1114,9 +1007,7 @@ def nonstatic_mask(imgs):
     n, C, H, W = (int(v) for v in imgs.shape)
     nhwc = imgs.permute(0, 2, 3, 1).contiguous()
     mask = torch.empty((W, H), dtype=torch.bool, device=imgs.device)
-    lib = _lib.load()
-    with torch.cuda.device(imgs.device):
-        check(lib.dva_nonstatic_mask(ptr(nhwc), n, H, W, C, ptr(mask), stream_ptr()), "dva_nonstatic_mask")
+    launch("dva_nonstatic_mask", imgs.device, nhwc, n, H, W, C, mask)
     return mask
 
 
@@ -1125,12 +1016,6 @@ def nonstatic_mask(imgs):
 # (csrc/image_color.cu)
 # --------------------------------------------------------------------------------------------
 _JITTER_CODES = {"brightness": 0, "contrast": 1, "saturation": 2}
-
-
-def _memory_format(x):
-    """channels_last when x is channels-last and not also contiguous (C == 1 or H == W == 1), else contiguous"""
-    cl = (not x.is_contiguous()) and x.is_contiguous(memory_format=torch.channels_last)
-    return torch.channels_last if cl else torch.contiguous_format
 
 
 def color_jitter_u8(x, ops_seq):
@@ -1152,12 +1037,9 @@ def color_jitter_u8(x, ops_seq):
         args += [float(factor), float(1.0 - float(factor))]   # 1 - ratio in float64, rounded to fp32 by ctypes
     args += [0.0, 0.0] * (3 - len(ops_seq))
     B, _, H, W = (int(v) for v in x.shape)
-    lib = _lib.load()
-    ws_bytes = int(lib.dva_color_jitter_u8_workspace_bytes(B))
-    ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=x.device)
-    with torch.cuda.device(x.device):
-        check(lib.dva_color_jitter_u8(ptr(x), ptr(out), B, H, W, int(fmt == torch.channels_last), len(ops_seq), codes,
-                                      *args, ptr(ws), ws_bytes, stream_ptr()), "dva_color_jitter_u8")
+    ws = _lib.workspace(_lib.load().dva_color_jitter_u8_workspace_bytes(B), x.device)
+    launch("dva_color_jitter_u8", x.device, x, out, B, H, W, int(fmt == torch.channels_last), len(ops_seq), codes,
+           *args, ws, ws.numel())
     return out
 
 
@@ -1188,8 +1070,6 @@ def image_to_float(x, mean=None, std=None):
     x = x.contiguous(memory_format=fmt)
     out = torch.empty(x.shape, dtype=torch.float32, device=x.device, memory_format=fmt)
     B, _, H, W = (int(v) for v in x.shape)
-    lib = _lib.load()
-    with torch.cuda.device(x.device):
-        check(lib.dva_image_to_float(ptr(x), int(x.dtype == torch.uint8), ptr(out), B, C, H, W,
-                                     int(fmt == torch.channels_last), *m, *s, stream_ptr()), "dva_image_to_float")
+    launch("dva_image_to_float", x.device, x, int(x.dtype == torch.uint8), out, B, C, H, W,
+           int(fmt == torch.channels_last), *m, *s)
     return out
