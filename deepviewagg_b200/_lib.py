@@ -61,6 +61,8 @@ SIGNATURES = {
     "dva_knn_cell_ids": (_i32, [_vp, _vp, _i64, _f32, _f32, _f32, _f32, _i32, _i32, _i32, _vp]),
     "dva_knn_grid": (_i32, [_vp, _vp, _vp, _vp, _i64, _i32, _f32, _f32, _f32, _f32, _i32, _i32, _i32,
                             _vp, _vp, _vp]),
+    "dva_knn_query": (_i32, [_vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _i64, _i32, _f32, _f32, _f32, _f32, _i32,
+                             _i32, _i32, _vp, _vp, _vp]),
     "dva_neighborhood_features": (_i32, [_vp, _vp, _i32, _vp, _vp, _vp, _vp, _i32, _f64, _i32, _i32, _vp,
                                          _i64, _i64, _vp]),
     "dva_scatter_add_rows": (_i32, [_vp, _vp, _vp, _i64, _i64, _i64, _i32, _vp]),
@@ -105,6 +107,9 @@ SIGNATURES = {
     "dva_color_jitter_u8": (_i32, [_vp, _vp, _i64, _i64, _i64, _i32, _i32, _i32, _f32, _f32, _f32, _f32, _f32, _f32,
                                    _vp, _sz, _vp]),
     "dva_image_to_float": (_i32, [_vp, _i32, _vp, _i64, _i64, _i64, _i64, _i32] + [_f32] * 8 + [_vp]),
+    "dva_csr_nll_fwd_workspace_bytes": (_sz, [_i64]),
+    "dva_csr_nll_fwd": (_i32, [_vp, _i32, _vp, _vp, _i64, _i64, _i32, _i64, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "dva_csr_nll_bwd": (_i32, [_vp, _i32, _vp, _vp, _i64, _i64, _i32, _i64, _vp, _vp, _vp, _vp, _vp]),
     "dva_csr_pointers_from_sorted": (_i32, [_vp, _vp, _i64, _i64, _vp]),
     "dva_csr_select_values": (_i32, [_vp, _vp, _vp, _vp, _i64, _i64, _vp]),
 }

@@ -133,22 +133,13 @@ def _grid_for(pos, cell_size):
         cell_size *= 1.26
 
 
-def knn_grid(pos, k, cell_size=None, return_dist2=False):
-    """Exact k nearest neighbours (self included, 1 <= k <= 128) of every point among all points,
-    on CUDA (replaces the KeOps `argKmin` of image.py:504-514 and visibility.py:1439-1444).
-    Squared distances are (dx*dx + dy*dy) + dz*dz in fp32, ties ordered by point index; points
-    with z = 0 give the exact 2D distance (image-plane search).  Returns neighbors [N,k] int64
-    (ascending distance) and optionally the squared distances."""
+def _knn_search_grid(pos, k, cell_size=None):
+    """Uniform grid over the search set `pos` [n,3] fp32 (CUDA, contiguous) shared by knn_grid and
+    knn_query: returns (lo, dims, cell_size, cell_s, order, cell_ptr, xyz_s), the points sorted by
+    cell, order[j] = original index of sorted slot j, cell_ptr [gx*gy*gz+1]."""
     from ..._lib import launch
     from .csr import pointers_from_sorted
-    if not pos.is_cuda:
-        raise RuntimeError("knn_grid runs on CUDA tensors only (no CPU fallback)")
-    pos = pos.float().contiguous()
     n = pos.shape[0]
-    if not 1 <= k <= 128:
-        raise ValueError("knn_grid: k must be in [1, 128]")
-    if n < k:
-        raise ValueError(f"knn_grid: need at least k={k} points, got {n}")
     cell = torch.empty(n, dtype=torch.int64, device=pos.device)
 
     def assign(cs):
@@ -181,10 +172,73 @@ def knn_grid(pos, k, cell_size=None, return_dist2=False):
     cell_s, order = torch.sort(cell, stable=True)
     cell_ptr = pointers_from_sorted(cell_s, dims[0] * dims[1] * dims[2])
     xyz_s = pos[order].contiguous()
+    return lo, dims, cell_size, cell_s, order, cell_ptr, xyz_s
+
+
+def knn_grid(pos, k, cell_size=None, return_dist2=False):
+    """Exact k nearest neighbours (self included, 1 <= k <= 128) of every point among all points,
+    on CUDA (replaces the KeOps `argKmin` of image.py:504-514 and visibility.py:1439-1444).
+    Squared distances are (dx*dx + dy*dy) + dz*dz in fp32, ties ordered by point index; points
+    with z = 0 give the exact 2D distance (image-plane search).  Returns neighbors [N,k] int64
+    (ascending distance) and optionally the squared distances."""
+    from ..._lib import launch
+    if not pos.is_cuda:
+        raise RuntimeError("knn_grid runs on CUDA tensors only (no CPU fallback)")
+    pos = pos.float().contiguous()
+    n = pos.shape[0]
+    if not 1 <= k <= 128:
+        raise ValueError("knn_grid: k must be in [1, 128]")
+    if n < k:
+        raise ValueError(f"knn_grid: need at least k={k} points, got {n}")
+    lo, dims, cell_size, cell_s, order, cell_ptr, xyz_s = _knn_search_grid(pos, k, cell_size)
     nbr = torch.empty((n, k), dtype=torch.int64, device=pos.device)
     d2 = torch.empty((n, k), dtype=torch.float32, device=pos.device) if return_dist2 else None
     launch("dva_knn_grid", pos.device, xyz_s, cell_s, order, cell_ptr, n, k, lo[0], lo[1], lo[2], cell_size, dims[0],
            dims[1], dims[2], nbr, d2)
+    return (nbr, d2) if return_dist2 else nbr
+
+
+_KNN_BLOCK = 8      # fine cells per coarse block and axis (csrc/knn_features.cu kKnnBlk)
+
+
+def knn_query(query, search, k, cell_size=None, return_dist2=False):
+    """Exact k nearest neighbours (1 <= k <= 128) of every point of `query` [M,3] among the points
+    of `search` [n,3], on CUDA (replaces the KeOps brute-force `argmin` of
+    models/segmentation/multimodal/no3d.py:105-125).  Same arithmetic and tie order as knn_grid:
+    (dx*dx + dy*dy) + dz*dz in fp32, ties to the lower search index; knn_query(p, p, k) equals
+    knn_grid(p, k).  The grid is built over the search set; a query far from every search point
+    walks a coarse level of 8^3-cell blocks that skips empty space, so it never scans the whole
+    set.  Returns neighbors [M,k] int64 (search indices, ascending distance) and optionally the
+    squared distances."""
+    from ..._lib import launch
+    if not (query.is_cuda and search.is_cuda):
+        raise RuntimeError("knn_query runs on CUDA tensors only (no CPU fallback)")
+    if query.device != search.device:
+        raise RuntimeError("knn_query: query and search must live on the same device")
+    if not 1 <= k <= 128:
+        raise ValueError("knn_query: k must be in [1, 128]")
+    search = search.float().contiguous()
+    query = query.float().contiguous()
+    m, n = query.shape[0], search.shape[0]
+    nbr = torch.empty((m, k), dtype=torch.int64, device=query.device)
+    d2 = torch.empty((m, k), dtype=torch.float32, device=query.device) if return_dist2 else None
+    if m == 0:
+        return (nbr, d2) if return_dist2 else nbr
+    if n < k:
+        raise ValueError(f"knn_query: need at least k={k} search points, got {n}")
+    lo, dims, cell_size, _, order, cell_ptr, xyz_s = _knn_search_grid(search, k, cell_size)
+    gx, gy, gz = dims
+    B = _KNN_BLOCK
+    counts = (cell_ptr[1:] - cell_ptr[:-1]).view(gz, gy, gx)
+    counts = torch.nn.functional.pad(counts, (0, (-gx) % B, 0, (-gy) % B, 0, (-gz) % B))
+    GZ, GY, GX = counts.shape[0] // B, counts.shape[1] // B, counts.shape[2] // B
+    blocks = counts.view(GZ, B, GY, B, GX, B).sum(dim=(1, 3, 5)).to(torch.int32).contiguous()
+    qcell = torch.empty(m, dtype=torch.int64, device=query.device)
+    launch("dva_knn_cell_ids", query.device, query, qcell, m, lo[0], lo[1], lo[2], cell_size, gx, gy, gz)
+    qcell_s, qorder = torch.sort(qcell, stable=True)
+    q_s = query[qorder].contiguous()
+    launch("dva_knn_query", query.device, q_s, qcell_s, qorder, m, xyz_s, order, cell_ptr, blocks, n, k, lo[0], lo[1],
+           lo[2], cell_size, gx, gy, gz, nbr, d2)
     return (nbr, d2) if return_dist2 else nbr
 
 

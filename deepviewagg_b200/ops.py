@@ -1073,3 +1073,76 @@ def image_to_float(x, mean=None, std=None):
     launch("dva_image_to_float", x.device, x, int(x.dtype == torch.uint8), out, B, C, H, W,
            int(fmt == torch.channels_last), *m, *s)
     return out
+
+
+# --------------------------------------------------------------------------------------------
+# log-softmax NLL over a view CSR (models/segmentation/multimodal/no3d.py:144-154; csrc/csr_nll.cu)
+# --------------------------------------------------------------------------------------------
+CSR_NLL_MAX_CLASSES = 64
+
+
+class _CSRNLLLoss(torch.autograd.Function):
+    @staticmethod
+    @_fwd
+    def forward(ctx, logits, labels, csr_idx, ignore_index):
+        V, K = logits.shape
+        N = labels.shape[0]
+        need_grad = ctx.needs_input_grad[0]
+        loss = torch.empty((), dtype=torch.float32, device=logits.device)
+        stats = torch.empty(3, dtype=torch.int64, device=logits.device)
+        lse = torch.empty(V, dtype=torch.float32, device=logits.device) if need_grad else None
+        ws = _lib.workspace(_lib.load().dva_csr_nll_fwd_workspace_bytes(N), logits.device)
+        launch("dva_csr_nll_fwd", logits.device, logits, dtype_code(logits), labels, csr_idx, V, N, K, int(ignore_index),
+               lse, loss, stats, ws, ws.numel())
+        _, bad, bad_csr = stats.tolist()
+        if bad:
+            raise ValueError(f"csr_nll_loss: {bad} view(s) have a label outside [0, {K}) that is not "
+                             f"ignore_index={ignore_index}")
+        if bad_csr:
+            raise ValueError(f"csr_nll_loss: csr_idx must run from 0 to the number of views ({V})")
+        ctx.cfg = (V, N, K, int(ignore_index))
+        ctx.save_for_backward(logits, labels, csr_idx, lse, stats)
+        return loss
+
+    @staticmethod
+    @_bwd
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_loss):
+        logits, labels, csr_idx, lse, stats = ctx.saved_tensors
+        V, N, K, ignore_index = ctx.cfg
+        grad = torch.empty_like(logits)
+        g = grad_loss.detach().float().contiguous().view(1)
+        launch("dva_csr_nll_bwd", logits.device, logits, dtype_code(logits), labels, csr_idx, V, N, K, ignore_index,
+               lse, g, stats, grad)
+        return grad, None, None, None
+
+
+def csr_nll_loss(logits, labels, csr_idx=None, ignore_index=-1):
+    """F.nll_loss(F.log_softmax(logits, -1), repeat_interleave(labels, csr_idx.diff()),
+    ignore_index=ignore_index) with the mean reduction (no3d.py:144-154), without the [V] target
+    and [V, K] log-prob tensors: view v takes the label of its point through the CSR.
+
+    logits [V, K] fp32 / bf16 / fp16 (fp32 math, K <= 64), labels [N] int64, csr_idx [N+1] int64 or
+    None for one view per point (V == N, the point-level loss).  Returns a float32 scalar: the mean
+    over views whose label is in [0, K) (NaN when there is none, as F.nll_loss); the sum is taken in
+    fp64 in a fixed order, so two calls give the same bits.  A label outside [0, K) that is not
+    ignore_index raises ValueError (read back after the forward; no device assert)."""
+    require_cuda(logits, labels, csr_idx)
+    if logits.dim() != 2:
+        raise ValueError(f"csr_nll_loss: logits must be [V, K], got shape {tuple(logits.shape)}")
+    if logits.dtype not in DTYPE_CODES:
+        raise TypeError(f"csr_nll_loss: unsupported logits dtype {logits.dtype}; expected float32/bfloat16/float16")
+    V, K = logits.shape
+    if not 1 <= K <= CSR_NLL_MAX_CLASSES:
+        raise ValueError(f"csr_nll_loss: {K} classes; this kernel supports 1 to {CSR_NLL_MAX_CLASSES}")
+    if labels.dim() != 1 or labels.dtype != torch.int64:
+        raise TypeError("csr_nll_loss: labels must be a 1D int64 tensor")
+    if csr_idx is None:
+        if labels.shape[0] != V:
+            raise ValueError(f"csr_nll_loss: without csr_idx, labels ({labels.shape[0]}) and logits ({V}) must "
+                             f"have one row per point")
+    else:
+        csr_idx = _check_csr(csr_idx, logits.device)
+        if csr_idx.numel() != labels.shape[0] + 1:
+            raise ValueError("csr_nll_loss: csr_idx must have one more entry than labels")
+    return _CSRNLLLoss.apply(logits.contiguous(), labels.contiguous(), csr_idx, ignore_index)

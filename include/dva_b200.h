@@ -226,6 +226,18 @@ int dva_interp_pool_bwd_det(const void* grad_out, int channels_last, const int64
  *                      inputs (z = 0) give the exact 2D squared distance (image-plane k-NN).
  *                      neighbors [n,k] int64 and dist2 [n,k] (nullable) are indexed by
  *                      ORIGINAL point id, ascending (dist2, id).
+ *   dva_knn_query    : the same search for a query set among a separate search set; replaces the
+ *                      KeOps brute-force `argmin` of models/segmentation/multimodal/no3d.py:105-125
+ *                      (nearest seen point of every unseen point).  The grid (origin, cell_size,
+ *                      gx x gy x gz) is built over the search set: search_sorted / search_order /
+ *                      cell_ptr as for dva_knn_grid.  Queries are cell-sorted too: query_cell_sorted
+ *                      from dva_knn_cell_ids on the same grid (clamped, so queries outside it fall in
+ *                      a border cell), query_order [nq] their original ids.  block_counts
+ *                      [ceil(gz/8)*ceil(gy/8)*ceil(gx/8)] int32 = search points per block of 8^3
+ *                      cells: a query still open after 6 fine shells walks shells of non-empty
+ *                      blocks, so far queries do not scan the search set.  Same arithmetic and tie
+ *                      order as dva_knn_grid; neighbors [nq,k] (search ids) and dist2 (nullable) are
+ *                      indexed by ORIGINAL query id.  nq == 0 launches nothing; ns < k is DVA_EINVAL.
  *   dva_neighborhood_features : out [V, nk*(density + occlusion)] fp32 = for every k of the
  *                      ascending klist: density of the view's point ((k+1)/(3.1416 d_k^2)/(1/voxel^2),
  *                      NaN -> 1, :527-537), then occlusion of the view ((1 + #neighbours seen by
@@ -238,6 +250,11 @@ int dva_knn_grid(const float* xyz_sorted, const int64_t* cell_sorted, const int6
                  const int64_t* cell_ptr, int64_t n, int k, float ox, float oy, float oz,
                  float cell_size, int gx, int gy, int gz, int64_t* neighbors, float* dist2,
                  void* stream);
+int dva_knn_query(const float* query_sorted, const int64_t* query_cell_sorted, const int64_t* query_order,
+                  int64_t nq, const float* search_sorted, const int64_t* search_order,
+                  const int64_t* cell_ptr, const int32_t* block_counts, int64_t ns, int k, float ox,
+                  float oy, float oz, float cell_size, int gx, int gy, int gz, int64_t* neighbors,
+                  float* dist2, void* stream);
 int dva_neighborhood_features(const float* xyz, const int64_t* neighbors, int kmax,
                               const int64_t* view_ptr, const int64_t* images,
                               const int64_t* view_point, const int32_t* klist, int nk,
@@ -507,6 +524,29 @@ int dva_color_jitter_u8(const uint8_t* in, uint8_t* out, int64_t B, int64_t H, i
 int dva_image_to_float(const void* in, int in_u8, float* out, int64_t B, int64_t C, int64_t H, int64_t W,
                        int channels_last, float m0, float m1, float m2, float m3, float s0, float s1, float s2,
                        float s3, void* stream);
+
+/* L1  log-softmax NLL over a view CSR           replaces models/segmentation/multimodal/no3d.py:144-154
+ *   F.nll_loss(F.log_softmax(head(last_view_x_mod)), repeat_interleave(labels, counts), ignore_index=-1),
+ *   mean reduction, without the [V] target and [V, K] log-prob tensors.  logits [V, K] (fp32 / bf16 / fp16
+ *   storage, fp32 math, 1 <= K <= 64, else DVA_EUNSUPPORTED), labels [N] int64, csr_idx [N+1] int64 (view v
+ *   belongs to point p for csr_idx[p] <= v < csr_idx[p+1]) or NULL for V == N (one view per point).
+ *   A view counts when its label lies in [0, K) and is not ignore_index.
+ *   dva_csr_nll_fwd : loss[0] = mean over counted views of lse - x[label] (NaN when none counts), from
+ *                     per-CTA fp64 partials (dva_csr_nll_fwd_workspace_bytes(N) bytes of workspace) summed in
+ *                     a fixed order; lse [V] fp32 (nullable) = log-sum-exp of each row, for the backward;
+ *                     stats [3] int64 = {counted views, views whose label is neither ignore_index nor in
+ *                     [0, K), 1 if csr_idx does not run from 0 to V}.  Such labels and rows are never read
+ *                     through; the caller raises on stats[1] / stats[2].
+ *   dva_csr_nll_bwd : grad_logits [V, K] (logits' dtype) = grad_loss[0] / stats[0] * (exp(x - lse) - onehot),
+ *                     0 on views that do not count; every element is written.
+ *   Bytes: the forward reads the logits once, the backward reads them once and writes the gradient once. */
+size_t dva_csr_nll_fwd_workspace_bytes(int64_t N);
+int dva_csr_nll_fwd(const void* logits, int dtype, const int64_t* labels, const int64_t* csr_idx, int64_t V,
+                    int64_t N, int K, int64_t ignore_index, float* lse, float* loss, int64_t* stats,
+                    void* workspace, size_t workspace_bytes, void* stream);
+int dva_csr_nll_bwd(const void* logits, int dtype, const int64_t* labels, const int64_t* csr_idx, int64_t V,
+                    int64_t N, int K, int64_t ignore_index, const float* lse, const float* grad_loss,
+                    const int64_t* stats, void* grad_logits, void* stream);
 
 /* C1  CSR pointers from sorted dense ids     replaces csr.py:158-172 + :197-229
  *   ids [n] int64 sorted ascending, values in [0,num_groups) -> ptr [num_groups+1] int64 with
