@@ -185,7 +185,7 @@ view_attention_fwd_kernel(const VAParams P) {
     const bool one_chunk = n <= 32;
     const SegStats st = seg_softmax_stats(cp, nG, G, lane, inv_sq, one_chunk, att_s);
     const float den = st.den + P.eps;
-    const float t = gating ? tanhf(fmaxf(fmaf(gw, st.m, gb), 0.f)) : 1.f;
+    const float t = gating ? gate_t(fmaf(gw, st.m, gb)) : 1.f;
     if (lane < G && P.seg_max != nullptr) {
       P.seg_max[i * G + lane] = st.m;
       P.seg_den[i * G + lane] = den;
@@ -387,7 +387,7 @@ view_attention_bwd_kernel(const VAParams P) {
     const int arg_v = P.s_arg[i * G + gl];
     const float inv_sq = P.group_scaling ? rsqrtf((float)n) : 1.f;
     const float z = fmaf(gw, m, gb);
-    const float t = gating ? tanhf(fmaxf(z, 0.f)) : 1.f;
+    const float t = gating ? gate_t(z) : 1.f;
     const bool one_chunk = n <= 32;
     float S = 0.f;                            // sum_v a_vg s'_vg for g = lane%G (partial per lane)
 
@@ -525,6 +525,7 @@ view_attention_bwd_kernel(const VAParams P) {
     }
 
     S = group_lane_sum(S, G);
+    // gate_grad() spelled out: through the helper the spilling instantiations of this kernel reload 4 - 12 bytes more
     const float one_m_t2 = 1.f - t * t;
     const float dLdt = (t != 0.f) ? S / t : 0.f;
     const bool open = gating && z > 0.f;
@@ -537,9 +538,7 @@ view_attention_bwd_kernel(const VAParams P) {
       float a, sv;
       if (one_chunk) { const int slot = gl * kTileStride + e / G; a = att_s[slot]; sv = s_s[slot]; }
       else { a = expf((__ldg(cp + e) - m) * inv_sq) * inv_den; sv = gc[e]; }
-      float d = a * (sv - S) * inv_sq;
-      if (p0 + e / G == arg_v) d += dq;
-      gc[e] = d;
+      gc[e] = compat_grad(a, sv, S, inv_sq, p0 + e / G == arg_v, dq);
     }
   }
 
@@ -681,6 +680,43 @@ template <typename T> static int bwd_typed(const VAParams& P, int* grid, cudaStr
   DVA_VA_DISPATCH(launch_bwd, T, cfg, P, cfg.reg, grid, st);
 }
 
+// The G = 4 short-row kernels (ring forward and backward, lane backward) need rows of whole 16-byte chunks, at most
+// 512 bytes, no chunk straddling a channel group; x, the scores and the row outputs o1 / o2 16-byte aligned; and
+// V < 2^31, R < 2^32 (32-bit view and row ids).
+template <typename T>
+static bool short_rows_ok(const VAParams& P, const void* o1, const void* o2) {
+  constexpr int V16 = Vec16<T>::N;
+  const int C = P.C, G = P.G;
+  if (G != 4) return false;
+  if (C % V16 != 0 || C / V16 > 32) return false;
+  if (!aligned16(P.x) || !aligned16(o1) || (o2 != nullptr && !aligned16(o2))) return false;
+  if (!aligned16(P.compat)) return false;
+  if (P.V >= (1ll << 31) || P.R >= (1ll << 32)) return false;
+  for (int c0 = 0; c0 < C; c0 += V16)
+    if (group_of_channel(c0, C, G) != group_of_channel(c0 + V16 - 1, C, G)) return false;
+  return true;
+}
+// ring forward: aligned attention and statistics outputs
+static bool ring_fwd_applicable(const VAParams& P, int dtype) {
+  if (!with_dtype(dtype, [&](auto tag) { return short_rows_ok<decltype(tag)>(P, P.out, nullptr); })) return false;
+  if (P.att != nullptr && !aligned16(P.att)) return false;
+  if (P.seg_max != nullptr && (!aligned16(P.seg_max) || !aligned16(P.seg_den) || !aligned16(P.seg_arg))) return false;
+  return true;
+}
+// ring and lane backward (the same conditions): the regular layout -- equal groups of a power-of-two number of
+// chunks, so a row is exactly LPR = 4, 8, 16 or 32 chunks -- and aligned saved statistics and grad_compat
+static bool short_bwd_applicable(const VAParams& P, int dtype) {
+  return with_dtype(dtype, [&](auto tag) {
+    using T = decltype(tag);
+    constexpr int V16 = Vec16<T>::N;
+    if (!short_rows_ok<T>(P, P.gout, P.gx)) return false;
+    if (P.C % P.G != 0 || (P.C / P.G) % V16 != 0) return false;
+    const int cpg = (P.C / P.G) / V16;
+    if ((cpg & (cpg - 1)) != 0) return false;
+    return aligned16(P.s_max) && aligned16(P.s_den) && aligned16(P.s_arg) && aligned16(P.gcompat);
+  });
+}
+
 static bool pow2_le32(int64_t g) { return g >= 1 && g <= 32 && (g & (g - 1)) == 0; }
 
 // 0 = auto, 1 = streaming kernels, 2 = ring kernels (when applicable).  Process-wide tuning knob
@@ -752,13 +788,8 @@ extern "C" int dva_view_attention_fwd(const void* x, const void* idx, int idx_is
   P.N = N; P.V = V; P.R = R; P.C = (int)C; P.G = (int)G; P.group_scaling = group_scaling; P.eps = eps;
   cudaStream_t st = (cudaStream_t)stream;
   if (dtype != DVA_F32 && dtype != DVA_BF16 && dtype != DVA_F16) return fail(DVA_EINVAL, "view_attention_fwd: unknown dtype");
-  if (use_ring(P, dtype, va_ring_fwd_applicable(P, dtype), false)) return va_ring_fwd(P, dtype, st);
-  switch (dtype) {
-    case DVA_F32: return fwd_typed<float>(P, st);
-    case DVA_BF16: return fwd_typed<__nv_bfloat16>(P, st);
-    case DVA_F16: return fwd_typed<__half>(P, st);
-    default: return fail(DVA_EINVAL, "view_attention_fwd: unknown dtype");
-  }
+  if (use_ring(P, dtype, ring_fwd_applicable(P, dtype), false)) return va_ring_fwd(P, dtype, st);
+  return with_dtype(dtype, [&](auto tag) { return fwd_typed<decltype(tag)>(P, st); });
 }
 
 extern "C" int dva_view_attention_set_path(int path) {
@@ -806,16 +837,13 @@ extern "C" int dva_view_attention_bwd(const void* x, const void* idx, int idx_is
   int grid = 1;
   int rc;
   if (dtype != DVA_F32 && dtype != DVA_BF16 && dtype != DVA_F16) return fail(DVA_EINVAL, "view_attention_bwd: unknown dtype");
-  if (use_ring(P, dtype, va_ring_bwd_applicable(P, dtype), true)) {
+  const bool short_rows = short_bwd_applicable(P, dtype);
+  if (use_ring(P, dtype, short_rows, true)) {
     rc = va_ring_bwd(P, dtype, &grid, st);
-  } else if (use_lane_bwd(P, va_lane_bwd_applicable(P, dtype))) {
+  } else if (use_lane_bwd(P, short_rows)) {
     rc = va_lane_bwd(P, dtype, &grid, st);
   } else {
-    switch (dtype) {
-      case DVA_F32: rc = bwd_typed<float>(P, &grid, st); break;
-      case DVA_BF16: rc = bwd_typed<__nv_bfloat16>(P, &grid, st); break;
-      default: rc = bwd_typed<__half>(P, &grid, st); break;
-    }
+    rc = with_dtype(dtype, [&](auto tag) { return bwd_typed<decltype(tag)>(P, &grid, st); });
   }
   if (rc) return rc;
   if (gating) {

@@ -1,11 +1,16 @@
-// Shared between the two implementations of the fused view-attention pair:
-//   view_attention.cu       streaming kernels (row chunks live in registers; best for long segments
-//                           of >= 512-byte rows)
-//   view_attention_ring.cu  ring kernels (rows staged in shared memory by cp.async / bulk copies,
-//                           several batches in flight per warp across point boundaries; best for
+// Shared between the three implementations of the fused view-attention pair:
+//   view_attention.cu       streaming kernels, forward and backward (row chunks live in registers; best for
+//                           long segments of >= 512-byte rows); host dispatch and the C ABI
+//   view_attention_ring.cu  ring kernels, forward and backward (rows staged in shared memory by cp.async /
+//                           bulk copies, several batches in flight per warp across point boundaries; best for
 //                           short segments and rows <= 512 bytes)
+//   view_attention_lane.cu  lane-per-view backward (a warp takes a group of points holding <= 32 views; rows
+//                           by bulk copy, one per view lane)
+// The per-point arithmetic below is written once for all of them; the attention weight itself is not, each
+// kernel keeps its own exp / division form.
 #pragma once
 #include "dva_common.cuh"
+#include <type_traits>
 
 namespace dva {
 
@@ -31,15 +36,156 @@ __device__ __forceinline__ float group_lane_sum(float v, int G) {
   return v;
 }
 
-// ring path (view_attention_ring.cu).  *_applicable: shape / alignment conditions of the ring
-// kernels; the launchers return a DVA_* / cudaError code like every other entry point.
-bool va_ring_fwd_applicable(const VAParams& P, int dtype);
-bool va_ring_bwd_applicable(const VAParams& P, int dtype);
+// ---- shared memory, mbarrier and bulk async copy (ring and lane kernels)
+__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
+__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
+  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
+}
+// makes the initialised barriers visible to the async proxy
+__device__ __forceinline__ void mbar_init_fence() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
+__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
+  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
+  uint32_t ok = 0;
+  while (!ok) {
+    asm volatile(
+        "{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2; selp.u32 %0, 1, 0, p; }"
+        : "=r"(ok) : "r"(bar), "r"(parity) : "memory");
+  }
+}
+__device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+               ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
+}
+__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+
+// x row of view v (identity when there is no index; the host guarantees R < 2^32)
+__device__ __forceinline__ uint32_t load_row_id(const void* idx, int idx64, int64_t v) {
+  if (idx == nullptr) return (uint32_t)v;
+  return idx64 ? (uint32_t) reinterpret_cast<const int64_t*>(idx)[v]
+               : (uint32_t) reinterpret_cast<const int32_t*>(idx)[v];
+}
+__device__ __forceinline__ float sel4(const float4& v, int g) {
+  return g == 0 ? v.x : (g == 1 ? v.y : (g == 2 ? v.z : v.w));
+}
+
+// ---- per-point math of one group g (gradients: see view_attention.cu)
+// gate on the group's max score m: z = w m + b, t = tanh(relu(z))
+__device__ __forceinline__ float gate_t(float z) { return tanhf(fmaxf(z, 0.f)); }
+__device__ __forceinline__ float4 gate_z4(const float4& w, const float4& m, const float4& b) {
+  return make_float4(fmaf(w.x, m.x, b.x), fmaf(w.y, m.y, b.y), fmaf(w.z, m.z, b.z), fmaf(w.w, m.w, b.w));
+}
+__device__ __forceinline__ float4 gate_t4(const float4& z) {
+  return make_float4(gate_t(z.x), gate_t(z.y), gate_t(z.z), gate_t(z.w));
+}
+
+// Gate gradient with S = sum_v a s' (= t dL/dt): 0 while the gate is closed (z <= 0); otherwise
+// u = dL/dt (1 - t^2) and the returned dq = u w flows to the arg-max view's score.  The lanes that `keep` the
+// term also accumulate dw += u m, db += u (lanes holding a copy of the same point's term pass false).
+__device__ __forceinline__ float gate_grad(float S, float z, float t, float w, float m, bool keep, float& dw,
+                                           float& db) {
+  if (!(z > 0.f)) return 0.f;
+  const float dLdt = (t != 0.f) ? S / t : 0.f;
+  const float u = dLdt * (1.f - t * t);
+  const float dq = u * w;
+  if (keep) {
+    dw += u * m;
+    db += u;
+  }
+  return dq;
+}
+__device__ __forceinline__ float4 gate_grad4(const float4& S, const float4& z, const float4& t, const float4& w,
+                                             const float4& m, bool keep, float4& dw, float4& db) {
+  return make_float4(gate_grad(S.x, z.x, t.x, w.x, m.x, keep, dw.x, db.x),
+                     gate_grad(S.y, z.y, t.y, w.y, m.y, keep, dw.y, db.y),
+                     gate_grad(S.z, z.z, t.z, w.z, m.z, keep, dw.z, db.z),
+                     gate_grad(S.w, z.w, t.w, w.w, m.w, keep, dw.w, db.w));
+}
+
+// grad_compat of one view: a (s' - S) / sqrt(n) + [view == arg-max] dq
+__device__ __forceinline__ float compat_grad(float a, float sv, float S, float inv_sq, bool is_arg, float dq) {
+  float d = a * (sv - S) * inv_sq;
+  if (is_arg) d += dq;
+  return d;
+}
+__device__ __forceinline__ float4 compat_grad4(const float4& a, const float4& sv, const float4& S, float inv_sq,
+                                               int v, const int4& arg, const float4& dq) {
+  return make_float4(compat_grad(a.x, sv.x, S.x, inv_sq, v == arg.x, dq.x),
+                     compat_grad(a.y, sv.y, S.y, inv_sq, v == arg.y, dq.y),
+                     compat_grad(a.z, sv.z, S.z, inv_sq, v == arg.z, dq.z),
+                     compat_grad(a.w, sv.w, S.w, inv_sq, v == arg.w, dq.w));
+}
+
+// Gate parameter gradients of a G = 4 backward CTA of WARPS warps: lane partials -> warp -> block partial
+// (fixed order, deterministic) -> partial[blockIdx.x][dw0..3, db0..3].  Every thread of the CTA calls it.
+template <int WARPS>
+__device__ __forceinline__ void store_gate_partial(float* __restrict__ partial, const float4& dw, const float4& db) {
+  __shared__ float gate_s[WARPS][8];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  float v[8] = {dw.x, dw.y, dw.z, dw.w, db.x, db.y, db.z, db.w};
+#pragma unroll
+  for (int q = 0; q < 8; ++q) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v[q] += __shfl_xor_sync(0xffffffffu, v[q], o);
+  }
+  if (lane == 0) {
+#pragma unroll
+    for (int q = 0; q < 8; ++q) gate_s[warp][q] = v[q];
+  }
+  __syncthreads();
+  if ((int)threadIdx.x < 8) {
+    float acc = 0.f;
+    for (int w = 0; w < WARPS; ++w) acc += gate_s[w][threadIdx.x];
+    partial[(int64_t)blockIdx.x * 8 + threadIdx.x] = acc;
+  }
+}
+
+// ---- host side
+// f(T{}) with T the storage type of dtype; the C entry points have rejected every other dtype
+template <typename F> decltype(auto) with_dtype(int dtype, F&& f) {
+  switch (dtype) {
+    case DVA_F32: return f(float{});
+    case DVA_BF16: return f(__nv_bfloat16{});
+    default: return f(__half{});
+  }
+}
+// f(std::integral_constant<int, LPR>{}) with LPR the lanes per row of the ring and lane kernels: the smallest of
+// 4, 8, 16, 32 that covers cv 16-byte chunks
+template <typename F> decltype(auto) with_lpr(int cv, F&& f) {
+  if (cv <= 4) return f(std::integral_constant<int, 4>{});
+  if (cv <= 8) return f(std::integral_constant<int, 8>{});
+  if (cv <= 16) return f(std::integral_constant<int, 16>{});
+  return f(std::integral_constant<int, 32>{});
+}
+
+// Persistent grid of the ring and lane kernels, whose warps stride over ranges of PR points: the co-resident CTAs
+// (kNumSMs x occupancy, at most max_ctas_per_sm), about ranges_per_warp ranges per warp and never fewer than 8
+// points per range, and no more CTAs than there are ranges.
+template <typename K>
+int range_geometry(K kern, size_t smem, int warps_per_cta, int max_ctas_per_sm, int ranges_per_warp, int64_t N,
+                   const char* what, int* grid_out, int* pr_out) {
+  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (e != cudaSuccess) return failf((int)e, "%s: %zu bytes of shared memory: %s", what, smem, cudaGetErrorString(e));
+  int occ = 0;
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, warps_per_cta * 32, smem) != cudaSuccess || occ < 1) occ = 1;
+  if (occ > max_ctas_per_sm) occ = max_ctas_per_sm;
+  int64_t grid = (int64_t)kNumSMs * occ;
+  const int64_t slots = grid * warps_per_cta * ranges_per_warp;
+  int64_t pr = (N + slots - 1) / slots;
+  if (pr < 8) pr = 8;
+  const int64_t n_ranges = (N + pr - 1) / pr;
+  const int64_t need = (n_ranges + warps_per_cta - 1) / warps_per_cta;
+  if (grid > need) grid = need;
+  if (grid < 1) grid = 1;
+  *grid_out = (int)grid; *pr_out = (int)pr;
+  return DVA_OK;
+}
+
+// ring kernels (view_attention_ring.cu) and lane-per-view backward (view_attention_lane.cu); the launchers return a
+// DVA_* / cudaError code like every other entry point.  Shape / alignment conditions: view_attention.cu.
 int va_ring_fwd(const VAParams& P, int dtype, cudaStream_t st);
 int va_ring_bwd(const VAParams& P, int dtype, int* grid_out, cudaStream_t st);
-
-// lane-per-view backward for short segments (view_attention_lane.cu)
-bool va_lane_bwd_applicable(const VAParams& P, int dtype);
 int va_lane_bwd(const VAParams& P, int dtype, int* grid_out, cudaStream_t st);
 
 }  // namespace dva

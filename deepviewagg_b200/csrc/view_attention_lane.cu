@@ -33,33 +33,6 @@ namespace dva {
 constexpr int kLaneWarps = 4;
 constexpr uint32_t kFull = 0xffffffffu;
 
-__device__ __forceinline__ uint32_t lane_smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void lane_mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
-}
-__device__ __forceinline__ void lane_mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void lane_mbar_wait(uint32_t bar, uint32_t parity) {
-  uint32_t ok = 0;
-  while (!ok) {
-    asm volatile(
-        "{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2; selp.u32 %0, 1, 0, p; }"
-        : "=r"(ok) : "r"(bar), "r"(parity) : "memory");
-  }
-}
-__device__ __forceinline__ void lane_bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-               ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
-}
-__device__ __forceinline__ void lane_fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-
-__device__ __forceinline__ uint32_t lane_row_id(const void* idx, int idx64, int64_t v) {
-  if (idx == nullptr) return (uint32_t)v;
-  return idx64 ? (uint32_t) reinterpret_cast<const int64_t*>(idx)[v] : (uint32_t) reinterpret_cast<const int32_t*>(idx)[v];
-}
-__device__ __forceinline__ float pick4(const float4& v, int g) { return g == 0 ? v.x : (g == 1 ? v.y : (g == 2 ? v.z : v.w)); }
-
 struct LaneSmem {            // per warp
   float wt[32][4];           // a * t per (view, group)
   float at[32][4];           // a
@@ -76,18 +49,17 @@ struct LaneSmem {            // per warp
 template <typename T, int LPR>
 __global__ void __launch_bounds__(kLaneWarps * 32, 5)
 va_lane_bwd_kernel(const VAParams P, const int PR) {
-  constexpr int VEC = Vec16<T>::N, RPI = 32 / LPR, CPE = LPR / 4, G = 4, U = 4, RS = LPR * 16;
+  constexpr int VEC = Vec16<T>::N, RPI = 32 / LPR, CPE = LPR / 4, U = 4, RS = LPR * 16;
   extern __shared__ __align__(128) unsigned char rows_all[];       // [kLaneWarps][32 rows][RS bytes]
   __shared__ LaneSmem sm_all[kLaneWarps];
-  __shared__ float gate_s[kLaneWarps][8];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   LaneSmem& sm = sm_all[warp];
   unsigned char* rows_s = rows_all + (size_t)warp * 32 * RS;
-  const uint32_t rows_u = lane_smem_u32(rows_s), bar_u = lane_smem_u32(&sm.bar);
+  const uint32_t rows_u = smem_u32(rows_s), bar_u = smem_u32(&sm.bar);
   uint32_t uses = 0;                                              // completed uses of the barrier (parity)
   if (lane == 0) {
-    lane_mbar_init(bar_u, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    mbar_init(bar_u, 1);
+    mbar_init_fence();
   }
   __syncwarp();
   const int sg = lane / LPR, lir = lane % LPR, gk = lir / CPE;
@@ -106,14 +78,14 @@ va_lane_bwd_kernel(const VAParams P, const int PR) {
 
   // every view lane copies its own row into the warp's buffer; wait_rows() before the rows are read
   auto issue_rows = [&](int nv, uint32_t rid) {
-    lane_fence_proxy_async();                                     // earlier generic reads of the buffer come first
+    fence_proxy_async();                                     // earlier generic reads of the buffer come first
     __syncwarp();
-    if (lane == 0) lane_mbar_expect_tx(bar_u, (uint32_t)nv * row_bytes);
+    if (lane == 0) mbar_expect_tx(bar_u, (uint32_t)nv * row_bytes);
     __syncwarp();
-    if (lane < nv) lane_bulk_g2s(rows_u + (uint32_t)lane * RS, xbase + (uint64_t)rid * row_bytes, row_bytes, bar_u);
+    if (lane < nv) bulk_g2s(rows_u + (uint32_t)lane * RS, xbase + (uint64_t)rid * row_bytes, row_bytes, bar_u);
   };
   auto wait_rows = [&]() {
-    lane_mbar_wait(bar_u, uses & 1u);
+    mbar_wait(bar_u, uses & 1u);
     ++uses;
   };
 
@@ -184,8 +156,8 @@ va_lane_bwd_kernel(const VAParams P, const int PR) {
         const float inv_sq = P.group_scaling ? rsqrtf((float)n) : 1.f;
         float4 z4 = make_float4(1.f, 1.f, 1.f, 1.f), t4 = z4;
         if (gating) {
-          z4 = make_float4(fmaf(gw4.x, smx.x, gb4.x), fmaf(gw4.y, smx.y, gb4.y), fmaf(gw4.z, smx.z, gb4.z), fmaf(gw4.w, smx.w, gb4.w));
-          t4 = make_float4(tanhf(fmaxf(z4.x, 0.f)), tanhf(fmaxf(z4.y, 0.f)), tanhf(fmaxf(z4.z, 0.f)), tanhf(fmaxf(z4.w, 0.f)));
+          z4 = gate_z4(gw4, smx, gb4);
+          t4 = gate_t4(z4);
         }
         float4 Sacc = make_float4(0.f, 0.f, 0.f, 0.f);
         for (int c0 = 0; c0 < n; c0 += 32) {
@@ -193,7 +165,7 @@ va_lane_bwd_kernel(const VAParams P, const int PR) {
           const int64_t v = gvb + c0 + lane;
           float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
           __syncwarp();
-          const uint32_t rid_l = lane < nv ? lane_row_id(P.idx, P.idx64, v) : 0u;
+          const uint32_t rid_l = lane < nv ? load_row_id(P.idx, P.idx64, v) : 0u;
           issue_rows(nv, rid_l);
           if (lane < nv) {
             const float4 c = __ldg(reinterpret_cast<const float4*>(P.compat) + v);
@@ -222,23 +194,13 @@ va_lane_bwd_kernel(const VAParams P, const int PR) {
           Sacc.z += __shfl_xor_sync(kFull, Sacc.z, o); Sacc.w += __shfl_xor_sync(kFull, Sacc.w, o);
         }
         float4 dq = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (gating) {
-#define DVA_LGATE(c)                                                                       \
-          if (z4.c > 0.f) {                                                                \
-            const float dLdt = (t4.c != 0.f) ? Sacc.c / t4.c : 0.f;                         \
-            const float uu = dLdt * (1.f - t4.c * t4.c);                                   \
-            dq.c = uu * gw4.c;                                                             \
-            if (lane == 0) { dw4.c += uu * smx.c; db4.c += uu; }                           \
-          }
-          DVA_LGATE(x) DVA_LGATE(y) DVA_LGATE(z) DVA_LGATE(w)
-#undef DVA_LGATE
-        }
+        if (gating) dq = gate_grad4(Sacc, z4, t4, gw4, smx, lane == 0, dw4, db4);   // every lane holds the point's terms
         __syncwarp();
         for (int c0 = lane; c0 < n; c0 += 32) {
           const int64_t v = gvb + c0;
           const float4 c = __ldg(reinterpret_cast<const float4*>(P.compat) + v);
           const float4 sp = __ldcg(reinterpret_cast<const float4*>(P.gcompat) + v);
-          float4 d;
+          float4 d;   // compat_grad4() spelled out: through the helper the fp16 LPR 8 / 16 instantiations spill more
           d.x = __expf((c.x - smx.x) * inv_sq) / sdn.x * (sp.x - Sacc.x) * inv_sq;
           d.y = __expf((c.y - smx.y) * inv_sq) / sdn.y * (sp.y - Sacc.y) * inv_sq;
           d.z = __expf((c.z - smx.z) * inv_sq) / sdn.z * (sp.z - Sacc.z) * inv_sq;
@@ -266,7 +228,7 @@ va_lane_bwd_kernel(const VAParams P, const int PR) {
       int4 sar = make_int4(-1, -1, -1, -1);
       const int64_t v = gvb + lane;
       __syncwarp();                                                 // previous group's tiles are free
-      const uint32_t rid_m = lane < nv ? lane_row_id(P.idx, P.idx64, v) : 0u;
+      const uint32_t rid_m = lane < nv ? load_row_id(P.idx, P.idx64, v) : 0u;
       if (nv > 0) issue_rows(nv, rid_m);                            // rows go in flight before anything else is loaded
       if (lane < nv) {
         const float4 c = __ldg(reinterpret_cast<const float4*>(P.compat) + v);
@@ -276,9 +238,7 @@ va_lane_bwd_kernel(const VAParams P, const int PR) {
         inv_sq = P.group_scaling ? rsqrtf((float)cntp) : 1.f;
         a = make_float4(__expf((c.x - smx.x) * inv_sq) / sdn.x, __expf((c.y - smx.y) * inv_sq) / sdn.y,
                         __expf((c.z - smx.z) * inv_sq) / sdn.z, __expf((c.w - smx.w) * inv_sq) / sdn.w);
-        if (gating)
-          t4 = make_float4(tanhf(fmaxf(fmaf(gw4.x, smx.x, gb4.x), 0.f)), tanhf(fmaxf(fmaf(gw4.y, smx.y, gb4.y), 0.f)),
-                           tanhf(fmaxf(fmaf(gw4.z, smx.z, gb4.z), 0.f)), tanhf(fmaxf(fmaf(gw4.w, smx.w, gb4.w), 0.f)));
+        if (gating) t4 = gate_t4(gate_z4(gw4, smx, gb4));
         sm.ri[lane] = rid_m;
         sm.orow[lane] = scatter ? rid_m : (uint32_t)v;
         sm.go[lane] = (uint32_t)mp;
@@ -308,18 +268,8 @@ va_lane_bwd_kernel(const VAParams P, const int PR) {
         }
         if (gating && cnt > 0) {
           const float4 smx = reinterpret_cast<const float4*>(P.s_max)[pk];
-#define DVA_LGATE(c)                                                                       \
-          {                                                                                \
-            const float z = fmaf(gw4.c, smx.c, gb4.c);                                     \
-            if (z > 0.f) {                                                                 \
-              const float t = tanhf(z);                                                    \
-              const float dLdt = (t != 0.f) ? S.c / t : 0.f;                               \
-              const float uu = dLdt * (1.f - t * t);                                       \
-              dq.c = uu * gw4.c; dw4.c += uu * smx.c; db4.c += uu;                         \
-            }                                                                              \
-          }
-          DVA_LGATE(x) DVA_LGATE(y) DVA_LGATE(z) DVA_LGATE(w)
-#undef DVA_LGATE
+          const float4 z4 = gate_z4(gw4, smx, gb4);
+          dq = gate_grad4(S, z4, gate_t4(z4), gw4, smx, true, dw4, db4);
         }
         *reinterpret_cast<float4*>(sm.Sp[lane]) = S;
         *reinterpret_cast<float4*>(sm.dq[lane]) = dq;
@@ -330,99 +280,29 @@ va_lane_bwd_kernel(const VAParams P, const int PR) {
         const float4 S = *reinterpret_cast<const float4*>(sm.Sp[mp]);
         const float4 dq = *reinterpret_cast<const float4*>(sm.dq[mp]);
         const float4 sv = *reinterpret_cast<const float4*>(sm.st[lane]);
-        float4 d;
-        d.x = a.x * (sv.x - S.x) * inv_sq; d.y = a.y * (sv.y - S.y) * inv_sq;
-        d.z = a.z * (sv.z - S.z) * inv_sq; d.w = a.w * (sv.w - S.w) * inv_sq;
-        if ((int)v == sar.x) d.x += dq.x;
-        if ((int)v == sar.y) d.y += dq.y;
-        if ((int)v == sar.z) d.z += dq.z;
-        if ((int)v == sar.w) d.w += dq.w;
-        reinterpret_cast<float4*>(P.gcompat)[v] = d;
+        reinterpret_cast<float4*>(P.gcompat)[v] = compat_grad4(a, sv, S, inv_sq, (int)v, sar, dq);
       }
       pg += kfit;
     }
   }
 
-  // ---- gate parameter gradients: lanes -> warp -> block partial (fixed order), block -> workspace
-  if (P.gate_partial != nullptr) {
-    float vv[8] = {dw4.x, dw4.y, dw4.z, dw4.w, db4.x, db4.y, db4.z, db4.w};
-#pragma unroll
-    for (int q = 0; q < 8; ++q) {
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) vv[q] += __shfl_xor_sync(kFull, vv[q], o);
-    }
-    if (lane == 0) {
-#pragma unroll
-      for (int q = 0; q < 8; ++q) gate_s[warp][q] = vv[q];
-    }
-    __syncthreads();
-    if ((int)threadIdx.x < 2 * G) {
-      float acc = 0.f;
-      for (int w = 0; w < kLaneWarps; ++w) acc += gate_s[w][threadIdx.x];
-      P.gate_partial[(int64_t)blockIdx.x * 2 * G + threadIdx.x] = acc;
-    }
-  }
-}
-
-template <typename T> static bool lane_bwd_ok(const VAParams& P) {
-  constexpr int V16 = Vec16<T>::N;
-  const int C = P.C;
-  if (P.G != 4 || C % V16 != 0 || C / V16 > 32 || C / V16 < 4) return false;
-  const int cv = C / V16;
-  if ((cv & (cv - 1)) != 0) return false;                       // a row is exactly LPR = 4, 8, 16 or 32 chunks
-  if (!aligned16(P.x) || !aligned16(P.gout) || !aligned16(P.gx) || !aligned16(P.compat) || !aligned16(P.gcompat)) return false;
-  if (!aligned16(P.s_max) || !aligned16(P.s_den) || !aligned16(P.s_arg)) return false;
-  if (P.V >= (1ll << 31) || P.R >= (1ll << 32)) return false;
-  return true;
-}
-
-bool va_lane_bwd_applicable(const VAParams& P, int dtype) {
-  switch (dtype) {
-    case DVA_F32: return lane_bwd_ok<float>(P);
-    case DVA_BF16: return lane_bwd_ok<__nv_bfloat16>(P);
-    case DVA_F16: return lane_bwd_ok<__half>(P);
-    default: return false;
-  }
-}
-
-template <typename T, int LPR>
-static int lane_bwd_launch(const VAParams& P, int* grid_out, cudaStream_t st) {
-  auto kern = va_lane_bwd_kernel<T, LPR>;
-  const size_t smem = (size_t)kLaneWarps * 32 * LPR * 16;          // row buffers: 32 rows per warp
-  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (e != cudaSuccess) return fail((int)e, "va_lane_bwd: cannot reserve shared memory");
-  int occ = 0;
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, kLaneWarps * 32, smem) != cudaSuccess || occ < 1) occ = 1;
-  if (occ > 8) occ = 8;                                          // gate partials: at most kNumSMs x 8 CTAs
-  int64_t grid = (int64_t)kNumSMs * occ;
-  const int64_t warps = grid * kLaneWarps;
-  int64_t pr = (P.N + warps * 4 - 1) / (warps * 4);              // ~4 ranges per warp: balances ragged counts
-  if (pr < 8) pr = 8;
-  const int64_t n_ranges = (P.N + pr - 1) / pr;
-  const int64_t need = (n_ranges + kLaneWarps - 1) / kLaneWarps;
-  if (grid > need) grid = need;
-  if (grid < 1) grid = 1;
-  kern<<<(unsigned)grid, kLaneWarps * 32, smem, st>>>(P, (int)pr);
-  *grid_out = (int)grid;
-  return check_launch("va_lane_bwd");
-}
-
-template <typename T>
-static int lane_bwd_typed(const VAParams& P, int* grid_out, cudaStream_t st) {
-  switch (P.C / Vec16<T>::N) {
-    case 4: return lane_bwd_launch<T, 4>(P, grid_out, st);
-    case 8: return lane_bwd_launch<T, 8>(P, grid_out, st);
-    case 16: return lane_bwd_launch<T, 16>(P, grid_out, st);
-    default: return lane_bwd_launch<T, 32>(P, grid_out, st);
-  }
+  if (P.gate_partial != nullptr) store_gate_partial<kLaneWarps>(P.gate_partial, dw4, db4);
 }
 
 int va_lane_bwd(const VAParams& P, int dtype, int* grid_out, cudaStream_t st) {
-  switch (dtype) {
-    case DVA_F32: return lane_bwd_typed<float>(P, grid_out, st);
-    case DVA_BF16: return lane_bwd_typed<__nv_bfloat16>(P, grid_out, st);
-    default: return lane_bwd_typed<__half>(P, grid_out, st);
-  }
+  return with_dtype(dtype, [&](auto tag) {
+    using T = decltype(tag);
+    return with_lpr(P.C / Vec16<T>::N, [&](auto lpr) {
+      constexpr int LPR = decltype(lpr)::value;
+      auto kern = va_lane_bwd_kernel<T, LPR>;
+      const size_t smem = (size_t)kLaneWarps * 32 * LPR * 16;    // row buffers: 32 rows per warp
+      int grid, pr;   // at most 8 CTAs per SM (gate partials); ~4 ranges per warp balance ragged counts
+      if (int rc = range_geometry(kern, smem, kLaneWarps, 8, 4, P.N, "va_lane_bwd", &grid, &pr)) return rc;
+      kern<<<grid, kLaneWarps * 32, smem, st>>>(P, pr);
+      *grid_out = grid;
+      return check_launch("va_lane_bwd");
+    });
+  });
 }
 
 }  // namespace dva

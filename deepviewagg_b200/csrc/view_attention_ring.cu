@@ -81,9 +81,6 @@ template <int LPR, bool BWD> struct RingGeom {
   static_assert(RB >= RPI && RB % RPI == 0 && (RB & (RB - 1)) == 0, "batch geometry");
 };
 
-__device__ __forceinline__ uint32_t smem_u32(const void* p) {
-  return (uint32_t)__cvta_generic_to_shared(p);
-}
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
 }
@@ -91,46 +88,14 @@ __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commi
 template <int N> __device__ __forceinline__ void cp_async_wait() {
   asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
 }
-// ---- mbarrier + bulk async copy (backward: contiguous grad_out rows of a window of points)
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  uint32_t ok = 0;
-  while (!ok) {
-    asm volatile(
-        "{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2; selp.u32 %0, 1, 0, p; }"
-        : "=r"(ok) : "r"(bar), "r"(parity) : "memory");
-  }
-}
-__device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-               ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
-}
-__device__ __forceinline__ void fence_proxy_async() {
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-}
 __device__ __forceinline__ void prefetch_l2(const void* p) {
   asm volatile("prefetch.global.L2 [%0];" ::"l"(p));
-}
-
-__device__ __forceinline__ uint32_t load_row_id(const void* idx, int idx64, int64_t v) {
-  if (idx == nullptr) return (uint32_t)v;
-  return idx64 ? (uint32_t) reinterpret_cast<const int64_t*>(idx)[v]
-               : (uint32_t) reinterpret_cast<const int32_t*>(idx)[v];
 }
 
 // weight / attention tiles hold one float4 (4 groups) per view, 8 views per 36-float row: lanes
 // that walk their own points at a stride of 8k views still hit distinct banks
 __device__ __forceinline__ int tix(int u) { return (u + (u >> 3)) << 2; }
 constexpr int tile_floats(int capv) { return (capv / 8) * 36; }
-
-__device__ __forceinline__ float sel4(const float4& v, int g) {
-  return g == 0 ? v.x : (g == 1 ? v.y : (g == 2 ? v.z : v.w));
-}
 
 // per-warp shared memory (bytes)
 template <int LPR, bool BWD> struct RingSmem {
@@ -323,7 +288,7 @@ va_ring_fwd_kernel(const VAParams P, const int PR) {
         }
         den = group_lane_sum(den, G) + P.eps;
         const float gwl = sel4(gw4, gl), gbl = sel4(gb4, gl);
-        const float t = gating ? tanhf(fmaxf(fmaf(gwl, m_run, gbl), 0.f)) : 1.f;
+        const float t = gating ? gate_t(fmaf(gwl, m_run, gbl)) : 1.f;
         if (lane < G && save) {
           P.seg_max[i * G + lane] = m_run; P.seg_den[i * G + lane] = den; P.seg_arg[i * G + lane] = am;
         }
@@ -398,10 +363,8 @@ va_ring_fwd_kernel(const VAParams P, const int PR) {
               }
             }
             if (gating) {
-              sc.x *= tanhf(fmaxf(fmaf(gw4.x, mx.x, gb4.x), 0.f));
-              sc.y *= tanhf(fmaxf(fmaf(gw4.y, mx.y, gb4.y), 0.f));
-              sc.z *= tanhf(fmaxf(fmaf(gw4.z, mx.z, gb4.z), 0.f));
-              sc.w *= tanhf(fmaxf(fmaf(gw4.w, mx.w, gb4.w), 0.f));
+              const float4 t = gate_t4(gate_z4(gw4, mx, gb4));
+              sc.x *= t.x; sc.y *= t.y; sc.z *= t.z; sc.w *= t.w;
             }
           }
           if (save) {
@@ -449,7 +412,6 @@ va_ring_bwd_kernel(const VAParams P, const int PR) {
   constexpr int VEC = Vec16<T>::N, RPI = Gm::RPI, RB = Gm::RB, RS = Gm::RS, S = kRingStages;
   constexpr int G = kRG, CAPV = DVA_RING_CAPV_BWD, PW = Gm::PW;
   extern __shared__ __align__(128) unsigned char smem_raw[];
-  __shared__ float gate_s[kRingWarps][2 * kRG];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int C = P.C;
   const RingSmem<LPR, true> L;
@@ -469,7 +431,7 @@ va_ring_bwd_kernel(const VAParams P, const int PR) {
   if (lane == 0) {
     mbar_init(bar_u[0], 1);
     mbar_init(bar_u[1], 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    mbar_init_fence();
   }
   fence_proxy_async();
   __syncwarp();
@@ -637,7 +599,7 @@ va_ring_bwd_kernel(const VAParams P, const int PR) {
         const float inv_sq = P.group_scaling ? rsqrtf((float)n) : 1.f;
         const float gwl = sel4(gw4, gl), gbl = sel4(gb4, gl);
         const float z = fmaf(gwl, m, gbl);
-        const float t = gating ? tanhf(fmaxf(z, 0.f)) : 1.f;
+        const float t = gating ? gate_t(z) : 1.f;
         float gd[VEC];
         {
           const uint4 raw = *reinterpret_cast<const uint4*>(gtile);
@@ -670,24 +632,17 @@ va_ring_bwd_kernel(const VAParams P, const int PR) {
           v += np;
         }
         Ssum = group_lane_sum(Ssum, G);
-        const float one_m_t2 = 1.f - t * t;
-        const float dLdt = (t != 0.f) ? Ssum / t : 0.f;
-        const bool open = gating && z > 0.f;
-        const float dq = open ? dLdt * one_m_t2 * gwl : 0.f;
-        if (open && lane < G) {
-          const float dwv = dLdt * one_m_t2 * m, dbv = dLdt * one_m_t2;
-          if (lane == 0) { dw4.x += dwv; db4.x += dbv; }
-          if (lane == 1) { dw4.y += dwv; db4.y += dbv; }
-          if (lane == 2) { dw4.z += dwv; db4.z += dbv; }
-          if (lane == 3) { dw4.w += dwv; db4.w += dbv; }
-        }
+        float dwv = 0.f, dbv = 0.f;                 // every lane holds group gl's terms; lane gl keeps them
+        const float dq = gating ? gate_grad(Ssum, z, t, gwl, m, true, dwv, dbv) : 0.f;
+        if (lane == 0) { dw4.x += dwv; db4.x += dbv; }
+        if (lane == 1) { dw4.y += dwv; db4.y += dbv; }
+        if (lane == 2) { dw4.z += dwv; db4.z += dbv; }
+        if (lane == 3) { dw4.w += dwv; db4.w += dbv; }
         __syncwarp();                               // raw s' written by other lanes of this warp
         const int first_view = (int)(vb + s);
         for (int e = lane; e < n * G; e += 32) {
           const float a = __expf((__ldg(cp + e) - m) * inv_sq) * inv_den;
-          float d = a * (__ldcg(gc + e) - Ssum) * inv_sq;
-          if (first_view + e / G == arg_v) d += dq;
-          gc[e] = d;
+          gc[e] = compat_grad(a, __ldcg(gc + e), Ssum, inv_sq, first_view + e / G == arg_v, dq);
         }
         __syncwarp();
         pg += 1; pl = pl_n; cnt = cnt_n; smx = smx_n; sdn = sdn_n; sar = sar_n;
@@ -717,10 +672,8 @@ va_ring_bwd_kernel(const VAParams P, const int PR) {
           }
         }
         if (gating) {
-          z4 = make_float4(fmaf(gw4.x, smx.x, gb4.x), fmaf(gw4.y, smx.y, gb4.y),
-                           fmaf(gw4.z, smx.z, gb4.z), fmaf(gw4.w, smx.w, gb4.w));
-          t4 = make_float4(tanhf(fmaxf(z4.x, 0.f)), tanhf(fmaxf(z4.y, 0.f)),
-                           tanhf(fmaxf(z4.z, 0.f)), tanhf(fmaxf(z4.w, 0.f)));
+          z4 = gate_z4(gw4, smx, gb4);
+          t4 = gate_t4(z4);
         }
       }
       reinterpret_cast<float4*>(tpt)[lane] = t4;
@@ -760,30 +713,13 @@ va_ring_bwd_kernel(const VAParams P, const int PR) {
           Ss.x = fmaf(a.x, sv.x, Ss.x); Ss.y = fmaf(a.y, sv.y, Ss.y);
           Ss.z = fmaf(a.z, sv.z, Ss.z); Ss.w = fmaf(a.w, sv.w, Ss.w);
         }
-        float4 dq = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (gating) {
-#define DVA_GATE_TERM(c)                                                                  \
-          if (z4.c > 0.f) {                                                               \
-            const float dLdt = (t4.c != 0.f) ? Ss.c / t4.c : 0.f;                         \
-            const float u = dLdt * (1.f - t4.c * t4.c);                                   \
-            dq.c = u * gw4.c; dw4.c += u * smx.c; db4.c += u;                             \
-          }
-          DVA_GATE_TERM(x) DVA_GATE_TERM(y) DVA_GATE_TERM(z) DVA_GATE_TERM(w)
-#undef DVA_GATE_TERM
-        }
+        const float4 dq = gating ? gate_grad4(Ss, z4, t4, gw4, smx, true, dw4, db4) : make_float4(0.f, 0.f, 0.f, 0.f);
         float4* __restrict__ gc = reinterpret_cast<float4*>(P.gcompat + (vb + pl) * G);
         const int fv0 = (int)(vb + pl);
         for (int j = 0; j < cnt; ++j) {
           const float4 a = *reinterpret_cast<const float4*>(at + tix(u0 + j));
           const float4 sv = *reinterpret_cast<const float4*>(st + tix(u0 + j));
-          float4 d;
-          d.x = a.x * (sv.x - Ss.x) * inv_sq_l; d.y = a.y * (sv.y - Ss.y) * inv_sq_l;
-          d.z = a.z * (sv.z - Ss.z) * inv_sq_l; d.w = a.w * (sv.w - Ss.w) * inv_sq_l;
-          if (fv0 + j == sar.x) d.x += dq.x;
-          if (fv0 + j == sar.y) d.y += dq.y;
-          if (fv0 + j == sar.z) d.z += dq.z;
-          if (fv0 + j == sar.w) d.w += dq.w;
-          gc[j] = d;
+          gc[j] = compat_grad4(a, sv, Ss, inv_sq_l, fv0 + j, sar, dq);
         }
       }
       __syncwarp();                                 // tiles are rewritten by the next group
@@ -793,160 +729,40 @@ va_ring_bwd_kernel(const VAParams P, const int PR) {
     __syncwarp();
   }
 
-  // ---- gate parameter gradients: lanes -> warp -> block partial (fixed order), block -> workspace
-  if (P.gate_partial != nullptr) {
-    float v[8] = {dw4.x, dw4.y, dw4.z, dw4.w, db4.x, db4.y, db4.z, db4.w};
-#pragma unroll
-    for (int q = 0; q < 8; ++q) {
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) v[q] += __shfl_xor_sync(FULL, v[q], o);
-    }
-    if (lane == 0) {
-#pragma unroll
-      for (int q = 0; q < 8; ++q) gate_s[warp][q] = v[q];
-    }
-    __syncthreads();
-    if ((int)threadIdx.x < 2 * G) {
-      float acc = 0.f;
-      for (int w = 0; w < kRingWarps; ++w) acc += gate_s[w][threadIdx.x];
-      P.gate_partial[(int64_t)blockIdx.x * 2 * G + threadIdx.x] = acc;
-    }
-  }
+  if (P.gate_partial != nullptr) store_gate_partial<kRingWarps>(P.gate_partial, dw4, db4);
 }
 
 // ---------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------
-template <typename T> static int ring_lpr(const VAParams& P) {
-  const int cv = P.C / Vec16<T>::N;                 // 16-byte chunks per row
-  if (cv <= 4) return 4;
-  if (cv <= 8) return 8;
-  if (cv <= 16) return 16;
-  return 32;
-}
-
-template <typename T>
-static bool ring_common_ok(const VAParams& P, const void* o1, const void* o2) {
-  constexpr int V16 = Vec16<T>::N;
-  const int C = P.C, G = P.G;
-  if (G != kRG) return false;
-  if (C % V16 != 0 || C / V16 > 32) return false;   // rows of at most 512 bytes, whole 16-byte chunks
-  if (!aligned16(P.x) || !aligned16(o1) || (o2 != nullptr && !aligned16(o2))) return false;
-  if (!aligned16(P.compat)) return false;
-  if (P.V >= (1ll << 31) || P.R >= (1ll << 32)) return false;
-  for (int c0 = 0; c0 < C; c0 += V16)               // chunks never straddle channel groups
-    if (group_of_channel(c0, C, G) != group_of_channel(c0 + V16 - 1, C, G)) return false;
-  return true;
-}
-
-template <typename T> static bool ring_fwd_ok(const VAParams& P) {
-  if (!ring_common_ok<T>(P, P.out, nullptr)) return false;
-  if (P.att != nullptr && !aligned16(P.att)) return false;
-  if (P.seg_max != nullptr && (!aligned16(P.seg_max) || !aligned16(P.seg_den) || !aligned16(P.seg_arg))) return false;
-  return true;
-}
-template <typename T> static bool ring_bwd_ok(const VAParams& P) {
-  constexpr int V16 = Vec16<T>::N;
-  if (!ring_common_ok<T>(P, P.gout, P.gx)) return false;
-  if (P.C % P.G != 0 || (P.C / P.G) % V16 != 0) return false;
-  const int cpg = (P.C / P.G) / V16;
-  if ((cpg & (cpg - 1)) != 0) return false;         // regular layout: a row is 4 * cpg = LPR chunks
-  if (!aligned16(P.s_max) || !aligned16(P.s_den) || !aligned16(P.s_arg) || !aligned16(P.gcompat)) return false;
-  return true;
-}
-
-bool va_ring_fwd_applicable(const VAParams& P, int dtype) {
-  switch (dtype) {
-    case DVA_F32: return ring_fwd_ok<float>(P);
-    case DVA_BF16: return ring_fwd_ok<__nv_bfloat16>(P);
-    case DVA_F16: return ring_fwd_ok<__half>(P);
-    default: return false;
-  }
-}
-bool va_ring_bwd_applicable(const VAParams& P, int dtype) {
-  switch (dtype) {
-    case DVA_F32: return ring_bwd_ok<float>(P);
-    case DVA_BF16: return ring_bwd_ok<__nv_bfloat16>(P);
-    case DVA_F16: return ring_bwd_ok<__half>(P);
-    default: return false;
-  }
-}
-
-// grid = co-resident CTAs (kNumSMs x occupancy); PR = points per range (one range per warp when
-// the problem is large enough, never fewer than 8 points)
-template <typename K>
-static int ring_launch_geometry(K kern, size_t smem, int64_t N, int max_ctas_per_sm, int* grid_out, int* pr_out) {
-  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (e != cudaSuccess) return failf((int)e, "view_attention ring: %zu bytes of shared memory: %s", smem, cudaGetErrorString(e));
-  int occ = 0;
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, kRingWarps * 32, smem) != cudaSuccess || occ < 1) occ = 1;
-  if (occ > max_ctas_per_sm) occ = max_ctas_per_sm;
-  int64_t grid = (int64_t)kNumSMs * occ;
-  const int64_t warps = grid * kRingWarps;
-  int64_t pr = (N + warps - 1) / warps;
-  if (pr < 8) pr = 8;
-  const int64_t n_ranges = (N + pr - 1) / pr;
-  const int64_t need = (n_ranges + kRingWarps - 1) / kRingWarps;
-  if (grid > need) grid = need;
-  if (grid < 1) grid = 1;
-  *grid_out = (int)grid; *pr_out = (int)pr;
-  return DVA_OK;
-}
-
-template <typename T, int LPR>
-static int ring_fwd_launch(const VAParams& P, cudaStream_t st) {
-  const RingSmem<LPR, false> L;
-  const size_t smem = L.total * kRingWarps;
-  auto kern = va_ring_fwd_kernel<T, LPR>;
-  int grid, pr;
-  if (int rc = ring_launch_geometry(kern, smem, P.N, 32, &grid, &pr)) return rc;
-  kern<<<grid, kRingWarps * 32, smem, st>>>(P, pr);
-  return check_launch("view_attention_fwd(ring)");
-}
-template <typename T, int LPR>
-static int ring_bwd_launch(const VAParams& P, int* grid_out, cudaStream_t st) {
-  const RingSmem<LPR, true> L;
-  const size_t smem = L.total * kRingWarps;
-  auto kern = va_ring_bwd_kernel<T, LPR>;
-  int grid, pr;
-  if (int rc = ring_launch_geometry(kern, smem, P.N, 8, &grid, &pr)) return rc;   // gate-gradient workspace: kNumSMs x 8 partials
-  *grid_out = grid;
-  kern<<<grid, kRingWarps * 32, smem, st>>>(P, pr);
-  return check_launch("view_attention_bwd(ring)");
-}
-
-template <typename T> static int ring_fwd_typed(const VAParams& P, cudaStream_t st) {
-  switch (ring_lpr<T>(P)) {
-    case 4: return ring_fwd_launch<T, 4>(P, st);
-    case 8: return ring_fwd_launch<T, 8>(P, st);
-    case 16: return ring_fwd_launch<T, 16>(P, st);
-    default: return ring_fwd_launch<T, 32>(P, st);
-  }
-}
-template <typename T> static int ring_bwd_typed(const VAParams& P, int* grid, cudaStream_t st) {
-  switch (ring_lpr<T>(P)) {
-    case 4: return ring_bwd_launch<T, 4>(P, grid, st);
-    case 8: return ring_bwd_launch<T, 8>(P, grid, st);
-    case 16: return ring_bwd_launch<T, 16>(P, grid, st);
-    default: return ring_bwd_launch<T, 32>(P, grid, st);
-  }
-}
-
 int va_ring_fwd(const VAParams& P, int dtype, cudaStream_t st) {
-  switch (dtype) {
-    case DVA_F32: return ring_fwd_typed<float>(P, st);
-    case DVA_BF16: return ring_fwd_typed<__nv_bfloat16>(P, st);
-    case DVA_F16: return ring_fwd_typed<__half>(P, st);
-    default: return fail(DVA_EINVAL, "view_attention_fwd: unknown dtype");
-  }
+  return with_dtype(dtype, [&](auto tag) {
+    using T = decltype(tag);
+    return with_lpr(P.C / Vec16<T>::N, [&](auto lpr) {
+      constexpr int LPR = decltype(lpr)::value;
+      const size_t smem = RingSmem<LPR, false>().total * kRingWarps;
+      auto kern = va_ring_fwd_kernel<T, LPR>;
+      int grid, pr;
+      if (int rc = range_geometry(kern, smem, kRingWarps, 32, 1, P.N, "view_attention_fwd(ring)", &grid, &pr)) return rc;
+      kern<<<grid, kRingWarps * 32, smem, st>>>(P, pr);
+      return check_launch("view_attention_fwd(ring)");
+    });
+  });
 }
 int va_ring_bwd(const VAParams& P, int dtype, int* grid_out, cudaStream_t st) {
-  switch (dtype) {
-    case DVA_F32: return ring_bwd_typed<float>(P, grid_out, st);
-    case DVA_BF16: return ring_bwd_typed<__nv_bfloat16>(P, grid_out, st);
-    case DVA_F16: return ring_bwd_typed<__half>(P, grid_out, st);
-    default: return fail(DVA_EINVAL, "view_attention_bwd: unknown dtype");
-  }
+  return with_dtype(dtype, [&](auto tag) {
+    using T = decltype(tag);
+    return with_lpr(P.C / Vec16<T>::N, [&](auto lpr) {
+      constexpr int LPR = decltype(lpr)::value;
+      const size_t smem = RingSmem<LPR, true>().total * kRingWarps;
+      auto kern = va_ring_bwd_kernel<T, LPR>;
+      int grid, pr;   // at most 8 CTAs per SM: the gate-gradient workspace holds kNumSMs x 8 partials
+      if (int rc = range_geometry(kern, smem, kRingWarps, 8, 1, P.N, "view_attention_bwd(ring)", &grid, &pr)) return rc;
+      *grid_out = grid;
+      kern<<<grid, kRingWarps * 32, smem, st>>>(P, pr);
+      return check_launch("view_attention_bwd(ring)");
+    });
+  });
 }
 
 }  // namespace dva
