@@ -252,29 +252,14 @@ bn_bwd_apply_kernel(const T* __restrict__ dy, const T* __restrict__ z, const flo
   }
 }
 
-static int bn_grid_reduce(int64_t R) {
-  int64_t g = (R + 63) / 64;                         // >= 64 rows per CTA
-  const int64_t cap = (int64_t)kNumSMs * 4;
-  return (int)(g > cap ? cap : (g < 1 ? 1 : g));
-}
-static int bn_grid_stream(int64_t R, int C, int vec) {   // CTAs of RG rows, 8 resident CTAs per SM
+// the reductions: at least 64 rows per CTA, 4 CTAs per SM
+static int bn_grid_reduce(int64_t R) { return grid_cap(R, 64, 4); }
+// rows per CTA of the streaming kernels (RG row groups of TC column threads)
+static int bn_row_groups(int C, int vec) {
   const int CV = C / vec;
-  const int TC = CV < kBnThreads ? CV : kBnThreads;
-  const int RG = kBnThreads / TC;
-  int64_t g = (R + RG - 1) / RG;
-  const int64_t cap = (int64_t)kNumSMs * 8;
-  return (int)(g > cap ? cap : (g < 1 ? 1 : g));
+  return kBnThreads / (CV < kBnThreads ? CV : kBnThreads);
 }
-static size_t bn_smem(int C, int vec) {
-  const int CV = C / vec;
-  const int TC = CV < kBnThreads ? CV : kBnThreads;
-  return (size_t)(kBnThreads / TC) * 2 * C * sizeof(float);
-}
-
-template <typename T> static int pick_vec(int64_t C, const void* a, const void* b) {
-  constexpr int V = Vec16<T>::N;
-  return (C % V == 0 && aligned16(a) && (b == nullptr || aligned16(b))) ? V : 1;
-}
+static size_t bn_smem(int C, int vec) { return (size_t)bn_row_groups(C, vec) * 2 * C * sizeof(float); }
 
 }  // namespace dva
 
@@ -284,13 +269,47 @@ extern "C" size_t dva_bn_workspace_bytes(int64_t R, int64_t C) {
   return (size_t)bn_grid_reduce(R) * 2 * (size_t)(C > 0 ? C : 1) * sizeof(float);
 }
 
-#define BN_TYPED(dtype, ...)                                                  \
-  switch (dtype) {                                                            \
-    case DVA_F32: { using T = float; __VA_ARGS__ } break;                     \
-    case DVA_BF16: { using T = __nv_bfloat16; __VA_ARGS__ } break;            \
-    case DVA_F16: { using T = __half; __VA_ARGS__ } break;                    \
-    default: return fail(DVA_EINVAL, "bn: unknown dtype");                    \
+// statistics pass (reduce) and row pass (stream) of one dtype and vector width
+template <typename T, int VEC>
+static int bn_fwd_launch(const void* z, const float* gamma, const float* beta, float* running_mean, float* running_var,
+                         float* mean, float* invstd, void* y, int64_t R, int C, float eps, float momentum, float slope,
+                         int training, void* workspace, cudaStream_t st) {
+  int rc;
+  if (training) {
+    const int grid = bn_grid_reduce(R);
+    const size_t smem = bn_smem(C, VEC);
+    (void)smem_opt_in(bn_stats_kernel<T, VEC>, smem);
+    bn_stats_kernel<T, VEC><<<grid, kBnThreads, smem, st>>>((const T*)z, (float*)workspace, R, C);
+    if ((rc = check_launch("bn_stats"))) return rc;
+    bn_finalize_kernel<T><<<(C + 7) / 8, 256, 0, st>>>((const T*)z, (const float*)workspace, grid, R, C, eps, momentum,
+                                                       mean, invstd, running_mean, running_var);
+    if ((rc = check_launch("bn_finalize"))) return rc;
   }
+  // eval: fixed statistics, mean = running_mean, invstd = rsqrt(running_var + eps) computed by the host mirror
+  bn_apply_kernel<T, VEC><<<grid_cap(R, bn_row_groups(C, VEC), 8), kBnThreads, 0, st>>>(
+      (const T*)z, mean, invstd, gamma, beta, (T*)y, R, C, slope);
+  return check_launch("bn_apply");
+}
+
+template <typename T, int VEC>
+static int bn_bwd_launch(const void* dy, const void* z, const float* gamma, const float* beta, const float* mean,
+                         const float* invstd, void* dz, float* dgamma_dbeta, int64_t R, int C, float slope, int training,
+                         void* workspace, cudaStream_t st) {
+  const int grid = bn_grid_reduce(R);
+  const size_t smem = bn_smem(C, VEC);
+  (void)smem_opt_in(bn_bwd_reduce_kernel<T, VEC>, smem);
+  bn_bwd_reduce_kernel<T, VEC><<<grid, kBnThreads, smem, st>>>((const T*)dy, (const T*)z, mean, invstd, gamma, beta,
+                                                             (float*)workspace, R, C, slope);
+  int rc;
+  if ((rc = check_launch("bn_bwd_reduce"))) return rc;
+  // dgamma_dbeta = [sum g ; sum g*zhat]  (note the order: [0] = d beta, [1] = d gamma)
+  bn_bwd_finalize_kernel<<<(2 * C + 7) / 8, 256, 0, st>>>((const float*)workspace, grid, C, dgamma_dbeta);
+  if ((rc = check_launch("bn_bwd_finalize"))) return rc;
+  if (!dz) return DVA_OK;
+  bn_bwd_apply_kernel<T, VEC><<<grid_cap(R, bn_row_groups(C, VEC), 8), kBnThreads, 0, st>>>(
+      (const T*)dy, (const T*)z, mean, invstd, gamma, beta, dgamma_dbeta, (T*)dz, R, C, slope, training);
+  return check_launch("bn_bwd_apply");
+}
 
 extern "C" int dva_bn_act_fwd(const void* z, const float* gamma, const float* beta, float* running_mean,
                               float* running_var, float* mean, float* invstd, void* y, int64_t R, int64_t C,
@@ -302,38 +321,17 @@ extern "C" int dva_bn_act_fwd(const void* z, const float* gamma, const float* be
   if (training && (!workspace || workspace_bytes < dva_bn_workspace_bytes(R, C)))
     return fail(DVA_EINVAL, "bn_act_fwd: workspace too small");
   if (!training && (!running_mean || !running_var)) return fail(DVA_EINVAL, "bn_act_fwd: eval mode needs running statistics");
+  if (!known_dtype(dtype)) return fail(DVA_EINVAL, "bn_act_fwd: unknown dtype");
   cudaStream_t st = (cudaStream_t)stream;
-  BN_TYPED(dtype, {
-    const int vec = pick_vec<T>(C, z, y);
-    int rc;
-    if (training) {
-      const int grid = bn_grid_reduce(R);
-      const size_t smem = bn_smem((int)C, vec);
-      if (smem > 200 * 1024) return fail(DVA_EUNSUPPORTED, "bn_act_fwd: C too large for the reduction tile");
-      if (vec > 1) {
-        if (smem > 48 * 1024) cudaFuncSetAttribute(bn_stats_kernel<T, Vec16<T>::N>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        bn_stats_kernel<T, Vec16<T>::N><<<grid, kBnThreads, smem, st>>>((const T*)z, (float*)workspace, R, (int)C);
-      } else {
-        if (smem > 48 * 1024) cudaFuncSetAttribute(bn_stats_kernel<T, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        bn_stats_kernel<T, 1><<<grid, kBnThreads, smem, st>>>((const T*)z, (float*)workspace, R, (int)C);
-      }
-      if ((rc = check_launch("bn_stats"))) return rc;
-      bn_finalize_kernel<T><<<(int)((C + 7) / 8), 256, 0, st>>>((const T*)z, (const float*)workspace, grid, R,
-                                                                   (int)C, eps, momentum, mean, invstd,
-                                                                   running_mean, running_var);
-      if ((rc = check_launch("bn_finalize"))) return rc;
-    } else {
-      // fixed statistics: mean = running_mean, invstd = rsqrt(running_var + eps) computed by the host mirror
-    }
-    if (vec > 1)
-      bn_apply_kernel<T, Vec16<T>::N><<<bn_grid_stream(R, (int)C, Vec16<T>::N), kBnThreads, 0, st>>>(
-          (const T*)z, mean, invstd, gamma, beta, (T*)y, R, (int)C, slope);
-    else
-      bn_apply_kernel<T, 1><<<bn_grid_stream(R, (int)C, 1), kBnThreads, 0, st>>>((const T*)z, mean, invstd, gamma,
-                                                                              beta, (T*)y, R, (int)C, slope);
-    return check_launch("bn_apply");
+  return with_dtype(dtype, [&](auto t) {
+    using T = decltype(t);
+    const bool vec = vec16_ok<T>(C, z, y);
+    if (training && bn_smem((int)C, vec ? Vec16<T>::N : 1) > 200 * 1024)
+      return fail(DVA_EUNSUPPORTED, "bn_act_fwd: C too large for the reduction tile");
+    auto launch = vec ? bn_fwd_launch<T, Vec16<T>::N> : bn_fwd_launch<T, 1>;
+    return launch(z, gamma, beta, running_mean, running_var, mean, invstd, y, R, (int)C, eps, momentum, slope, training,
+                  workspace, st);
   });
-  return DVA_OK;
 }
 
 extern "C" int dva_bn_act_bwd(const void* dy, const void* z, const float* gamma, const float* beta,
@@ -349,34 +347,13 @@ extern "C" int dva_bn_act_bwd(const void* dy, const void* z, const float* gamma,
   // dz == nullptr: statistics pass only (the caller differentiates the rows itself: mlp_layer.cu)
   if (!dy || !z || !mean || !invstd || !dgamma_dbeta) return fail(DVA_EINVAL, "bn_act_bwd: null pointer");
   if (!workspace || workspace_bytes < dva_bn_workspace_bytes(R, C)) return fail(DVA_EINVAL, "bn_act_bwd: workspace too small");
-  BN_TYPED(dtype, {
-    const int v1 = pick_vec<T>(C, z, dy), v2 = pick_vec<T>(C, dz, nullptr);
-    const int vec = (v1 > 1 && v2 > 1) ? v1 : 1;
-    const int grid = bn_grid_reduce(R);
-    const size_t smem = bn_smem((int)C, vec);
-    if (smem > 200 * 1024) return fail(DVA_EUNSUPPORTED, "bn_act_bwd: C too large for the reduction tile");
-    int rc;
-    if (vec > 1) {
-      if (smem > 48 * 1024) cudaFuncSetAttribute(bn_bwd_reduce_kernel<T, Vec16<T>::N>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-      bn_bwd_reduce_kernel<T, Vec16<T>::N><<<grid, kBnThreads, smem, st>>>((const T*)dy, (const T*)z, mean, invstd,
-                                                                         gamma, beta, (float*)workspace, R, (int)C, slope);
-    } else {
-      if (smem > 48 * 1024) cudaFuncSetAttribute(bn_bwd_reduce_kernel<T, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-      bn_bwd_reduce_kernel<T, 1><<<grid, kBnThreads, smem, st>>>((const T*)dy, (const T*)z, mean, invstd, gamma, beta,
-                                                               (float*)workspace, R, (int)C, slope);
-    }
-    if ((rc = check_launch("bn_bwd_reduce"))) return rc;
-    // dgamma_dbeta = [sum g ; sum g*zhat]  (note the order: [0] = d beta, [1] = d gamma)
-    bn_bwd_finalize_kernel<<<(int)((2 * C + 7) / 8), 256, 0, st>>>((const float*)workspace, grid, (int)C, dgamma_dbeta);
-    if ((rc = check_launch("bn_bwd_finalize"))) return rc;
-    if (!dz) return DVA_OK;
-    if (vec > 1)
-      bn_bwd_apply_kernel<T, Vec16<T>::N><<<bn_grid_stream(R, (int)C, Vec16<T>::N), kBnThreads, 0, st>>>(
-          (const T*)dy, (const T*)z, mean, invstd, gamma, beta, dgamma_dbeta, (T*)dz, R, (int)C, slope, training);
-    else
-      bn_bwd_apply_kernel<T, 1><<<bn_grid_stream(R, (int)C, 1), kBnThreads, 0, st>>>(
-          (const T*)dy, (const T*)z, mean, invstd, gamma, beta, dgamma_dbeta, (T*)dz, R, (int)C, slope, training);
-    return check_launch("bn_bwd_apply");
+  if (!known_dtype(dtype)) return fail(DVA_EINVAL, "bn_act_bwd: unknown dtype");
+  return with_dtype(dtype, [&](auto t) {
+    using T = decltype(t);
+    const bool vec = vec16_ok<T>(C, z, dy, dz);
+    if (bn_smem((int)C, vec ? Vec16<T>::N : 1) > 200 * 1024)
+      return fail(DVA_EUNSUPPORTED, "bn_act_bwd: C too large for the reduction tile");
+    auto launch = vec ? bn_bwd_launch<T, Vec16<T>::N> : bn_bwd_launch<T, 1>;
+    return launch(dy, z, gamma, beta, mean, invstd, dz, dgamma_dbeta, R, (int)C, slope, training, workspace, st);
   });
-  return DVA_OK;
 }

@@ -16,12 +16,6 @@ namespace bk {
 
 constexpr int kScanItems = 2048;          // elements per scan block (256 threads x 8)
 
-static inline int grid_for(int64_t total, int per_block = 256) {
-  int64_t blocks = (total + per_block - 1) / per_block;
-  const int64_t cap = (int64_t)kNumSMs * 16;
-  return (int)(blocks > cap ? cap : (blocks < 1 ? 1 : blocks));
-}
-
 // ---- exclusive scan int32 -> int64 (three phases; sizes up to 2^31 blocks of 2048) -------------------
 static __global__ void __launch_bounds__(256)
 scan_block_sums(const int32_t* __restrict__ in, int64_t n, int64_t* __restrict__ block_sums) {
@@ -200,12 +194,10 @@ struct BucketIndex {
   int64_t *off, *block_sums, *bucket, *sorted;
 };
 
-static inline size_t align256(size_t v) { return (v + 255) & ~(size_t)255; }
-
 // carves the index out of base (nullptr: size query); returns the bytes used
 static size_t carve_index(uint8_t* base, int64_t n_entries, int64_t nb, BucketIndex* w) {
   size_t o = 0;
-  auto take = [&](size_t bytes) { uint8_t* p = base ? base + o : nullptr; o += align256(bytes); return p; };
+  auto take = [&](size_t bytes) { uint8_t* p = base ? base + o : nullptr; o += round256(bytes); return p; };
   uint8_t* p;
   p = take((size_t)(nb + 1) * 8); if (w) { w->cnt = (int32_t*)p; w->cursor = w->cnt ? w->cnt + (nb + 1) : nullptr; }
   p = take((size_t)(nb + 1) * 8); if (w) w->off = (int64_t*)p;
@@ -225,15 +217,15 @@ static int build_index(KeyOf key_of, int64_t n_items, int64_t nb, const BucketIn
   if (e != cudaSuccess) return fail((int)e, "bucket index: memset failed");
   int rc;
   if (n_items > 0) {
-    count_keys<NK><<<grid_for(n_items), 256, 0, st>>>(key_of, n_items, nb, w.cnt);
+    count_keys<NK><<<grid_cap(n_items, 256, 16), 256, 0, st>>>(key_of, n_items, nb, w.cnt);
     if ((rc = check_launch("bucket_count_keys"))) return rc;
   }
   if ((rc = exclusive_scan(w.cnt, nb, w.off, w.block_sums, st))) return rc;
   if (n_items > 0) {
-    scatter_keys<NK><<<grid_for(n_items), 256, 0, st>>>(key_of, n_items, nb, w.off, w.cursor, w.bucket);
+    scatter_keys<NK><<<grid_cap(n_items, 256, 16), 256, 0, st>>>(key_of, n_items, nb, w.off, w.cursor, w.bucket);
     if ((rc = check_launch("bucket_scatter_keys"))) return rc;
     if (!order) return DVA_OK;
-    order_by_id<<<grid_for(nb * 32), 256, 0, st>>>(w.off, w.bucket, w.sorted, nb);
+    order_by_id<<<grid_cap(nb * 32, 256, 16), 256, 0, st>>>(w.off, w.bucket, w.sorted, nb);
     if ((rc = check_launch("bucket_order_by_id"))) return rc;
   }
   return DVA_OK;

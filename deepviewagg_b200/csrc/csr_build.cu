@@ -32,12 +32,6 @@ csr_select_values_kernel(const int64_t* __restrict__ ptr, const int64_t* __restr
   }
 }
 
-static inline int c_grid(int64_t total) {
-  int64_t blocks = (total + 255) / 256;
-  const int64_t cap = (int64_t)kNumSMs * 16;
-  return (int)(blocks > cap ? cap : (blocks < 1 ? 1 : blocks));
-}
-
 }  // namespace dva
 
 using namespace dva;
@@ -46,7 +40,7 @@ extern "C" int dva_csr_pointers_from_sorted(const int64_t* ids, int64_t* ptr, in
                                             int64_t num_groups, void* stream) {
   if (n < 0 || num_groups < 0) return fail(DVA_EINVAL, "csr_pointers_from_sorted: negative size");
   if (!ptr || (n > 0 && !ids)) return fail(DVA_EINVAL, "csr_pointers_from_sorted: null pointer");
-  csr_pointers_kernel<<<c_grid(n + 1), 256, 0, (cudaStream_t)stream>>>(ids, ptr, n, num_groups);
+  csr_pointers_kernel<<<grid_cap(n + 1, 256, 16), 256, 0, (cudaStream_t)stream>>>(ids, ptr, n, num_groups);
   return check_launch("csr_pointers");
 }
 
@@ -56,6 +50,6 @@ extern "C" int dva_csr_select_values(const int64_t* ptr, const int64_t* sel,
   if (k < 0 || n_new_items < 0) return fail(DVA_EINVAL, "csr_select_values: negative size");
   if (k == 0 || n_new_items == 0) return DVA_OK;
   if (!ptr || !sel || !ptr_new || !val_idx) return fail(DVA_EINVAL, "csr_select_values: null pointer");
-  csr_select_values_kernel<<<c_grid(k * 8), 256, 0, (cudaStream_t)stream>>>(ptr, sel, ptr_new, val_idx, k);
+  csr_select_values_kernel<<<grid_cap(k * 8, 256, 16), 256, 0, (cudaStream_t)stream>>>(ptr, sel, ptr_new, val_idx, k);
   return check_launch("csr_select_values");
 }

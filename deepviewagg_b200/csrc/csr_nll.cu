@@ -20,11 +20,8 @@ namespace dva {
 constexpr int kNllThreads = 256;
 constexpr int kNllMaxK = 64;
 
-static inline int nll_blocks(int64_t N) {
-  const int64_t b = (N + kNllThreads - 1) / kNllThreads;
-  const int64_t cap = (int64_t)kNumSMs * 8;
-  return (int)(b > cap ? cap : (b < 1 ? 1 : b));
-}
+// one forward partial per CTA: the workspace query and the launches share the grid
+static inline int nll_blocks(int64_t N) { return grid_cap(N, kNllThreads, 8); }
 
 struct NllPartial {
   double loss;
@@ -135,14 +132,6 @@ csr_nll_bwd_kernel(const T* __restrict__ logits, const int64_t* __restrict__ lab
 
 using namespace dva;
 
-#define DVA_NLL_DISPATCH(dtype, ...)                                          \
-  switch (dtype) {                                                            \
-    case DVA_F32:  { using T = float; __VA_ARGS__; } break;                   \
-    case DVA_BF16: { using T = __nv_bfloat16; __VA_ARGS__; } break;           \
-    case DVA_F16:  { using T = __half; __VA_ARGS__; } break;                  \
-    default: return fail(DVA_EINVAL, "csr_nll: unknown dtype");               \
-  }
-
 extern "C" size_t dva_csr_nll_fwd_workspace_bytes(int64_t N) {
   return (size_t)nll_blocks(N) * sizeof(NllPartial);
 }
@@ -160,7 +149,9 @@ extern "C" int dva_csr_nll_fwd(const void* logits, int dtype, const int64_t* lab
   cudaStream_t st = (cudaStream_t)stream;
   NllPartial* part = (NllPartial*)workspace;
   if (nb > 0) {
-    DVA_NLL_DISPATCH(dtype, {
+    if (!known_dtype(dtype)) return fail(DVA_EINVAL, "csr_nll_fwd: unknown dtype");
+    with_dtype(dtype, [&](auto t) {
+      using T = decltype(t);
       csr_nll_fwd_kernel<T><<<nb, kNllThreads, 0, st>>>((const T*)logits, labels, csr_idx, V, N, K, ignore_index,
                                                          lse, part);
     });
@@ -179,7 +170,9 @@ extern "C" int dva_csr_nll_bwd(const void* logits, int dtype, const int64_t* lab
   if (csr_idx == nullptr && V != N) return fail(DVA_EINVAL, "csr_nll_bwd: without csr_idx, V must equal N");
   if (V == 0 || N == 0) return DVA_OK;
   if (!logits || !labels || !lse || !grad_loss || !stats || !grad_logits) return fail(DVA_EINVAL, "csr_nll_bwd: null pointer");
-  DVA_NLL_DISPATCH(dtype, {
+  if (!known_dtype(dtype)) return fail(DVA_EINVAL, "csr_nll_bwd: unknown dtype");
+  with_dtype(dtype, [&](auto t) {
+    using T = decltype(t);
     csr_nll_bwd_kernel<T><<<nll_blocks(N), kNllThreads, 0, (cudaStream_t)stream>>>(
         (const T*)logits, labels, csr_idx, V, N, K, ignore_index, lse, grad_loss, stats, (T*)grad_logits);
   });

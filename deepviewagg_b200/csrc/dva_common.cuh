@@ -7,6 +7,7 @@
 #include <stdio.h>
 #include <string.h>
 #include <atomic>
+#include <type_traits>
 #include "../../include/dva_b200.h"
 
 namespace dva {
@@ -39,6 +40,58 @@ inline int check_launch(const char* what) {
 
 inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
+// ---- host-side launch vocabulary: every launcher takes these decisions from here
+// f(T{}) with T the storage type of dtype; the C entry points have rejected every other dtype
+template <typename F> decltype(auto) with_dtype(int dtype, F&& f) {
+  switch (dtype) {
+    case DVA_F32: return f(float{});
+    case DVA_BF16: return f(__nv_bfloat16{});
+    default: return f(__half{});
+  }
+}
+inline bool known_dtype(int dtype) { return dtype == DVA_F32 || dtype == DVA_BF16 || dtype == DVA_F16; }
+
+// f(std::integral_constant<int, V>{}) for the V of Vs equal to v; false (f not called) when there is none
+template <int... Vs, typename F> bool with_value(int v, F&& f) {
+  return ((v == Vs && (f(std::integral_constant<int, Vs>{}), true)) || ...);
+}
+// f(std::integral_constant<int, RED>{}) with RED the reduce code; false for an unknown code
+template <typename F> bool with_reduce(int reduce, F&& f) {
+  return with_value<DVA_SUM, DVA_MEAN, DVA_MAX, DVA_MIN>(reduce, f);
+}
+// f(PIX{}) with PIX the type of the (x, y) pixel pairs of pix_code 0 = int16, 1 = int32, 2 = int64; false for any
+// other code
+template <typename F> bool with_pix(int pix_code, F&& f) {
+  return with_value<0, 1, 2>(pix_code, [&](auto c) {
+    constexpr int k = decltype(c)::value;
+    f(std::conditional_t<k == 0, int16_t, std::conditional_t<k == 1, int32_t, int64_t>>{});
+  });
+}
+// f(std::integral_constant<int, LPR>{}) with LPR the lanes per row of the sub-warp row kernels: the smallest of
+// 4, 8, 16, 32 that covers cv 16-byte chunks
+template <typename F> decltype(auto) with_lpr(int64_t cv, F&& f) {
+  if (cv <= 4) return f(std::integral_constant<int, 4>{});
+  if (cv <= 8) return f(std::integral_constant<int, 8>{});
+  if (cv <= 16) return f(std::integral_constant<int, 16>{});
+  return f(std::integral_constant<int, 32>{});
+}
+
+// Grid of a grid-stride launch: one CTA per per_block items, at least 1 and at most ctas_per_sm CTAs per SM
+inline int grid_cap(int64_t items, int64_t per_block, int ctas_per_sm) {
+  const int64_t blocks = (items + per_block - 1) / per_block, cap = (int64_t)kNumSMs * ctas_per_sm;
+  return (int)(blocks > cap ? cap : (blocks < 1 ? 1 : blocks));
+}
+
+// workspaces are carved in 256-byte aligned pieces from a 256-byte aligned base
+inline size_t round256(size_t bytes) { return (bytes + 255) & ~(size_t)255; }
+inline uint8_t* align256(void* p) { return reinterpret_cast<uint8_t*>(round256(reinterpret_cast<uintptr_t>(p))); }
+
+// the opt-in a kernel needs to launch with more than 48 KB of dynamic shared memory
+template <typename K> cudaError_t smem_opt_in(K* kern, size_t smem) {
+  if (smem <= 48 * 1024) return cudaSuccess;
+  return cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+}
+
 // ---- storage-type traits: load/store as fp32
 template <typename T> struct Cvt;
 template <> struct Cvt<float> {
@@ -57,6 +110,12 @@ template <> struct Cvt<__half> {
 // 16-byte vector of T: float x4, bf16/half x8
 template <typename T> struct Vec16 { static constexpr int N = 16 / sizeof(T); };
 
+// rows of n elements of T can move as 16-byte vectors: n is a multiple of Vec16<T>::N and every pointer is
+// 16-byte aligned (a null pointer, an absent operand, counts as aligned)
+template <typename T, typename... P> bool vec16_ok(int64_t n, const P*... p) {
+  return n % Vec16<T>::N == 0 && (aligned16(p) && ...);
+}
+
 template <typename T, int N>
 struct alignas(sizeof(T) * N) Pack { T v[N]; };
 
@@ -70,6 +129,10 @@ __device__ __forceinline__ uint4 ldg_stream16(const void* p) {
 __device__ __forceinline__ void stg_stream16(void* p, const uint4& v) {
   asm volatile("st.global.L1::no_allocate.v4.u32 [%0], {%1,%2,%3,%4};"
                :: "l"(p), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
+}
+// 16-byte vector reduction into global memory (sm_90+): one instruction per four channels
+__device__ __forceinline__ void red_add_v4(float* addr, float a, float b, float c, float d) {
+  asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
 }
 
 template <typename T, int VEC>

@@ -243,11 +243,6 @@ gather_pool_fwd_cl_kernel(const T* __restrict__ fmap, const int64_t* __restrict_
   }
 }
 
-// 16-byte vector reduction into global memory (sm_90+): one instruction per four channels
-__device__ __forceinline__ void red_add_v4(float* addr, float a, float b, float c, float d) {
-  asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
-}
-
 template <typename PIX, bool INTERP, int VEC>
 __device__ __forceinline__ void scatter_chunk(float* __restrict__ gmap_b /* image + chunk offset */,
                                               const PIX* __restrict__ pix, int64_t p, int C, int H, int W,
@@ -327,112 +322,70 @@ gather_pool_bwd_cl_kernel(const T* __restrict__ gout, const int64_t* __restrict_
   }
 }
 
-template <typename T> static int gp_cl_lpr(int64_t C) {
-  const int64_t cv = C / Vec16<T>::N;
-  return cv <= 4 ? 4 : (cv <= 8 ? 8 : (cv <= 16 ? 16 : 32));
-}
 template <typename T> static bool gp_cl_vec_ok(const void* map, const void* rows, int64_t C, int64_t H, int64_t W) {
-  return C % Vec16<T>::N == 0 && aligned16(map) && aligned16(rows) && C < (1 << 20) && H * W < (1ll << 31);
-}
-static inline int gp_cl_grid(int64_t items, int rpi, int unroll) {
-  int64_t blocks = (items + (int64_t)kGpWarps * rpi * unroll - 1) / ((int64_t)kGpWarps * rpi * unroll);
-  const int64_t cap = (int64_t)kNumSMs * 8;
-  return (int)(blocks > cap ? cap : (blocks < 1 ? 1 : blocks));
+  return vec16_ok<T>(C, map, rows) && C < (1 << 20) && H * W < (1ll << 31);
 }
 
-static inline int gp_grid(int64_t total) {
-  int64_t blocks = (total + 255) / 256;
-  const int64_t cap = (int64_t)kNumSMs * 16;
-  return (int)(blocks > cap ? cap : (blocks < 1 ? 1 : blocks));
+// f(T{}, PIX{}, std::bool_constant<CL>{}, std::integral_constant<int, RED>{}) for the storage type, pixel
+// coordinate type (int16 / int32), map layout (channels-last / NCHW) and reduce of a call
+template <typename F>
+static int gp_dispatch(const char* who, int dtype, int reduce, int channels_last, int pix_is_i16, F&& f) {
+  if (!known_dtype(dtype)) return failf(DVA_EINVAL, "%s: unknown dtype", who);
+  int rc = DVA_OK;
+  const bool known = with_reduce(reduce, [&](auto red) {
+    rc = with_dtype(dtype, [&](auto t) {
+      auto pix = [&](auto cl) { return pix_is_i16 ? f(t, int16_t{}, cl, red) : f(t, int32_t{}, cl, red); };
+      return channels_last ? pix(std::true_type{}) : pix(std::false_type{});
+    });
+  });
+  return known ? rc : failf(DVA_EINVAL, "%s: unknown reduce", who);
 }
 
-template <typename T, typename PIX, bool CL, bool INTERP>
-static int gp_fwd_red(const void* fmap, const int64_t* img, const void* pix, const int64_t* aptr,
-                      void* out, int64_t* arg, int64_t C, int64_t H, int64_t W, int64_t Vw,
-                      int64_t P, float mw1, float mh1, int reduce, cudaStream_t st, int64_t B) {
+template <typename T, typename PIX, bool CL, int RED, bool INTERP>
+static int gp_fwd(const void* fmap, const int64_t* img, const void* pix, const int64_t* aptr,
+                  void* out, int64_t* arg, int64_t C, int64_t H, int64_t W, int64_t Vw,
+                  int64_t P, float mw1, float mh1, cudaStream_t st, int64_t B) {
   if constexpr (CL) {
     if (gp_cl_vec_ok<T>(fmap, out, C, H, W)) {
-      const int lpr = gp_cl_lpr<T>(C);
-      const int64_t cvv = C / Vec16<T>::N;
-      const int64_t items = Vw * ((cvv + lpr - 1) / lpr);
-      const int gridv = gp_cl_grid(items, 32 / lpr, INTERP ? 2 : 4);
-#define GP_FV(R, L) gather_pool_fwd_cl_kernel<T, PIX, L, R, INTERP><<<gridv, kGpWarps * 32, 0, st>>>((const T*)fmap, img, (const PIX*)pix, aptr, (T*)out, arg, (int)C, (int)H, (int)W, Vw, P, mw1, mh1, B)
-#define GP_FVL(R) do { if (lpr == 4) GP_FV(R, 4); else if (lpr == 8) GP_FV(R, 8); else if (lpr == 16) GP_FV(R, 16); else GP_FV(R, 32); } while (0)
-      switch (reduce) {
-        case DVA_SUM: GP_FVL(DVA_SUM); break;
-        case DVA_MEAN: GP_FVL(DVA_MEAN); break;
-        case DVA_MAX: GP_FVL(DVA_MAX); break;
-        case DVA_MIN: GP_FVL(DVA_MIN); break;
-        default: return fail(DVA_EINVAL, "gather_pool_fwd: unknown reduce");
-      }
-#undef GP_FVL
-#undef GP_FV
+      const int64_t cv = C / Vec16<T>::N;
+      with_lpr(cv, [&](auto lpr) {
+        constexpr int LPR = decltype(lpr)::value;
+        const int grid = grid_cap(Vw * ((cv + LPR - 1) / LPR), kGpWarps * (32 / LPR) * (INTERP ? 2 : 4), 8);
+        gather_pool_fwd_cl_kernel<T, PIX, LPR, RED, INTERP><<<grid, kGpWarps * 32, 0, st>>>(
+            (const T*)fmap, img, (const PIX*)pix, aptr, (T*)out, arg, (int)C, (int)H, (int)W, Vw, P, mw1, mh1, B);
+      });
       return check_launch("gather_pool_fwd(cl)");
     }
   }
-  const int grid = gp_grid(Vw * C);
-#define GP_F(R) gather_pool_fwd_kernel<T, PIX, CL, R, INTERP><<<grid, 256, 0, st>>>((const T*)fmap, img, (const PIX*)pix, aptr, (T*)out, arg, C, H, W, Vw, P, mw1, mh1, B)
-  switch (reduce) {
-    case DVA_SUM: GP_F(DVA_SUM); break;
-    case DVA_MEAN: GP_F(DVA_MEAN); break;
-    case DVA_MAX: GP_F(DVA_MAX); break;
-    case DVA_MIN: GP_F(DVA_MIN); break;
-    default: return fail(DVA_EINVAL, "gather_pool_fwd: unknown reduce");
-  }
-#undef GP_F
+  gather_pool_fwd_kernel<T, PIX, CL, RED, INTERP><<<grid_cap(Vw * C, 256, 16), 256, 0, st>>>(
+      (const T*)fmap, img, (const PIX*)pix, aptr, (T*)out, arg, C, H, W, Vw, P, mw1, mh1, B);
   return check_launch("gather_pool_fwd");
 }
 
-template <typename T, typename PIX, bool CL, bool INTERP>
-static int gp_bwd_red(const void* gout, const int64_t* img, const void* pix, const int64_t* aptr,
-                      const int64_t* arg, float* gfmap, int64_t C, int64_t H, int64_t W,
-                      int64_t Vw, float mw1, float mh1, int reduce, cudaStream_t st, int64_t B) {
+template <typename T, typename PIX, bool CL, int RED, bool INTERP>
+static int gp_bwd(const void* gout, const int64_t* img, const void* pix, const int64_t* aptr,
+                  const int64_t* arg, float* gfmap, int64_t C, int64_t H, int64_t W,
+                  int64_t Vw, float mw1, float mh1, cudaStream_t st, int64_t B) {
   if constexpr (CL) {
     if (gp_cl_vec_ok<T>(gfmap, gout, C, H, W) && C % 4 == 0) {
-      const int lpr = gp_cl_lpr<T>(C);
-      const int64_t cvv = C / Vec16<T>::N;
-      const int64_t items = Vw * ((cvv + lpr - 1) / lpr);
-      const int gridv = gp_cl_grid(items, 32 / lpr, 4);
-#define GP_BV(R, L) gather_pool_bwd_cl_kernel<T, PIX, L, R, INTERP><<<gridv, kGpWarps * 32, 0, st>>>((const T*)gout, img, (const PIX*)pix, aptr, arg, gfmap, (int)C, (int)H, (int)W, Vw, mw1, mh1, B)
-#define GP_BVL(R) do { if (lpr == 4) GP_BV(R, 4); else if (lpr == 8) GP_BV(R, 8); else if (lpr == 16) GP_BV(R, 16); else GP_BV(R, 32); } while (0)
-      switch (reduce) {
-        case DVA_SUM: GP_BVL(DVA_SUM); break;
-        case DVA_MEAN: GP_BVL(DVA_MEAN); break;
-        case DVA_MAX: GP_BVL(DVA_MAX); break;
-        case DVA_MIN: GP_BVL(DVA_MIN); break;
-        default: return fail(DVA_EINVAL, "gather_pool_bwd: unknown reduce");
-      }
-#undef GP_BVL
-#undef GP_BV
+      const int64_t cv = C / Vec16<T>::N;
+      with_lpr(cv, [&](auto lpr) {
+        constexpr int LPR = decltype(lpr)::value;
+        const int grid = grid_cap(Vw * ((cv + LPR - 1) / LPR), kGpWarps * (32 / LPR) * 4, 8);
+        gather_pool_bwd_cl_kernel<T, PIX, LPR, RED, INTERP><<<grid, kGpWarps * 32, 0, st>>>(
+            (const T*)gout, img, (const PIX*)pix, aptr, arg, gfmap, (int)C, (int)H, (int)W, Vw, mw1, mh1, B);
+      });
       return check_launch("gather_pool_bwd(cl)");
     }
   }
-  const int grid = gp_grid(Vw * C);
-#define GP_B(R) gather_pool_bwd_kernel<T, PIX, CL, R, INTERP><<<grid, 256, 0, st>>>((const T*)gout, img, (const PIX*)pix, aptr, arg, gfmap, C, H, W, Vw, mw1, mh1, B)
-  switch (reduce) {
-    case DVA_SUM: GP_B(DVA_SUM); break;
-    case DVA_MEAN: GP_B(DVA_MEAN); break;
-    case DVA_MAX: GP_B(DVA_MAX); break;
-    case DVA_MIN: GP_B(DVA_MIN); break;
-    default: return fail(DVA_EINVAL, "gather_pool_bwd: unknown reduce");
-  }
-#undef GP_B
+  gather_pool_bwd_kernel<T, PIX, CL, RED, INTERP><<<grid_cap(Vw * C, 256, 16), 256, 0, st>>>(
+      (const T*)gout, img, (const PIX*)pix, aptr, arg, gfmap, C, H, W, Vw, mw1, mh1, B);
   return check_launch("gather_pool_bwd");
 }
 
 }  // namespace dva
 
 using namespace dva;
-
-#define GP_DISPATCH(FN, INTERP, ...)                                                      \
-  do {                                                                                    \
-    if (channels_last) {                                                                  \
-      if (pix_is_i16) return FN<T, int16_t, true, INTERP>(__VA_ARGS__);                   \
-      return FN<T, int32_t, true, INTERP>(__VA_ARGS__);                                   \
-    }                                                                                     \
-    if (pix_is_i16) return FN<T, int16_t, false, INTERP>(__VA_ARGS__);                    \
-    return FN<T, int32_t, false, INTERP>(__VA_ARGS__);                                    \
-  } while (0)
 
 template <bool INTERP>
 static int gather_pool_fwd_impl(const char* who, const void* fmap, int channels_last, const int64_t* img,
@@ -448,12 +401,10 @@ static int gather_pool_fwd_impl(const char* who, const void* fmap, int channels_
     return failf(DVA_EINVAL, "%s: bad map / mapping size", who);
   const float mw1 = (float)(map_w - 1), mh1 = (float)(map_h - 1);
   cudaStream_t st = (cudaStream_t)stream;
-  switch (dtype) {
-    case DVA_F32: { using T = float; GP_DISPATCH(gp_fwd_red, INTERP, fmap, img, pix, aptr, out, arg, C, H, W, Vw, P, mw1, mh1, reduce, st, B); }
-    case DVA_BF16: { using T = __nv_bfloat16; GP_DISPATCH(gp_fwd_red, INTERP, fmap, img, pix, aptr, out, arg, C, H, W, Vw, P, mw1, mh1, reduce, st, B); }
-    case DVA_F16: { using T = __half; GP_DISPATCH(gp_fwd_red, INTERP, fmap, img, pix, aptr, out, arg, C, H, W, Vw, P, mw1, mh1, reduce, st, B); }
-    default: return failf(DVA_EINVAL, "%s: unknown dtype", who);
-  }
+  return gp_dispatch(who, dtype, reduce, channels_last, pix_is_i16, [&](auto t, auto p, auto cl, auto red) {
+    return gp_fwd<decltype(t), decltype(p), decltype(cl)::value, decltype(red)::value, INTERP>(
+        fmap, img, pix, aptr, out, arg, C, H, W, Vw, P, mw1, mh1, st, B);
+  });
 }
 
 template <bool INTERP>
@@ -471,12 +422,10 @@ static int gather_pool_bwd_impl(const char* who, const void* grad_out, int chann
     return failf(DVA_EINVAL, "%s: bad map / mapping size", who);
   const float mw1 = (float)(map_w - 1), mh1 = (float)(map_h - 1);
   cudaStream_t st = (cudaStream_t)stream;
-  switch (dtype) {
-    case DVA_F32: { using T = float; GP_DISPATCH(gp_bwd_red, INTERP, grad_out, img, pix, aptr, arg, grad_fmap, C, H, W, Vw, mw1, mh1, reduce, st, B); }
-    case DVA_BF16: { using T = __nv_bfloat16; GP_DISPATCH(gp_bwd_red, INTERP, grad_out, img, pix, aptr, arg, grad_fmap, C, H, W, Vw, mw1, mh1, reduce, st, B); }
-    case DVA_F16: { using T = __half; GP_DISPATCH(gp_bwd_red, INTERP, grad_out, img, pix, aptr, arg, grad_fmap, C, H, W, Vw, mw1, mh1, reduce, st, B); }
-    default: return failf(DVA_EINVAL, "%s: unknown dtype", who);
-  }
+  return gp_dispatch(who, dtype, reduce, channels_last, pix_is_i16, [&](auto t, auto p, auto cl, auto red) {
+    return gp_bwd<decltype(t), decltype(p), decltype(cl)::value, decltype(red)::value, INTERP>(
+        grad_out, img, pix, aptr, arg, grad_fmap, C, H, W, Vw, mw1, mh1, st, B);
+  });
 }
 
 extern "C" int dva_gather_pool_fwd(const void* fmap, int channels_last, const int64_t* img,
@@ -681,7 +630,7 @@ struct Workspace {
 
 static size_t carve(uint8_t* base, int64_t P, int64_t n_entries, int64_t NB, Workspace* w) {
   size_t o = 0;
-  auto take = [&](size_t bytes) { uint8_t* p = base ? base + o : nullptr; o += bk::align256(bytes); return p; };
+  auto take = [&](size_t bytes) { uint8_t* p = base ? base + o : nullptr; o += round256(bytes); return p; };
   uint8_t* p;
   p = take((size_t)(P + 1) * 8); if (w) w->view_of = (int64_t*)p;
   p = take((size_t)(n_entries + 1) * sizeof(Ent)); if (w) w->ent = (Ent*)p;
@@ -694,58 +643,40 @@ static size_t workspace_bytes(int64_t B, int64_t H, int64_t W, int64_t P, int K)
   return carve(nullptr, P, P * K, B * H * W, nullptr) + 256;
 }
 
-template <typename T, typename PIX, bool CL, bool INTERP>
+template <typename T, typename PIX, bool CL, int RED, bool INTERP>
 static int gp_bwd_det(const void* gout, const int64_t* img, const void* pix, const int64_t* aptr,
                       const int64_t* arg, float* gfmap, int64_t B, int64_t C, int64_t H, int64_t W,
-                      int64_t Vw, int64_t P, float mw1, float mh1, int reduce, void* workspace,
-                      cudaStream_t st) {
+                      int64_t Vw, int64_t P, float mw1, float mh1, void* workspace, cudaStream_t st) {
   constexpr int K = INTERP ? 4 : 1;
   const int64_t NB = B * H * W;
   Workspace ws;
-  uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(workspace) + 255) & ~(uintptr_t)255);
-  carve(base, P, P * K, NB, &ws);
+  carve(align256(workspace), P, P * K, NB, &ws);
   cudaError_t e = cudaMemsetAsync(ws.view_of, 0xff, (size_t)P * 8, st);           // -1: slot in no view
   if (e != cudaSuccess) return fail((int)e, "gather_pool_bwd_det: memset failed");
-  slot_views_kernel<<<bk::grid_for(Vw * 32), 256, 0, st>>>(aptr, Vw, P, ws.view_of);
+  slot_views_kernel<<<grid_cap(Vw * 32, 256, 16), 256, 0, st>>>(aptr, Vw, P, ws.view_of);
   int rc = check_launch("gp_det_slot_views");
   if (rc) return rc;
   const PixelKey<PIX, INTERP> key{ws.view_of, img, (const PIX*)pix, B, (int)H, (int)W, mw1, mh1};
   if ((rc = bk::build_index<K>(key, P, NB, ws.idx, st))) return rc;
-  describe_entries<PIX, INTERP><<<bk::grid_for(P * K), 256, 0, st>>>(ws.idx.sorted, ws.idx.off + NB, P * K, ws.view_of,
-                                                                      (const PIX*)pix, (int)H, (int)W, mw1, mh1, ws.ent);
+  describe_entries<PIX, INTERP><<<grid_cap(P * K, 256, 16), 256, 0, st>>>(ws.idx.sorted, ws.idx.off + NB, P * K, ws.view_of,
+                                                                           (const PIX*)pix, (int)H, (int)W, mw1, mh1, ws.ent);
   if ((rc = check_launch("gp_det_describe_entries"))) return rc;
   const T* g = (const T*)gout;
   if constexpr (CL) {
     if (gp_cl_vec_ok<T>(gfmap, gout, C, H, W) && C % 4 == 0) {
-      const int lpr = gp_cl_lpr<T>(C);
-      const int64_t cvv = C / Vec16<T>::N;
-      const int64_t items = NB * ((cvv + lpr - 1) / lpr);
-      const int gridv = gp_cl_grid(items, 32 / lpr, 1);
-#define GD_BV(R, L) gather_pool_bwd_det_cl_kernel<T, L, R, INTERP><<<gridv, kGpWarps * 32, 0, st>>>(g, aptr, arg, ws.idx.off, ws.idx.sorted, ws.ent, gfmap, (int)C, NB)
-#define GD_BVL(R) do { if (lpr == 4) GD_BV(R, 4); else if (lpr == 8) GD_BV(R, 8); else if (lpr == 16) GD_BV(R, 16); else GD_BV(R, 32); } while (0)
-      switch (reduce) {
-        case DVA_SUM: GD_BVL(DVA_SUM); break;
-        case DVA_MEAN: GD_BVL(DVA_MEAN); break;
-        case DVA_MAX: GD_BVL(DVA_MAX); break;
-        case DVA_MIN: GD_BVL(DVA_MIN); break;
-        default: return fail(DVA_EINVAL, "gather_pool_bwd_det: unknown reduce");
-      }
-#undef GD_BVL
-#undef GD_BV
+      const int64_t cv = C / Vec16<T>::N;
+      with_lpr(cv, [&](auto lpr) {
+        constexpr int LPR = decltype(lpr)::value;
+        const int grid = grid_cap(NB * ((cv + LPR - 1) / LPR), kGpWarps * (32 / LPR), 8);
+        gather_pool_bwd_det_cl_kernel<T, LPR, RED, INTERP><<<grid, kGpWarps * 32, 0, st>>>(
+            g, aptr, arg, ws.idx.off, ws.idx.sorted, ws.ent, gfmap, (int)C, NB);
+      });
       return check_launch("gather_pool_bwd_det(cl)");
     }
   }
   const int64_t total = NB * C;
-  const int grid = gp_grid(total);
-#define GD_B(R) gather_pool_bwd_det_kernel<T, CL, R, INTERP><<<grid, 256, 0, st>>>(g, aptr, arg, ws.idx.off, ws.idx.sorted, ws.ent, gfmap, C, H * W, total)
-  switch (reduce) {
-    case DVA_SUM: GD_B(DVA_SUM); break;
-    case DVA_MEAN: GD_B(DVA_MEAN); break;
-    case DVA_MAX: GD_B(DVA_MAX); break;
-    case DVA_MIN: GD_B(DVA_MIN); break;
-    default: return fail(DVA_EINVAL, "gather_pool_bwd_det: unknown reduce");
-  }
-#undef GD_B
+  gather_pool_bwd_det_kernel<T, CL, RED, INTERP><<<grid_cap(total, 256, 16), 256, 0, st>>>(
+      g, aptr, arg, ws.idx.off, ws.idx.sorted, ws.ent, gfmap, C, H * W, total);
   return check_launch("gather_pool_bwd_det");
 }
 
@@ -761,7 +692,7 @@ static int gather_pool_bwd_det_impl(const char* who, const void* grad_out, int c
                                     size_t workspace_bytes, void* stream) {
   if (B < 0 || C < 0 || H < 0 || W < 0 || Vw < 0 || P < 0) return failf(DVA_EINVAL, "%s: negative size", who);
   if (reduce < DVA_SUM || reduce > DVA_MIN) return failf(DVA_EINVAL, "%s: unknown reduce", who);
-  if (dtype < DVA_F32 || dtype > DVA_F16) return failf(DVA_EINVAL, "%s: unknown dtype", who);
+  if (!known_dtype(dtype)) return failf(DVA_EINVAL, "%s: unknown dtype", who);
   const bool work = Vw > 0 && P > 0;
   if (work && C > 0 && (B < 1 || H < 1 || W < 1)) return failf(DVA_EINVAL, "%s: pixels given but the map is empty", who);
   if (B * C * H * W == 0) return DVA_OK;
@@ -779,11 +710,10 @@ static int gather_pool_bwd_det_impl(const char* who, const void* grad_out, int c
   if (workspace_bytes < det::workspace_bytes(B, H, W, P, INTERP ? 4 : 1))
     return failf(DVA_EINVAL, "%s: workspace too small", who);
   const float mw1 = (float)(map_w - 1), mh1 = (float)(map_h - 1);
-  switch (dtype) {
-    case DVA_F32: { using T = float; GP_DISPATCH(det::gp_bwd_det, INTERP, grad_out, img, pix, aptr, arg, grad_fmap, B, C, H, W, Vw, P, mw1, mh1, reduce, workspace, st); }
-    case DVA_BF16: { using T = __nv_bfloat16; GP_DISPATCH(det::gp_bwd_det, INTERP, grad_out, img, pix, aptr, arg, grad_fmap, B, C, H, W, Vw, P, mw1, mh1, reduce, workspace, st); }
-    default: { using T = __half; GP_DISPATCH(det::gp_bwd_det, INTERP, grad_out, img, pix, aptr, arg, grad_fmap, B, C, H, W, Vw, P, mw1, mh1, reduce, workspace, st); }
-  }
+  return gp_dispatch(who, dtype, reduce, channels_last, pix_is_i16, [&](auto t, auto p, auto cl, auto red) {
+    return det::gp_bwd_det<decltype(t), decltype(p), decltype(cl)::value, decltype(red)::value, INTERP>(
+        grad_out, img, pix, aptr, arg, grad_fmap, B, C, H, W, Vw, P, mw1, mh1, workspace, st);
+  });
 }
 
 extern "C" size_t dva_gather_pool_bwd_det_workspace_bytes(int64_t B, int64_t H, int64_t W, int64_t P) {
@@ -851,12 +781,11 @@ extern "C" int dva_transpose_last2(const void* src, void* dst, int64_t B, int64_
   if (!src || !dst) return fail(DVA_EINVAL, "transpose_last2: null pointer");
   if (B > 65535 || (R + 31) / 32 > 65535) return fail(DVA_EUNSUPPORTED, "transpose_last2: batch / row count too large");
   const dim3 grid((unsigned)((S + 31) / 32), (unsigned)((R + 31) / 32), (unsigned)B);
+  if (!known_dtype(dtype)) return fail(DVA_EINVAL, "transpose_last2: unknown dtype");
   cudaStream_t st = (cudaStream_t)stream;
-  switch (dtype) {
-    case DVA_F32: transpose_last2_kernel<float><<<grid, 256, 0, st>>>((const float*)src, (float*)dst, R, S); break;
-    case DVA_BF16:
-    case DVA_F16: transpose_last2_kernel<uint16_t><<<grid, 256, 0, st>>>((const uint16_t*)src, (uint16_t*)dst, R, S); break;
-    default: return fail(DVA_EINVAL, "transpose_last2: unknown dtype");
-  }
+  if (dtype == DVA_F32)   // bf16 and fp16 move as the same 2-byte words
+    transpose_last2_kernel<float><<<grid, 256, 0, st>>>((const float*)src, (float*)dst, R, S);
+  else
+    transpose_last2_kernel<uint16_t><<<grid, 256, 0, st>>>((const uint16_t*)src, (uint16_t*)dst, R, S);
   return check_launch("transpose_last2");
 }

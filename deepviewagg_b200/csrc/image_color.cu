@@ -255,12 +255,6 @@ to_float_vec_kernel(const Tin* __restrict__ in, float* __restrict__ out, int64_t
   }
 }
 
-// grid-stride launches: at most 16 blocks of 256 per SM
-static inline int c_grid(int64_t items) {
-  const int64_t blocks = (items + 255) / 256, cap = (int64_t)kNumSMs * 16;
-  return (int)(blocks > cap ? cap : (blocks < 1 ? 1 : blocks));
-}
-
 }  // namespace dva
 
 using namespace dva;
@@ -332,12 +326,12 @@ extern "C" int dva_image_to_float(const void* in, int in_u8, float* out, int64_t
   const bool vec = aligned16(in) && aligned16(out) && total % 16 == 0 && (cl || HW % 16 == 0);
   if (in_u8) {
     const uint8_t* x = (const uint8_t*)in;
-    if (vec) to_float_vec_kernel<uint8_t><<<c_grid(total / 16), 256, 0, s>>>(x, out, total, HW, (int)C, cl, st);
-    else to_float_kernel<uint8_t><<<c_grid(total), 256, 0, s>>>(x, out, total, HW, (int)C, cl, st);
+    if (vec) to_float_vec_kernel<uint8_t><<<grid_cap(total / 16, 256, 16), 256, 0, s>>>(x, out, total, HW, (int)C, cl, st);
+    else to_float_kernel<uint8_t><<<grid_cap(total, 256, 16), 256, 0, s>>>(x, out, total, HW, (int)C, cl, st);
   } else {
     const float* x = (const float*)in;
-    if (vec) to_float_vec_kernel<float><<<c_grid(total / 4), 256, 0, s>>>(x, out, total, HW, (int)C, cl, st);
-    else to_float_kernel<float><<<c_grid(total), 256, 0, s>>>(x, out, total, HW, (int)C, cl, st);
+    if (vec) to_float_vec_kernel<float><<<grid_cap(total / 4, 256, 16), 256, 0, s>>>(x, out, total, HW, (int)C, cl, st);
+    else to_float_kernel<float><<<grid_cap(total, 256, 16), 256, 0, s>>>(x, out, total, HW, (int)C, cl, st);
   }
   return check_launch("image_to_float");
 }

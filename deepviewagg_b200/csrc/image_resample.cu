@@ -12,12 +12,6 @@ namespace dva {
 
 static constexpr int kPrecisionBits = 32 - 8 - 2;
 
-// grid-stride launches: at most 16 blocks of 256 per SM
-static inline int r_grid(int64_t total) {
-  const int64_t blocks = (total + 255) / 256, cap = (int64_t)kNumSMs * 16;
-  return (int)(blocks > cap ? cap : (blocks < 1 ? 1 : blocks));
-}
-
 // Pillow's clip8: the sum carries a +2^21 rounding term; >> 22, clamped to [0, 255]
 __device__ __forceinline__ uint8_t clip8(int32_t s) {
   const int32_t v = s >> kPrecisionBits;
@@ -112,14 +106,14 @@ static int resample_launch(const uint8_t* in, uint8_t* tmp, uint8_t* out, int64_
                            cudaStream_t st) {
   if (xc) {
     uint8_t* dst = yc ? tmp : out;
-    resample_h_kernel<C><<<r_grid(B * T * Wo), 256, 0, st>>>(in, dst, B, Hi, Wi, T, Wo, xb, xc, kx, xpi, yfirst);
+    resample_h_kernel<C><<<grid_cap(B * T * Wo, 256, 16), 256, 0, st>>>(in, dst, B, Hi, Wi, T, Wo, xb, xc, kx, xpi, yfirst);
     const int rc = check_launch("resample_u8_horizontal");
     if (rc) return rc;
   }
   if (yc) {
     const uint8_t* src = xc ? tmp : in;
     const int64_t Hs = xc ? T : Hi;
-    resample_v_kernel<C><<<r_grid(B * Ho * Wo), 256, 0, st>>>(src, out, B, Hs, Wo, Ho, yb, yc, ky, ypi);
+    resample_v_kernel<C><<<grid_cap(B * Ho * Wo, 256, 16), 256, 0, st>>>(src, out, B, Hs, Wo, Ho, yb, yc, ky, ypi);
     return check_launch("resample_u8_vertical");
   }
   return DVA_OK;
@@ -166,7 +160,7 @@ extern "C" int dva_nonstatic_mask(const uint8_t* imgs, int64_t n, int64_t H, int
   if (H == 0 || W == 0) return DVA_OK;
   if (!imgs || !mask) return fail(DVA_EINVAL, "nonstatic_mask: null pointer");
   cudaStream_t st = (cudaStream_t)stream;
-  const int g = r_grid(H * W);
+  const int g = grid_cap(H * W, 256, 16);
   switch (C) {
     case 1: nonstatic_mask_kernel<1><<<g, 256, 0, st>>>(imgs, n, H, W, mask); break;
     case 2: nonstatic_mask_kernel<2><<<g, 256, 0, st>>>(imgs, n, H, W, mask); break;

@@ -12,8 +12,6 @@
 
 namespace dva {
 
-static inline int t_grid(int64_t total, int per_block = 256) { return bk::grid_for(total, per_block); }
-
 // ---- (a) per-image statistics ----------------------------------------------------------------------------
 // stats layout: count int64 [n]; bbox int32 [n, 4] = (x_min, x_max, y_min, y_max); occ uint32 [n, 8]
 static __global__ void __launch_bounds__(256)
@@ -195,9 +193,9 @@ static size_t carve_coverage(uint8_t* base, int64_t V, int64_t n_img, int64_t N,
   o += bk::carve_index(base, V, n_img, w ? &w->by_img : nullptr);
   o += bk::carve_index(base ? base + o : nullptr, V, N, w ? &w->by_pt : nullptr);
   if (w) w->img_pts = base ? (int64_t*)(base + o) : nullptr;
-  o += bk::align256((size_t)(V + 1) * 8);
+  o += round256((size_t)(V + 1) * 8);
   if (w) w->pt_imgs = base ? (int64_t*)(base + o) : nullptr;
-  o += bk::align256((size_t)(V + 1) * 8);
+  o += round256((size_t)(V + 1) * 8);
   return o;
 }
 
@@ -246,21 +244,19 @@ extern "C" int dva_mapping_image_stats(const int64_t* images, const int64_t* ato
   if (!count || !bbox || (V > 0 && (!images || !atomic_ptr || !pixels)))
     return fail(DVA_EINVAL, "mapping_image_stats: null pointer");
   cudaStream_t st = (cudaStream_t)stream;
-  stats_init<<<t_grid(n_img), 256, 0, st>>>(count, bbox, occ, n_img);
+  stats_init<<<grid_cap(n_img, 256, 16), 256, 0, st>>>(count, bbox, occ, n_img);
   int rc = check_launch("mapping_image_stats_init");
   if (rc) return rc;
   if (V > 0) {
     const float rw = (float)ref_w;
-    const int g = t_grid(V);
-    if (pix_code == 0)
-      stats_accumulate<int16_t><<<g, 256, 0, st>>>(images, atomic_ptr, (const int16_t*)pixels, V, n_img, rw, count, bbox, occ);
-    else if (pix_code == 1)
-      stats_accumulate<int32_t><<<g, 256, 0, st>>>(images, atomic_ptr, (const int32_t*)pixels, V, n_img, rw, count, bbox, occ);
-    else
-      stats_accumulate<int64_t><<<g, 256, 0, st>>>(images, atomic_ptr, (const int64_t*)pixels, V, n_img, rw, count, bbox, occ);
+    with_pix(pix_code, [&](auto p) {
+      using PIX = decltype(p);
+      stats_accumulate<PIX><<<grid_cap(V, 256, 16), 256, 0, st>>>(images, atomic_ptr, (const PIX*)pixels, V, n_img, rw,
+                                                                  count, bbox, occ);
+    });
     if ((rc = check_launch("mapping_image_stats"))) return rc;
   }
-  stats_finalize<<<t_grid(n_img), 256, 0, st>>>(count, bbox, n_img);
+  stats_finalize<<<grid_cap(n_img, 256, 16), 256, 0, st>>>(count, bbox, n_img);
   return check_launch("mapping_image_stats_finalize");
 }
 
@@ -271,7 +267,7 @@ extern "C" int dva_center_roll(const uint32_t* occ, int64_t n_img, int angular_r
   if (ref_w <= 0) return fail(DVA_EINVAL, "center_roll: ref_w must be positive");
   if (n_img == 0) return DVA_OK;
   if (!occ || !rollings) return fail(DVA_EINVAL, "center_roll: null pointer");
-  center_roll_kernel<<<t_grid(n_img * 32), 256, 0, (cudaStream_t)stream>>>(occ, n_img, 256 / angular_res,
+  center_roll_kernel<<<grid_cap(n_img * 32, 256, 16), 256, 0, (cudaStream_t)stream>>>(occ, n_img, 256 / angular_res,
                                                                           (float)ref_w, rollings);
   return check_launch("center_roll");
 }
@@ -295,7 +291,7 @@ extern "C" int dva_image_remap(const void* in, void* out, int64_t B, int64_t C, 
   a.rolls = rolls; a.offsets = offsets; a.flip = flip ? 1 : 0; a.channels_last = channels_last ? 1 : 0;
   const int out_aligned = aligned16(out) && (a.row_bytes % 16 == 0);
   const int64_t total = B * a.rows_per_img * a.chunks_per_row;
-  remap_kernel<<<t_grid(total), 256, 0, (cudaStream_t)stream>>>(a, total, out_aligned);
+  remap_kernel<<<grid_cap(total, 256, 16), 256, 0, (cudaStream_t)stream>>>(a, total, out_aligned);
   return check_launch("image_remap");
 }
 
@@ -318,7 +314,7 @@ extern "C" int dva_coverage_index(const int64_t* gimg, const int64_t* vpoint, in
   int rc = bk::build_index<1>(KeyFrom{gimg}, V, n_img, w.by_img, st, /*order=*/false);
   if (rc) return rc;
   if ((rc = bk::build_index<1>(KeyFrom{vpoint}, V, N, w.by_pt, st, /*order=*/false))) return rc;
-  coverage_fill<<<t_grid(V > n_img ? (V > N ? V : N) : (n_img > N ? n_img : N)), 256, 0, st>>>(
+  coverage_fill<<<grid_cap(V > n_img ? (V > N ? V : N) : (n_img > N ? n_img : N), 256, 16), 256, 0, st>>>(
       gimg, vpoint, w.by_img.bucket, w.by_pt.bucket, V, w.img_pts, w.pt_imgs, w.by_img.off, n_img, unseen, seen, N);
   return check_launch("coverage_fill");
 }

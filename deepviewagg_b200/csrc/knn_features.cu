@@ -228,12 +228,6 @@ neighborhood_features_kernel(const float* __restrict__ xyz, const int64_t* __res
   }
 }
 
-static inline int k_grid(int64_t total, int threads) {
-  int64_t blocks = (total + threads - 1) / threads;
-  const int64_t cap = (int64_t)kNumSMs * 16;
-  return (int)(blocks > cap ? cap : (blocks < 1 ? 1 : blocks));
-}
-
 }  // namespace dva
 
 using namespace dva;
@@ -243,7 +237,7 @@ extern "C" int dva_knn_cell_ids(const float* xyz, int64_t* cell, int64_t n, floa
   if (n < 0 || gx < 1 || gy < 1 || gz < 1 || !(cell_size > 0.f)) return fail(DVA_EINVAL, "knn_cell_ids: bad sizes");
   if (n == 0) return DVA_OK;
   if (!xyz || !cell) return fail(DVA_EINVAL, "knn_cell_ids: null pointer");
-  knn_cell_ids_kernel<<<k_grid(n, 256), 256, 0, (cudaStream_t)stream>>>(xyz, cell, n, ox, oy, oz, 1.f / cell_size, gx, gy, gz);
+  knn_cell_ids_kernel<<<grid_cap(n, 256, 16), 256, 0, (cudaStream_t)stream>>>(xyz, cell, n, ox, oy, oz, 1.f / cell_size, gx, gy, gz);
   return check_launch("knn_cell_ids");
 }
 
@@ -257,11 +251,11 @@ extern "C" int dva_knn_grid(const float* xyz_sorted, const int64_t* cell_sorted,
   if (!xyz_sorted || !cell_sorted || !order || !cell_ptr || !neighbors) return fail(DVA_EINVAL, "knn_grid: null pointer");
   // the self case: the search set is its own query set
   if (k <= kKnnMax)
-    knn_grid_kernel<kKnnMax, false><<<k_grid(n, 128), 128, 0, (cudaStream_t)stream>>>(
+    knn_grid_kernel<kKnnMax, false><<<grid_cap(n, 128, 16), 128, 0, (cudaStream_t)stream>>>(
         xyz_sorted, cell_sorted, order, n, xyz_sorted, order, cell_ptr, n, k, ox, oy, oz, cell_size, gx, gy, gz,
         nullptr, 0, 0, 0, neighbors, dist2);
   else
-    knn_grid_kernel<kKnnMaxWide, false><<<k_grid(n, 128), 128, 0, (cudaStream_t)stream>>>(
+    knn_grid_kernel<kKnnMaxWide, false><<<grid_cap(n, 128, 16), 128, 0, (cudaStream_t)stream>>>(
         xyz_sorted, cell_sorted, order, n, xyz_sorted, order, cell_ptr, n, k, ox, oy, oz, cell_size, gx, gy, gz,
         nullptr, 0, 0, 0, neighbors, dist2);
   return check_launch("knn_grid");
@@ -282,11 +276,11 @@ extern "C" int dva_knn_query(const float* query_sorted, const int64_t* query_cel
     return fail(DVA_EINVAL, "knn_query: null pointer");
   const int GX = (gx + kKnnBlk - 1) / kKnnBlk, GY = (gy + kKnnBlk - 1) / kKnnBlk, GZ = (gz + kKnnBlk - 1) / kKnnBlk;
   if (k <= kKnnMax)
-    knn_grid_kernel<kKnnMax, true><<<k_grid(nq, 128), 128, 0, (cudaStream_t)stream>>>(
+    knn_grid_kernel<kKnnMax, true><<<grid_cap(nq, 128, 16), 128, 0, (cudaStream_t)stream>>>(
         query_sorted, query_cell_sorted, query_order, nq, search_sorted, search_order, cell_ptr, ns, k, ox, oy, oz,
         cell_size, gx, gy, gz, block_counts, GX, GY, GZ, neighbors, dist2);
   else
-    knn_grid_kernel<kKnnMaxWide, true><<<k_grid(nq, 128), 128, 0, (cudaStream_t)stream>>>(
+    knn_grid_kernel<kKnnMaxWide, true><<<grid_cap(nq, 128, 16), 128, 0, (cudaStream_t)stream>>>(
         query_sorted, query_cell_sorted, query_order, nq, search_sorted, search_order, cell_ptr, ns, k, ox, oy, oz,
         cell_size, gx, gy, gz, block_counts, GX, GY, GZ, neighbors, dist2);
   return check_launch("knn_query");
@@ -304,7 +298,7 @@ extern "C" int dva_neighborhood_features(const float* xyz, const int64_t* neighb
     return fail(DVA_EINVAL, "neighborhood_features: null pointer");
   // voxel_density = 1 / voxel**2 evaluated in double, then used as an fp32 scalar            :531
   const float voxel_density = (float)(1.0 / (voxel * voxel));
-  neighborhood_features_kernel<<<k_grid(V, 256), 256, 0, (cudaStream_t)stream>>>(
+  neighborhood_features_kernel<<<grid_cap(V, 256, 16), 256, 0, (cudaStream_t)stream>>>(
       xyz, neighbors, kmax, view_ptr, images, view_point, klist, nk, voxel_density, density, occlusion, out, V);
   return check_launch("neighborhood_features");
 }

@@ -180,9 +180,6 @@ view_cat_sorting_kernel(const int64_t* const* __restrict__ ptrs, const int64_t* 
   }
 }
 
-using bk::grid_for;
-using bk::align256;
-
 struct Workspace {
   int32_t *cnt, *cursor, *n_views, *n_pix, *status;
   int64_t *off, *pix_ptr, *bucket, *sorted, *block_sums;
@@ -191,7 +188,7 @@ struct Workspace {
 
 static size_t carve(uint8_t* base, int64_t n, int64_t N, Workspace* w) {
   size_t o = 0;
-  auto take = [&](size_t bytes) { uint8_t* p = base ? base + o : nullptr; o += align256(bytes); return p; };
+  auto take = [&](size_t bytes) { uint8_t* p = base ? base + o : nullptr; o += round256(bytes); return p; };
   const int64_t nb = bk::scan_block_words(N);
   uint8_t* p;
   p = take((size_t)(N + 1) * 4); if (w) w->cnt = (int32_t*)p;
@@ -234,39 +231,40 @@ extern "C" int dva_mapping_build(const int64_t* point_ids, const int64_t* image_
   if (workspace_bytes < dva_mapping_build_workspace_bytes(n_items, num_points)) return fail(DVA_EINVAL, "mapping_build: workspace too small");
   cudaStream_t st = (cudaStream_t)stream;
   mb::Workspace w;
-  uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(workspace) + 255) & ~(uintptr_t)255);
-  mb::carve(base, n_items, num_points, &w);
+  mb::carve(align256(workspace), n_items, num_points, &w);
   cudaError_t e = cudaMemsetAsync(w.cnt, 0, (size_t)((uint8_t*)w.n_views - (uint8_t*)w.cnt), st);   // cnt + cursor
   if (e == cudaSuccess) e = cudaMemsetAsync(w.status, 0, 256, st);
   if (e != cudaSuccess) return fail((int)e, "mapping_build: memset failed");
   int rc;
   if (n_items > 0) {
-    bk::count_keys<1><<<mb::grid_for(n_items), 256, 0, st>>>(mb::PointKey{point_ids, num_points, w.status}, n_items,
+    bk::count_keys<1><<<grid_cap(n_items, 256, 16), 256, 0, st>>>(mb::PointKey{point_ids, num_points, w.status}, n_items,
                                                              num_points, w.cnt);
     if ((rc = check_launch("mb_count_points"))) return rc;
   }
   if ((rc = bk::exclusive_scan(w.cnt, num_points, w.off, w.block_sums, st))) return rc;
   if (n_items > 0) {
-    bk::scatter_keys<1><<<mb::grid_for(n_items), 256, 0, st>>>(mb::PointKey{point_ids, num_points, nullptr}, n_items,
+    bk::scatter_keys<1><<<grid_cap(n_items, 256, 16), 256, 0, st>>>(mb::PointKey{point_ids, num_points, nullptr}, n_items,
                                                                num_points, w.off, w.cursor, w.bucket);
     if ((rc = check_launch("mb_scatter_items"))) return rc;
   }
-  const int pgrid = mb::grid_for(num_points * 32);
-#define MB_PIX(CALL) do { if (pix_code == 0) { using PIX = int16_t; CALL; } else if (pix_code == 1) { using PIX = int32_t; CALL; } else { using PIX = int64_t; CALL; } } while (0)
+  const int pgrid = grid_cap(num_points * 32, 256, 16);
   if (num_points > 0) {
-    MB_PIX((mb::order_points<PIX><<<pgrid, 256, 0, st>>>(image_ids, pixels, w.off, w.bucket, w.sorted, w.flags, w.n_views,
-                                                          w.n_pix, num_points, dedupe_pixels)));
+    with_pix(pix_code, [&](auto p) {
+      mb::order_points<decltype(p)><<<pgrid, 256, 0, st>>>(image_ids, pixels, w.off, w.bucket, w.sorted, w.flags, w.n_views,
+                                                           w.n_pix, num_points, dedupe_pixels);
+    });
     if ((rc = check_launch("mb_order_points"))) return rc;
   }
   if ((rc = bk::exclusive_scan(w.n_views, num_points, view_ptr, w.block_sums, st))) return rc;
   if ((rc = bk::exclusive_scan(w.n_pix, num_points, w.pix_ptr, w.block_sums, st))) return rc;
   if (num_points > 0 && n_items > 0) {
-    MB_PIX((mb::emit_points<PIX><<<pgrid, 256, 0, st>>>(image_ids, pixels, feat, feat_row, feat_on, (int)F, w.off, w.sorted,
-                                                         w.flags, view_ptr, w.pix_ptr, num_points, images_out, atomic_ptr,
-                                                         pixels_out, feat_out, order_out)));
+    with_pix(pix_code, [&](auto p) {
+      mb::emit_points<decltype(p)><<<pgrid, 256, 0, st>>>(image_ids, pixels, feat, feat_row, feat_on, (int)F, w.off,
+                                                          w.sorted, w.flags, view_ptr, w.pix_ptr, num_points, images_out,
+                                                          atomic_ptr, pixels_out, feat_out, order_out);
+    });
     if ((rc = check_launch("mb_emit_points"))) return rc;
   }
-#undef MB_PIX
   mb::finish_counts<<<1, 1, 0, st>>>(view_ptr, w.pix_ptr, num_points, atomic_ptr, counts, w.status);
   return check_launch("mb_finish_counts");
 }
@@ -277,6 +275,6 @@ extern "C" int dva_view_cat_sorting(const int64_t* const* ptrs, const int64_t* b
                                     int64_t* sorting, int64_t* csr_cat, void* stream) {
   if (S < 1 || N < 0) return fail(DVA_EINVAL, "view_cat_sorting: bad sizes");
   if (!ptrs || !bases || !csr_cat) return fail(DVA_EINVAL, "view_cat_sorting: null pointer");
-  mb::view_cat_sorting_kernel<<<mb::grid_for(N + 1), 256, 0, (cudaStream_t)stream>>>(ptrs, bases, (int)S, N, sorting, csr_cat);
+  mb::view_cat_sorting_kernel<<<grid_cap(N + 1, 256, 16), 256, 0, (cudaStream_t)stream>>>(ptrs, bases, (int)S, N, sorting, csr_cat);
   return check_launch("view_cat_sorting");
 }

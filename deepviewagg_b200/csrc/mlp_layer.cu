@@ -287,13 +287,9 @@ static size_t ml_smem_bytes(int nt) {
   const int KP = nt * 8 + 8;
   return (size_t)(2 * kMlN * KP + 6 * kMlN + kMlWarps * 2 * kMlRows * (2 * kMlNP + KP)) * sizeof(float);
 }
-static int ml_grid(int64_t M, int nt) {
-  const int64_t tiles = (M + kMlRows - 1) / kMlRows;
-  const int64_t want = (tiles + kMlWarps - 1) / kMlWarps;
-  const int64_t cap = (int64_t)kNumSMs * (nt == 8 ? 2 : 3);   // shared memory: 92 KB (K = 64) / 67 KB (K = 32) per CTA
-  return (int)(want < cap ? (want < 1 ? 1 : want) : cap);
-}
-static size_t ml_round256(size_t b) { return (b + 255) & ~(size_t)255; }
+// one dW partial per CTA: the workspace query and the launch share the grid.  Shared memory: 92 KB (K = 64) / 67 KB
+// (K = 32) per CTA
+static int ml_grid(int64_t M, int nt) { return grid_cap(M, kMlRows * kMlWarps, nt == 8 ? 2 : 3); }
 
 template <int NT>
 static int ml_launch(const MlParams& p, int grid, cudaStream_t st) {
@@ -317,7 +313,7 @@ extern "C" int dva_mlp_layer_bwd_supported(int64_t M, int64_t N, int64_t K) {
 
 extern "C" size_t dva_mlp_layer_bwd_workspace_bytes(int64_t M, int64_t N, int64_t K) {
   if (!dva_mlp_layer_bwd_supported(M, N, K)) return 0;
-  return ml_round256(dva_bn_workspace_bytes(M, N)) + (size_t)ml_grid(M, ml_nt(K)) * N * K * sizeof(float);
+  return round256(dva_bn_workspace_bytes(M, N)) + (size_t)ml_grid(M, ml_nt(K)) * N * K * sizeof(float);
 }
 
 extern "C" int dva_mlp_layer_bwd(const float* dA, const float* Z, const float* X, const float* W, const float* gamma,
@@ -331,7 +327,7 @@ extern "C" int dva_mlp_layer_bwd(const float* dA, const float* Z, const float* X
   if (!workspace || workspace_bytes < dva_mlp_layer_bwd_workspace_bytes(M, N, K)) return fail(DVA_EINVAL, "mlp_layer_bwd: workspace too small");
   cudaStream_t st = (cudaStream_t)stream;
   // pass 1: dgamma_dbeta = [sum g ; sum g zhat] (bn_act.cu; dz = nullptr stops after the reduction)
-  const size_t bn_bytes = ml_round256(dva_bn_workspace_bytes(M, N));
+  const size_t bn_bytes = round256(dva_bn_workspace_bytes(M, N));
   int rc = dva_bn_act_bwd(dA, Z, gamma, beta, mean, invstd, nullptr, dgamma_dbeta, M, N, slope, 1, DVA_F32, workspace,
                           bn_bytes, stream);
   if (rc) return rc;

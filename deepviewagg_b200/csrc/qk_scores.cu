@@ -144,18 +144,6 @@ static inline int qk_vec_cpr(int64_t G, int64_t D, const void* a, const void* b,
   if (!aligned16(a) || !aligned16(b) || (c && !aligned16(c)) || (d && !aligned16(d))) return 0;
   return (int)cpr;
 }
-static inline int qk_vec_grid(int64_t N, int cpr) {
-  const int64_t warps = (N + (32 / cpr) - 1) / (32 / cpr);
-  int64_t blocks = (warps + 7) / 8;
-  const int64_t cap = (int64_t)kNumSMs * 16;
-  return (int)(blocks > cap ? cap : (blocks < 1 ? 1 : blocks));
-}
-
-static inline int qk_grid(int64_t total) {
-  int64_t blocks = (total + 255) / 256;
-  const int64_t cap = (int64_t)kNumSMs * 16;
-  return (int)(blocks > cap ? cap : (blocks < 1 ? 1 : blocks));
-}
 
 }  // namespace dva
 
@@ -169,16 +157,15 @@ extern "C" int dva_qk_scores_fwd(const float* keys, const float* queries, const 
   if (!keys || !queries || !ptr || !compat) return fail(DVA_EINVAL, "qk_scores_fwd: null pointer");
   cudaStream_t st = (cudaStream_t)stream;
   if (const int cpr = qk_vec_cpr(G, D, keys, queries, nullptr, nullptr)) {
-    const int grid = qk_vec_grid(N, cpr);
-    const float4* k4 = reinterpret_cast<const float4*>(keys);
-    const float4* q4 = reinterpret_cast<const float4*>(queries);
-#define QK_F(C) qk_scores_fwd_vec_kernel<C><<<grid, 256, 0, st>>>(k4, q4, ptr, compat, N, (int)G, (int)(D / 4), scale)
-    switch (cpr) { case 1: QK_F(1); break; case 2: QK_F(2); break; case 4: QK_F(4); break; case 8: QK_F(8); break;
-                   case 16: QK_F(16); break; default: QK_F(32); break; }
-#undef QK_F
+    const int grid = grid_cap(N, 8 * (32 / cpr), 16);   // 8 warps of 32 / cpr points
+    with_value<1, 2, 4, 8, 16, 32>(cpr, [&](auto c) {
+      qk_scores_fwd_vec_kernel<decltype(c)::value><<<grid, 256, 0, st>>>(
+          reinterpret_cast<const float4*>(keys), reinterpret_cast<const float4*>(queries), ptr, compat, N, (int)G,
+          (int)(D / 4), scale);
+    });
     return check_launch("qk_scores_fwd(vec)");
   }
-  qk_scores_fwd_kernel<<<qk_grid(N * G), 256, 0, st>>>(keys, queries, ptr, compat, N, (int)G, (int)D, scale);
+  qk_scores_fwd_kernel<<<grid_cap(N * G, 256, 16), 256, 0, st>>>(keys, queries, ptr, compat, N, (int)G, (int)D, scale);
   return check_launch("qk_scores_fwd");
 }
 
@@ -192,14 +179,15 @@ extern "C" int dva_qk_scores_bwd(const float* keys, const float* queries, const 
     return fail(DVA_EINVAL, "qk_scores_bwd: null pointer");
   cudaStream_t st = (cudaStream_t)stream;
   if (const int cpr = (V > 0) ? qk_vec_cpr(G, D, keys, queries, grad_keys, grad_queries) : 0) {
-    const int grid = qk_vec_grid(N, cpr);
-#define QK_B(C) qk_scores_bwd_vec_kernel<C><<<grid, 256, 0, st>>>(reinterpret_cast<const float4*>(keys), reinterpret_cast<const float4*>(queries), ptr, grad_compat, reinterpret_cast<float4*>(grad_keys), reinterpret_cast<float4*>(grad_queries), N, (int)G, (int)(D / 4), scale)
-    switch (cpr) { case 1: QK_B(1); break; case 2: QK_B(2); break; case 4: QK_B(4); break; case 8: QK_B(8); break;
-                   case 16: QK_B(16); break; default: QK_B(32); break; }
-#undef QK_B
+    const int grid = grid_cap(N, 8 * (32 / cpr), 16);
+    with_value<1, 2, 4, 8, 16, 32>(cpr, [&](auto c) {
+      qk_scores_bwd_vec_kernel<decltype(c)::value><<<grid, 256, 0, st>>>(
+          reinterpret_cast<const float4*>(keys), reinterpret_cast<const float4*>(queries), ptr, grad_compat,
+          reinterpret_cast<float4*>(grad_keys), reinterpret_cast<float4*>(grad_queries), N, (int)G, (int)(D / 4), scale);
+    });
     return check_launch("qk_scores_bwd(vec)");
   }
-  qk_scores_bwd_kernel<<<qk_grid(N * G * D), 256, 0, st>>>(
+  qk_scores_bwd_kernel<<<grid_cap(N * G * D, 256, 16), 256, 0, st>>>(
       keys, queries, ptr, grad_compat, grad_keys, grad_queries, N, (int)G, (int)D, scale);
   return check_launch("qk_scores_bwd");
 }

@@ -303,8 +303,7 @@ scatter_add_rows_kernel(const T* __restrict__ src, const int64_t* __restrict__ i
       unpack16<T, VEC>(*reinterpret_cast<const uint4*>(src + v * C + cv * VEC), f);
       float* d = dst + r * C + cv * VEC;
 #pragma unroll
-      for (int j = 0; j < VEC; j += 4)
-        asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(d + j), "f"(f[j]), "f"(f[j + 1]), "f"(f[j + 2]), "f"(f[j + 3]) : "memory");
+      for (int j = 0; j < VEC; j += 4) red_add_v4(d + j, f[j], f[j + 1], f[j + 2], f[j + 3]);
     }
   }
 }
@@ -351,59 +350,31 @@ scatter_add_rows_det_kernel(const T* __restrict__ src, const int64_t* __restrict
 }
 
 // ---- host-side dispatch ---------------------------------------------------------------------
-static inline int grid_for(int64_t total, int threads = 256) {
-  int64_t blocks = (total + threads - 1) / threads;
-  const int64_t cap = (int64_t)kNumSMs * 16;  // 16 resident 256-thread CTAs cover 2048 thr/SM x2
-  if (blocks > cap) blocks = cap;
-  if (blocks < 1) blocks = 1;
-  return (int)blocks;
-}
-
-template <typename T>
-static int vec_width(int64_t K, const void* a, const void* b) {
-  constexpr int V = Vec16<T>::N;
-  if (K % V == 0 && aligned16(a) && aligned16(b)) return V;
-  return 1;
-}
-
+// Grid-stride launches of 256 threads, at most 16 CTAs per SM (2048 threads per SM, twice over).
 template <typename T, int VEC>
 static int seg_fwd_launch(const void* src, const int64_t* ptr, void* out, int64_t* arg,
                           int64_t n_seg, int64_t n_items, int64_t K, int reduce,
                           cudaStream_t st) {
-  const int grid = grid_for(n_seg * (K / VEC));
-  const T* s = (const T*)src; T* o = (T*)out;
-  switch (reduce) {
-    case DVA_SUM:  segment_csr_fwd_kernel<T, VEC, DVA_SUM><<<grid, 256, 0, st>>>(s, ptr, o, arg, n_seg, n_items, K); break;
-    case DVA_MEAN: segment_csr_fwd_kernel<T, VEC, DVA_MEAN><<<grid, 256, 0, st>>>(s, ptr, o, arg, n_seg, n_items, K); break;
-    case DVA_MAX:  segment_csr_fwd_kernel<T, VEC, DVA_MAX><<<grid, 256, 0, st>>>(s, ptr, o, arg, n_seg, n_items, K); break;
-    case DVA_MIN:  segment_csr_fwd_kernel<T, VEC, DVA_MIN><<<grid, 256, 0, st>>>(s, ptr, o, arg, n_seg, n_items, K); break;
-    default: return fail(DVA_EINVAL, "segment_csr_fwd: unknown reduce");
-  }
+  const int grid = grid_cap(n_seg * (K / VEC), 256, 16);
+  if (!with_reduce(reduce, [&](auto red) {
+        segment_csr_fwd_kernel<T, VEC, decltype(red)::value><<<grid, 256, 0, st>>>((const T*)src, ptr, (T*)out, arg,
+                                                                                  n_seg, n_items, K);
+      }))
+    return fail(DVA_EINVAL, "segment_csr_fwd: unknown reduce");
   return check_launch("segment_csr_fwd");
 }
 
 template <typename T, int VEC>
 static int seg_bwd_launch(const void* gout, const int64_t* ptr, const int64_t* arg, void* gsrc,
                           int64_t n_seg, int64_t n_items, int64_t K, int reduce, cudaStream_t st) {
-  const int grid = grid_for(n_seg * (K / VEC));
-  const T* g = (const T*)gout; T* o = (T*)gsrc;
-  switch (reduce) {
-    case DVA_SUM:  segment_csr_bwd_kernel<T, VEC, DVA_SUM><<<grid, 256, 0, st>>>(g, ptr, arg, o, n_seg, n_items, K); break;
-    case DVA_MEAN: segment_csr_bwd_kernel<T, VEC, DVA_MEAN><<<grid, 256, 0, st>>>(g, ptr, arg, o, n_seg, n_items, K); break;
-    case DVA_MAX:  segment_csr_bwd_kernel<T, VEC, DVA_MAX><<<grid, 256, 0, st>>>(g, ptr, arg, o, n_seg, n_items, K); break;
-    case DVA_MIN:  segment_csr_bwd_kernel<T, VEC, DVA_MIN><<<grid, 256, 0, st>>>(g, ptr, arg, o, n_seg, n_items, K); break;
-    default: return fail(DVA_EINVAL, "segment_csr_bwd: unknown reduce");
-  }
+  const int grid = grid_cap(n_seg * (K / VEC), 256, 16);
+  if (!with_reduce(reduce, [&](auto red) {
+        segment_csr_bwd_kernel<T, VEC, decltype(red)::value><<<grid, 256, 0, st>>>((const T*)gout, ptr, arg, (T*)gsrc,
+                                                                                  n_seg, n_items, K);
+      }))
+    return fail(DVA_EINVAL, "segment_csr_bwd: unknown reduce");
   return check_launch("segment_csr_bwd");
 }
-
-#define DVA_DISPATCH_DTYPE(dtype, ...)                                        \
-  switch (dtype) {                                                            \
-    case DVA_F32:  { using T = float; __VA_ARGS__; } break;                   \
-    case DVA_BF16: { using T = __nv_bfloat16; __VA_ARGS__; } break;           \
-    case DVA_F16:  { using T = __half; __VA_ARGS__; } break;                  \
-    default: return fail(DVA_EINVAL, "unknown dtype");                        \
-  }
 
 // no segment at all: every element-level output row is uncovered
 static int zero_all_rows(void* dst, int64_t n_items, int64_t K, int dtype, cudaStream_t st) {
@@ -424,13 +395,14 @@ extern "C" int dva_segment_csr_fwd(const void* src, const int64_t* ptr, void* ou
   if (n_seg == 0 || K == 0) return DVA_OK;
   if (!src && n_items > 0) return fail(DVA_EINVAL, "segment_csr_fwd: null src");
   if (!ptr || !out) return fail(DVA_EINVAL, "segment_csr_fwd: null ptr/out");
+  if (!known_dtype(dtype)) return fail(DVA_EINVAL, "segment_csr_fwd: unknown dtype");
   cudaStream_t st = (cudaStream_t)stream;
-  DVA_DISPATCH_DTYPE(dtype, {
-    if (vec_width<T>(K, src, out) > 1)
+  return with_dtype(dtype, [&](auto t) {
+    using T = decltype(t);
+    if (vec16_ok<T>(K, src, out))
       return seg_fwd_launch<T, Vec16<T>::N>(src, ptr, out, arg, n_seg, n_items, K, reduce, st);
     return seg_fwd_launch<T, 1>(src, ptr, out, arg, n_seg, n_items, K, reduce, st);
   });
-  return DVA_OK;
 }
 
 extern "C" int dva_segment_csr_bwd(const void* grad_out, const int64_t* ptr, const int64_t* arg,
@@ -442,13 +414,14 @@ extern "C" int dva_segment_csr_bwd(const void* grad_out, const int64_t* ptr, con
   if (!grad_out || !ptr || !grad_src) return fail(DVA_EINVAL, "segment_csr_bwd: null pointer");
   if ((reduce == DVA_MAX || reduce == DVA_MIN) && !arg)
     return fail(DVA_EINVAL, "segment_csr_bwd: max/min need arg");
+  if (!known_dtype(dtype)) return fail(DVA_EINVAL, "segment_csr_bwd: unknown dtype");
   cudaStream_t st = (cudaStream_t)stream;
-  DVA_DISPATCH_DTYPE(dtype, {
-    if (vec_width<T>(K, grad_out, grad_src) > 1)
+  return with_dtype(dtype, [&](auto t) {
+    using T = decltype(t);
+    if (vec16_ok<T>(K, grad_out, grad_src))
       return seg_bwd_launch<T, Vec16<T>::N>(grad_out, ptr, arg, grad_src, n_seg, n_items, K, reduce, st);
     return seg_bwd_launch<T, 1>(grad_out, ptr, arg, grad_src, n_seg, n_items, K, reduce, st);
   });
-  return DVA_OK;
 }
 
 extern "C" int dva_gather_csr(const void* src, const int64_t* ptr, void* out, int64_t n_seg,
@@ -457,19 +430,20 @@ extern "C" int dva_gather_csr(const void* src, const int64_t* ptr, void* out, in
   if (K == 0 || n_items == 0) return DVA_OK;
   if (n_seg == 0) return zero_all_rows(out, n_items, K, dtype, (cudaStream_t)stream);
   if (!src || !ptr || !out) return fail(DVA_EINVAL, "gather_csr: null pointer");
+  if (!known_dtype(dtype)) return fail(DVA_EINVAL, "gather_csr: unknown dtype");
   cudaStream_t st = (cudaStream_t)stream;
-  DVA_DISPATCH_DTYPE(dtype, {
-    if (vec_width<T>(K, src, out) > 1) {
+  with_dtype(dtype, [&](auto t) {
+    using T = decltype(t);
+    if (vec16_ok<T>(K, src, out)) {
       constexpr int VEC = Vec16<T>::N;
-      gather_csr_kernel<T, VEC><<<grid_for(n_seg * (K / VEC)), 256, 0, st>>>(
+      gather_csr_kernel<T, VEC><<<grid_cap(n_seg * (K / VEC), 256, 16), 256, 0, st>>>(
           (const T*)src, ptr, (T*)out, n_seg, n_items, K);
     } else {
-      gather_csr_kernel<T, 1><<<grid_for(n_seg * K), 256, 0, st>>>((const T*)src, ptr, (T*)out,
-                                                                   n_seg, n_items, K);
+      gather_csr_kernel<T, 1><<<grid_cap(n_seg * K, 256, 16), 256, 0, st>>>((const T*)src, ptr, (T*)out,
+                                                                            n_seg, n_items, K);
     }
-    return check_launch("gather_csr");
   });
-  return DVA_OK;
+  return check_launch("gather_csr");
 }
 
 extern "C" int dva_segment_softmax_csr_fwd(const void* src, const int64_t* ptr, void* out,
@@ -480,17 +454,18 @@ extern "C" int dva_segment_softmax_csr_fwd(const void* src, const int64_t* ptr, 
   if (n_seg == 0) return zero_all_rows(out, n_items, K, dtype, (cudaStream_t)stream);
   if (!src || !ptr || !out) return fail(DVA_EINVAL, "segment_softmax_fwd: null pointer");
   cudaStream_t st = (cudaStream_t)stream;
-  if (dtype == DVA_F32 && K % 4 == 0 && aligned16(src) && aligned16(out)) {
-    segment_softmax_fwd_v4_kernel<<<grid_for(n_seg * (K / 4)), 256, 0, st>>>((const float*)src, ptr, (float*)out, n_seg,
-                                                                           n_items, K, eps, scaling);
+  if (dtype == DVA_F32 && vec16_ok<float>(K, src, out)) {
+    segment_softmax_fwd_v4_kernel<<<grid_cap(n_seg * (K / 4), 256, 16), 256, 0, st>>>(
+        (const float*)src, ptr, (float*)out, n_seg, n_items, K, eps, scaling);
     return check_launch("segment_softmax_fwd");
   }
-  DVA_DISPATCH_DTYPE(dtype, {
-    segment_softmax_fwd_kernel<T><<<grid_for(n_seg * K), 256, 0, st>>>(
+  if (!known_dtype(dtype)) return fail(DVA_EINVAL, "segment_softmax_fwd: unknown dtype");
+  with_dtype(dtype, [&](auto t) {
+    using T = decltype(t);
+    segment_softmax_fwd_kernel<T><<<grid_cap(n_seg * K, 256, 16), 256, 0, st>>>(
         (const T*)src, ptr, (T*)out, n_seg, n_items, K, eps, scaling);
-    return check_launch("segment_softmax_fwd");
   });
-  return DVA_OK;
+  return check_launch("segment_softmax_fwd");
 }
 
 extern "C" int dva_segment_softmax_csr_bwd(const void* out, const void* grad_out,
@@ -502,17 +477,18 @@ extern "C" int dva_segment_softmax_csr_bwd(const void* out, const void* grad_out
   if (n_seg == 0) return zero_all_rows(grad_src, n_items, K, dtype, (cudaStream_t)stream);
   if (!out || !grad_out || !ptr || !grad_src) return fail(DVA_EINVAL, "segment_softmax_bwd: null pointer");
   cudaStream_t st = (cudaStream_t)stream;
-  if (dtype == DVA_F32 && K % 4 == 0 && aligned16(out) && aligned16(grad_out) && aligned16(grad_src)) {
-    segment_softmax_bwd_v4_kernel<<<grid_for(n_seg * (K / 4)), 256, 0, st>>>((const float*)out, (const float*)grad_out, ptr,
-                                                                           (float*)grad_src, n_seg, n_items, K, scaling);
+  if (dtype == DVA_F32 && vec16_ok<float>(K, out, grad_out, grad_src)) {
+    segment_softmax_bwd_v4_kernel<<<grid_cap(n_seg * (K / 4), 256, 16), 256, 0, st>>>(
+        (const float*)out, (const float*)grad_out, ptr, (float*)grad_src, n_seg, n_items, K, scaling);
     return check_launch("segment_softmax_bwd");
   }
-  DVA_DISPATCH_DTYPE(dtype, {
-    segment_softmax_bwd_kernel<T><<<grid_for(n_seg * K), 256, 0, st>>>(
+  if (!known_dtype(dtype)) return fail(DVA_EINVAL, "segment_softmax_bwd: unknown dtype");
+  with_dtype(dtype, [&](auto t) {
+    using T = decltype(t);
+    segment_softmax_bwd_kernel<T><<<grid_cap(n_seg * K, 256, 16), 256, 0, st>>>(
         (const T*)out, (const T*)grad_out, ptr, (T*)grad_src, n_seg, n_items, K, scaling);
-    return check_launch("segment_softmax_bwd");
   });
-  return DVA_OK;
+  return check_launch("segment_softmax_bwd");
 }
 
 extern "C" int dva_heuristic_pool_fwd(const void* x_mod, const float* x_map, int64_t map_stride,
@@ -525,20 +501,21 @@ extern "C" int dva_heuristic_pool_fwd(const void* x_mod, const float* x_map, int
   if (!ptr || !out || !arg || (V > 0 && (!x_mod || !x_map)))
     return fail(DVA_EINVAL, "heuristic_pool: null pointer");
   cudaStream_t st = (cudaStream_t)stream;
-  heuristic_arg_kernel<<<grid_for(N), 256, 0, st>>>(x_map, map_stride, feat, ptr, arg, N, V, use_max);
+  heuristic_arg_kernel<<<grid_cap(N, 256, 16), 256, 0, st>>>(x_map, map_stride, feat, ptr, arg, N, V, use_max);
   int rc = check_launch("heuristic_arg");
   if (rc) return rc;
   if (C == 0) return DVA_OK;
-  DVA_DISPATCH_DTYPE(dtype, {
-    if (vec_width<T>(C, x_mod ? x_mod : out, out) > 1) {
+  if (!known_dtype(dtype)) return fail(DVA_EINVAL, "heuristic_pool: unknown dtype");
+  with_dtype(dtype, [&](auto t) {
+    using T = decltype(t);
+    if (vec16_ok<T>(C, x_mod, out)) {
       constexpr int VEC = Vec16<T>::N;
-      pick_rows_kernel<T, VEC><<<grid_for(N * (C / VEC)), 256, 0, st>>>((const T*)x_mod, arg, (T*)out, N, V, C);
+      pick_rows_kernel<T, VEC><<<grid_cap(N * (C / VEC), 256, 16), 256, 0, st>>>((const T*)x_mod, arg, (T*)out, N, V, C);
     } else {
-      pick_rows_kernel<T, 1><<<grid_for(N * C), 256, 0, st>>>((const T*)x_mod, arg, (T*)out, N, V, C);
+      pick_rows_kernel<T, 1><<<grid_cap(N * C, 256, 16), 256, 0, st>>>((const T*)x_mod, arg, (T*)out, N, V, C);
     }
-    return check_launch("pick_rows");
   });
-  return DVA_OK;
+  return check_launch("pick_rows");
 }
 
 extern "C" int dva_scatter_add_rows(const void* src, const int64_t* idx, float* dst, int64_t V, int64_t R,
@@ -546,17 +523,18 @@ extern "C" int dva_scatter_add_rows(const void* src, const int64_t* idx, float* 
   if (V < 0 || R < 0 || C < 0) return fail(DVA_EINVAL, "scatter_add_rows: negative size");
   if (V == 0 || C == 0) return DVA_OK;
   if (!src || !idx || !dst) return fail(DVA_EINVAL, "scatter_add_rows: null pointer");
+  if (!known_dtype(dtype)) return fail(DVA_EINVAL, "scatter_add_rows: unknown dtype");
   cudaStream_t st = (cudaStream_t)stream;
-  DVA_DISPATCH_DTYPE(dtype, {
-    constexpr int VEC = Vec16<T>::N;
-    if (C % VEC == 0 && aligned16(src) && aligned16(dst)) {
-      scatter_add_rows_kernel<T, VEC><<<grid_for(V * (C / VEC)), 256, 0, st>>>((const T*)src, idx, dst, V, R, C);
+  with_dtype(dtype, [&](auto t) {
+    using T = decltype(t);
+    if (vec16_ok<T>(C, src, dst)) {
+      constexpr int VEC = Vec16<T>::N;
+      scatter_add_rows_kernel<T, VEC><<<grid_cap(V * (C / VEC), 256, 16), 256, 0, st>>>((const T*)src, idx, dst, V, R, C);
     } else {
-      scatter_add_rows_kernel<T, 1><<<grid_for(V * C), 256, 0, st>>>((const T*)src, idx, dst, V, R, C);
+      scatter_add_rows_kernel<T, 1><<<grid_cap(V * C, 256, 16), 256, 0, st>>>((const T*)src, idx, dst, V, R, C);
     }
-    return check_launch("scatter_add_rows");
   });
-  return DVA_OK;
+  return check_launch("scatter_add_rows");
 }
 
 static size_t scatter_rows_det_carve(uint8_t* base, int64_t V, int64_t R, bk::BucketIndex* w) {
@@ -572,7 +550,7 @@ extern "C" int dva_scatter_add_rows_det(const void* src, const int64_t* idx, flo
                                         int64_t C, int dtype, void* workspace, size_t workspace_bytes,
                                         void* stream) {
   if (V < 0 || R < 0 || C < 0) return fail(DVA_EINVAL, "scatter_add_rows_det: negative size");
-  if (dtype < DVA_F32 || dtype > DVA_F16) return fail(DVA_EINVAL, "scatter_add_rows_det: unknown dtype");
+  if (!known_dtype(dtype)) return fail(DVA_EINVAL, "scatter_add_rows_det: unknown dtype");
   if (R == 0 || C == 0) return DVA_OK;
   if (!dst) return fail(DVA_EINVAL, "scatter_add_rows_det: null pointer");
   cudaStream_t st = (cudaStream_t)stream;
@@ -584,18 +562,18 @@ extern "C" int dva_scatter_add_rows_det(const void* src, const int64_t* idx, flo
   if (workspace_bytes < dva_scatter_add_rows_det_workspace_bytes(V, R))
     return fail(DVA_EINVAL, "scatter_add_rows_det: workspace too small");
   bk::BucketIndex w;
-  uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(workspace) + 255) & ~(uintptr_t)255);
-  scatter_rows_det_carve(base, V, R, &w);
+  scatter_rows_det_carve(align256(workspace), V, R, &w);
   int rc = bk::build_index<1>(RowKey{idx, R}, V, R, w, st);
   if (rc) return rc;
-  DVA_DISPATCH_DTYPE(dtype, {
-    constexpr int VEC = Vec16<T>::N;
-    if (C % VEC == 0 && aligned16(src) && aligned16(dst)) {
-      scatter_add_rows_det_kernel<T, VEC><<<grid_for(R * (C / VEC)), 256, 0, st>>>((const T*)src, w.off, w.sorted, dst, R, C);
+  with_dtype(dtype, [&](auto t) {
+    using T = decltype(t);
+    if (vec16_ok<T>(C, src, dst)) {
+      constexpr int VEC = Vec16<T>::N;
+      scatter_add_rows_det_kernel<T, VEC><<<grid_cap(R * (C / VEC), 256, 16), 256, 0, st>>>((const T*)src, w.off, w.sorted,
+                                                                                            dst, R, C);
     } else {
-      scatter_add_rows_det_kernel<T, 1><<<grid_for(R * C), 256, 0, st>>>((const T*)src, w.off, w.sorted, dst, R, C);
+      scatter_add_rows_det_kernel<T, 1><<<grid_cap(R * C, 256, 16), 256, 0, st>>>((const T*)src, w.off, w.sorted, dst, R, C);
     }
-    return check_launch("scatter_add_rows_det");
   });
-  return DVA_OK;
+  return check_launch("scatter_add_rows_det");
 }

@@ -293,12 +293,9 @@ static int sk_launch_rows_mma(const float* A, const float* B, float* D, int64_t 
   constexpr int WS = ((NT * 8 + 31) / 32) * 32 + 8;
   const size_t smem = (size_t)(2 * RED8 * WS + 2 * kSkTile * (REDP > WS ? REDP : WS)) * sizeof(float);
   auto kern = skinny_rows_mma_kernel<TRANS, NT>;
-  if (smem > 48 * 1024) cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  (void)smem_opt_in(kern, smem);
   const int avec = (RED % 4 == 0) && aligned16(A), dvec = (OUT % 4 == 0) && aligned16(D);
-  const int64_t tiles = (M + kSkTile - 1) / kSkTile;
-  const int64_t cap = (int64_t)kNumSMs * 5;
-  const int grid = (int)(tiles < cap ? tiles : cap);
-  kern<<<grid, 128, smem, st>>>(A, B, D, M, RED, OUT, avec, dvec);
+  kern<<<grid_cap(M, kSkTile, 5), 128, smem, st>>>(A, B, D, M, RED, OUT, avec, dvec);
   return check_launch("skinny_gemm(rows, 3xTF32 mma)");
 }
 template <bool TRANS>
@@ -568,11 +565,8 @@ skinny_dw_reduce_kernel(const float* __restrict__ partial, float* __restrict__ D
   if (lane == 0) D[e] = s;
 }
 
-static int sk_dw_grid(int64_t M) {
-  const int64_t tiles = (M + kSkTile - 1) / kSkTile;
-  const int64_t cap = (int64_t)kNumSMs * 3;    // 74 KB of shared memory per CTA at N = K = 32
-  return (int)(tiles < cap ? (tiles < 1 ? 1 : tiles) : cap);
-}
+// one partial per CTA: the workspace query and the launch share the grid.  74 KB of shared memory per CTA at N = K = 32
+static int sk_dw_grid(int64_t M) { return grid_cap(M, kSkTile, 3); }
 
 }  // namespace dva
 
@@ -586,8 +580,7 @@ extern "C" int dva_skinny_gemm_supported(int64_t M, int64_t N, int64_t K, int la
 
 extern "C" size_t dva_skinny_gemm_workspace_bytes(int64_t M, int64_t N, int64_t K, int layout) {
   if (layout != 2) return 16;
-  const int64_t t64 = (M + kSkDwRows - 1) / kSkDwRows, cap = (int64_t)kNumSMs * 4;
-  const size_t ctas = (size_t)(t64 < cap ? t64 : cap);
+  const size_t ctas = (size_t)grid_cap(M, kSkDwRows, 4);   // the 3xTF32 kernel's grid
   const size_t a = (size_t)sk_dw_grid(M), c = a > ctas ? a : ctas;
   return c * (size_t)N * (size_t)K * sizeof(float) + 16;
 }
@@ -610,14 +603,12 @@ extern "C" int dva_skinny_gemm(const float* A, const float* B, float* D, int64_t
     const size_t smem = (size_t)(RED4 * OUTP + 2 * tile_floats) * sizeof(float);
     const int threads = 16 * (OUTP / 8);             // 64 (OUT <= 32) or 128
     const int avec = (RED % 4 == 0) && aligned16(A), dvec = (OUT % 4 == 0) && aligned16(D);
-    const int64_t tiles = (M + kSkTile - 1) / kSkTile;
-    const int64_t cap = (int64_t)kNumSMs * 5;    // ~41 KB per CTA at K = N = 32
-    const int grid = (int)(tiles < cap ? tiles : cap);
+    const int grid = grid_cap(M, kSkTile, 5);    // ~41 KB per CTA at K = N = 32
     if (layout == 0) {
-      if (smem > 48 * 1024) cudaFuncSetAttribute(skinny_rows_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+      (void)smem_opt_in(skinny_rows_kernel<true>, smem);
       skinny_rows_kernel<true><<<grid, threads, smem, st>>>(A, B, D, M, RED, OUT, avec, dvec);
     } else {
-      if (smem > 48 * 1024) cudaFuncSetAttribute(skinny_rows_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+      (void)smem_opt_in(skinny_rows_kernel<false>, smem);
       skinny_rows_kernel<false><<<grid, threads, smem, st>>>(A, B, D, M, RED, OUT, avec, dvec);
     }
     return check_launch("skinny_gemm(rows)");
@@ -627,9 +618,7 @@ extern "C" int dva_skinny_gemm(const float* A, const float* B, float* D, int64_t
     // output N x K in column blocks of at most 32 (64 when N <= 32) so that MT * NT <= 16 register tiles
     const int MT = N <= 32 ? 2 : 4;
     const int kblk = (MT == 2) ? 64 : 32;
-    const int64_t tiles = (M + kSkDwRows - 1) / kSkDwRows;
-    const int64_t cap = (int64_t)kNumSMs * 4;
-    const int grid = (int)(tiles < cap ? tiles : cap);
+    const int grid = grid_cap(M, kSkDwRows, 4);
     if (!workspace || workspace_bytes < (size_t)grid * N * K * sizeof(float))
       return fail(DVA_EINVAL, "skinny_gemm: workspace too small");
     float* partial = reinterpret_cast<float*>(workspace);
@@ -642,15 +631,12 @@ extern "C" int dva_skinny_gemm(const float* A, const float* B, float* D, int64_t
       size_t smem = (size_t)2 * kSkDwRows * (NP + KP) * sizeof(float);
       const size_t red = (size_t)4 * MT * 16 * NT * 8 * sizeof(float);
       if (smem < red) smem = red;
-#define SK_DW(MTv, NTv)                                                                            \
-      do {                                                                                         \
-        auto kern = skinny_dw_mma_kernel<MTv, NTv>;                                                \
-        if (smem > 48 * 1024) cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
-        kern<<<grid, 128, smem, st>>>(A, B, partial, M, (int)N, (int)K, kofs, kcols, avec, bvec);  \
-      } while (0)
-      if (MT == 2) { if (NT == 1) SK_DW(2, 1); else if (NT == 4) SK_DW(2, 4); else SK_DW(2, 8); }
-      else { if (NT == 1) SK_DW(4, 1); else SK_DW(4, 4); }
-#undef SK_DW
+      // the (MT, NT) tile pairs that occur, coded MT * 16 + NT (MT = 4 means kcols <= 32: NT is 1 or 4)
+      with_value<0x21, 0x24, 0x28, 0x41, 0x44>(MT * 16 + NT, [&](auto tile) {
+        auto kern = skinny_dw_mma_kernel<decltype(tile)::value / 16, decltype(tile)::value % 16>;
+        (void)smem_opt_in(kern, smem);
+        kern<<<grid, 128, smem, st>>>(A, B, partial, M, (int)N, (int)K, kofs, kcols, avec, bvec);
+      });
       if (int rc = check_launch("skinny_gemm(dw, 3xTF32 mma)")) return rc;
       skinny_dw_reduce_cols_kernel<<<((int)N * kcols + 7) / 8, 256, 0, st>>>(partial, D, grid, (int)N, (int)K, kofs, kcols);
       if (int rc = check_launch("skinny_gemm(dw reduce)")) return rc;
@@ -663,7 +649,7 @@ extern "C" int dva_skinny_gemm(const float* A, const float* B, float* D, int64_t
   const int N8 = ((int)N + 7) & ~7, K8 = ((int)K + 7) & ~7;
   size_t smem = (size_t)2 * (kSkTile * (N8 + 4) + kSkTile * (K8 + 4)) * sizeof(float);
   if (smem < (size_t)kSkDwThreads * 64 * sizeof(float)) smem = (size_t)kSkDwThreads * 64 * sizeof(float);
-  if (smem > 48 * 1024) cudaFuncSetAttribute(skinny_dw_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  (void)smem_opt_in(skinny_dw_kernel, smem);
   const int avec = (N % 4 == 0) && aligned16(A), bvec = (K % 4 == 0) && aligned16(B);
   float* partial = reinterpret_cast<float*>(workspace);
   skinny_dw_kernel<<<grid, kSkDwThreads, smem, st>>>(A, B, partial, M, (int)N, (int)K, avec, bvec);

@@ -555,8 +555,7 @@ extern "C" int dva_tc_rows_gemm(const float* X, const float* W, float* D, int64_
   float* wlo = whi + (size_t)n_pad * k_red;
   {
     const int64_t total = (int64_t)n_pad * k_red;
-    const int grid = (int)((total + 255) / 256 > 4 * kNumSMs ? 4 * kNumSMs : (total + 255) / 256);
-    tc::split_weight_kernel<<<grid, 256, 0, st>>>(W, whi, wlo, (int)n_out, n_pad, (int)k_red, ldw, transpose_w);
+    tc::split_weight_kernel<<<grid_cap(total, 256, 4), 256, 0, st>>>(W, whi, wlo, (int)n_out, n_pad, (int)k_red, ldw, transpose_w);
     int rc = check_launch("split_weight");
     if (rc) return rc;
   }
@@ -645,7 +644,7 @@ extern "C" int dva_tc_dw_gemm(const float* dZ, const float* X, float* D, int64_t
   rc = check_launch("tc_dw_gemm");
   if (rc) return rc;
   const int64_t total = n_out * k_in;
-  tc::dw_reduce_kernel<<<(int)((total + 255) / 256 > 8 * kNumSMs ? 8 * kNumSMs : (total + 255) / 256), 256, 0, st>>>(
+  tc::dw_reduce_kernel<<<grid_cap(total, 256, 8), 256, 0, st>>>(
       p.partial, D, (int)n_out, (int)k_in, p.n_pad, p.k_pad, sp, ldo);
   return check_launch("tc_dw_reduce");
 }

@@ -632,7 +632,7 @@ template <typename T, int VEC, int LPR, int CPL>
 static int launch_fwd(const VAParams& P, cudaStream_t st) {
   const size_t smem = fwd_smem(P.G);
   auto kern = view_attention_fwd_kernel<T, VEC, LPR, CPL, (CPL >= 4 ? 2 : kMinBlocksFwd)>;
-  if (smem > 48 * 1024) cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  (void)smem_opt_in(kern, smem);
   kern<<<va_grid(kern, smem, P.N), kWarps * 32, smem, st>>>(P);
   return check_launch("view_attention_fwd");
 }
@@ -641,7 +641,7 @@ template <typename T, int VEC, int LPR, int CPL, bool REG>
 static int launch_bwd_k(const VAParams& P, int* grid_out, cudaStream_t st) {
   const size_t smem = bwd_smem(P.G);
   auto kern = view_attention_bwd_kernel<T, VEC, LPR, CPL, (CPL >= 4 ? 2 : kMinBlocksBwd), REG>;
-  if (smem > 48 * 1024) cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  (void)smem_opt_in(kern, smem);
   const int grid = va_grid(kern, smem, P.N);
   *grid_out = grid;
   kern<<<grid, kWarps * 32, smem, st>>>(P);
@@ -656,28 +656,33 @@ static int launch_bwd(const VAParams& P, bool reg, int* grid_out, cudaStream_t s
   return launch_bwd_k<T, VEC, LPR, CPL, true>(P, grid_out, st);
 }
 
-#define DVA_VA_DISPATCH(FN, T, cfg, ...)                                                   \
-  do {                                                                                     \
-    constexpr int V16 = Vec16<T>::N;                                                       \
-    if (cfg.vec == 1) {                                                                    \
-      if (cfg.cpl == 1) return FN<T, 1, 32, 1>(__VA_ARGS__);                               \
-      return FN<T, 1, 32, 4>(__VA_ARGS__);                                                 \
-    }                                                                                      \
-    if (cfg.lpr == 4) return FN<T, V16, 4, 1>(__VA_ARGS__);                                \
-    if (cfg.lpr == 8) return FN<T, V16, 8, 1>(__VA_ARGS__);                                \
-    if (cfg.lpr == 16) return FN<T, V16, 16, 1>(__VA_ARGS__);                              \
-    if (cfg.cpl == 1) return FN<T, V16, 32, 1>(__VA_ARGS__);                               \
-    if (cfg.cpl == 2) return FN<T, V16, 32, 2>(__VA_ARGS__);                               \
-    return FN<T, V16, 32, 4>(__VA_ARGS__);                                                 \
-  } while (0)
+// f(std::integral_constant<int, VEC>{}, <LPR>{}, <CPL>{}) for the configurations choose_config picks, coded
+// [VEC > 1] * 1000 + LPR * 10 + CPL; false for any other
+template <typename T, typename F> static bool with_config(const VAConfig& cfg, F&& f) {
+  return with_value<321, 324, 1041, 1081, 1161, 1321, 1322, 1324>(
+      (cfg.vec == 1 ? 0 : 1000) + cfg.lpr * 10 + cfg.cpl, [&](auto code) {
+        constexpr int c = decltype(code)::value;
+        f(std::integral_constant<int, c >= 1000 ? Vec16<T>::N : 1>{}, std::integral_constant<int, c % 1000 / 10>{},
+          std::integral_constant<int, c % 10>{});
+      });
+}
 
 template <typename T> static int fwd_typed(const VAParams& P, cudaStream_t st) {
-  const VAConfig cfg = choose_config<T>(P, P.out, nullptr, false);
-  DVA_VA_DISPATCH(launch_fwd, T, cfg, P, st);
+  int rc = DVA_OK;
+  if (!with_config<T>(choose_config<T>(P, P.out, nullptr, false), [&](auto vec, auto lpr, auto cpl) {
+        rc = launch_fwd<T, decltype(vec)::value, decltype(lpr)::value, decltype(cpl)::value>(P, st);
+      }))
+    return fail(DVA_EUNSUPPORTED, "view_attention_fwd: no kernel for this row layout");
+  return rc;
 }
 template <typename T> static int bwd_typed(const VAParams& P, int* grid, cudaStream_t st) {
   const VAConfig cfg = choose_config<T>(P, P.gout, P.gx, true);
-  DVA_VA_DISPATCH(launch_bwd, T, cfg, P, cfg.reg, grid, st);
+  int rc = DVA_OK;
+  if (!with_config<T>(cfg, [&](auto vec, auto lpr, auto cpl) {
+        rc = launch_bwd<T, decltype(vec)::value, decltype(lpr)::value, decltype(cpl)::value>(P, cfg.reg, grid, st);
+      }))
+    return fail(DVA_EUNSUPPORTED, "view_attention_bwd: no kernel for this row layout");
+  return rc;
 }
 
 // The G = 4 short-row kernels (ring forward and backward, lane backward) need rows of whole 16-byte chunks, at most
@@ -787,7 +792,7 @@ extern "C" int dva_view_attention_fwd(const void* x, const void* idx, int idx_is
   P.seg_max = seg_max; P.seg_den = seg_den; P.seg_arg = seg_arg;
   P.N = N; P.V = V; P.R = R; P.C = (int)C; P.G = (int)G; P.group_scaling = group_scaling; P.eps = eps;
   cudaStream_t st = (cudaStream_t)stream;
-  if (dtype != DVA_F32 && dtype != DVA_BF16 && dtype != DVA_F16) return fail(DVA_EINVAL, "view_attention_fwd: unknown dtype");
+  if (!known_dtype(dtype)) return fail(DVA_EINVAL, "view_attention_fwd: unknown dtype");
   if (use_ring(P, dtype, ring_fwd_applicable(P, dtype), false)) return va_ring_fwd(P, dtype, st);
   return with_dtype(dtype, [&](auto tag) { return fwd_typed<decltype(tag)>(P, st); });
 }
@@ -836,7 +841,7 @@ extern "C" int dva_view_attention_bwd(const void* x, const void* idx, int idx_is
   P.N = N; P.V = V; P.R = R; P.C = (int)C; P.G = (int)G; P.group_scaling = group_scaling;
   int grid = 1;
   int rc;
-  if (dtype != DVA_F32 && dtype != DVA_BF16 && dtype != DVA_F16) return fail(DVA_EINVAL, "view_attention_bwd: unknown dtype");
+  if (!known_dtype(dtype)) return fail(DVA_EINVAL, "view_attention_bwd: unknown dtype");
   const bool short_rows = short_bwd_applicable(P, dtype);
   if (use_ring(P, dtype, short_rows, true)) {
     rc = va_ring_bwd(P, dtype, &grid, st);

@@ -10,7 +10,6 @@
 // kernel keeps its own exp / division form.
 #pragma once
 #include "dva_common.cuh"
-#include <type_traits>
 
 namespace dva {
 
@@ -142,23 +141,6 @@ __device__ __forceinline__ void store_gate_partial(float* __restrict__ partial, 
 }
 
 // ---- host side
-// f(T{}) with T the storage type of dtype; the C entry points have rejected every other dtype
-template <typename F> decltype(auto) with_dtype(int dtype, F&& f) {
-  switch (dtype) {
-    case DVA_F32: return f(float{});
-    case DVA_BF16: return f(__nv_bfloat16{});
-    default: return f(__half{});
-  }
-}
-// f(std::integral_constant<int, LPR>{}) with LPR the lanes per row of the ring and lane kernels: the smallest of
-// 4, 8, 16, 32 that covers cv 16-byte chunks
-template <typename F> decltype(auto) with_lpr(int cv, F&& f) {
-  if (cv <= 4) return f(std::integral_constant<int, 4>{});
-  if (cv <= 8) return f(std::integral_constant<int, 8>{});
-  if (cv <= 16) return f(std::integral_constant<int, 16>{});
-  return f(std::integral_constant<int, 32>{});
-}
-
 // Persistent grid of the ring and lane kernels, whose warps stride over ranges of PR points: the co-resident CTAs
 // (kNumSMs x occupancy, at most max_ctas_per_sm), about ranges_per_warp ranges per warp and never fewer than 8
 // points per range, and no more CTAs than there are ranges.

@@ -233,12 +233,6 @@ zbuffer_centres_kernel(const uint8_t* __restrict__ seen, const double* __restric
   }
 }
 
-static inline int z_grid(int64_t total) {
-  int64_t blocks = (total + 255) / 256;
-  const int64_t cap = (int64_t)kNumSMs * 16;
-  return (int)(blocks > cap ? cap : (blocks < 1 ? 1 : blocks));
-}
-
 }  // namespace dva
 
 using namespace dva;
@@ -253,7 +247,7 @@ extern "C" int dva_project_equirectangular(const float* xyz, const float* img_po
   if (n == 0) return DVA_OK;
   if (!xyz || !img_pose || !dist || !x_proj || !y_proj || !keep)
     return fail(DVA_EINVAL, "project_equirectangular: null pointer");
-  project_equirect_kernel<<<z_grid(n), 256, 0, (cudaStream_t)stream>>>(
+  project_equirect_kernel<<<grid_cap(n, 256, 16), 256, 0, (cudaStream_t)stream>>>(
       xyz, img_pose, dist, x_proj, y_proj, keep, n, (int)W, (int)H, (int)crop_top,
       (int)crop_bottom, r_min, r_max);
   return check_launch("project_equirect");
@@ -268,7 +262,7 @@ extern "C" int dva_project_camera(const float* xyz, const float* cam, int camera
   if (camera != 1 && camera != 3) return fail(DVA_EUNSUPPORTED, "project_camera: camera must be 1 (pinhole) or 3 (fisheye)");
   if (n == 0) return DVA_OK;
   if (!xyz || !cam || !dist || !x_proj || !y_proj || !keep) return fail(DVA_EINVAL, "project_camera: null pointer");
-  project_camera_kernel<<<z_grid(n), 256, 0, (cudaStream_t)stream>>>(
+  project_camera_kernel<<<grid_cap(n, 256, 16), 256, 0, (cudaStream_t)stream>>>(
       xyz, cam, camera, dist, x_proj, y_proj, keep, n, (int)W, (int)H, (int)crop_top, (int)crop_bottom, r_min, r_max);
   return check_launch("project_camera");
 }
@@ -283,7 +277,7 @@ extern "C" int dva_splat_boxes(const double* x_proj, const double* y_proj, const
   if (m == 0) return DVA_OK;
   if (!x_proj || !y_proj || !dist || !splat) return fail(DVA_EINVAL, "splat_boxes: null pointer");
   if (!aligned16(splat)) return fail(DVA_EALIGN, "splat_boxes: splat must be 16-byte aligned");
-  splat_boxes_kernel<<<z_grid(m), 256, 0, (cudaStream_t)stream>>>(
+  splat_boxes_kernel<<<grid_cap(m, 256, 16), 256, 0, (cudaStream_t)stream>>>(
       x_proj, y_proj, dist, splat, m, (int)W, (int)H, (int)crop_top, (int)crop_bottom, voxel,
       k_swell, log(d_swell), camera, fx, fy);
   return check_launch("splat_boxes");
@@ -297,7 +291,7 @@ extern "C" int dva_splat_boxes_from_width(const double* x_proj, const double* y_
   if (m == 0) return DVA_OK;
   if (!x_proj || !y_proj || !width || !splat) return fail(DVA_EINVAL, "splat_boxes_from_width: null pointer");
   if (!aligned16(splat)) return fail(DVA_EALIGN, "splat_boxes_from_width: splat must be 16-byte aligned");
-  splat_boxes_width_kernel<<<z_grid(m), 256, 0, (cudaStream_t)stream>>>(
+  splat_boxes_width_kernel<<<grid_cap(m, 256, 16), 256, 0, (cudaStream_t)stream>>>(
       x_proj, y_proj, width, splat, m, (int)W, (int)H, (int)crop_top, (int)crop_bottom);
   return check_launch("splat_boxes_from_width");
 }
@@ -314,7 +308,7 @@ extern "C" int dva_zbuffer_splat(const int32_t* splat, const float* dist, const 
   if (m > 0 && !aligned16(splat)) return fail(DVA_EALIGN, "zbuffer_splat: splat must be 16-byte aligned");
   cudaStream_t st = (cudaStream_t)stream;
   const int64_t Hc = H - crop_top - crop_bottom, npix = W * Hc;
-  fill_u64_kernel<<<z_grid(npix), 256, 0, st>>>(zbuf, kEmpty, npix);
+  fill_u64_kernel<<<grid_cap(npix, 256, 16), 256, 0, st>>>(zbuf, kEmpty, npix);
   int rc = check_launch("zbuffer_fill");
   if (rc) return rc;
   if (exact && m > 0) {
@@ -322,15 +316,15 @@ extern "C" int dva_zbuffer_splat(const int32_t* splat, const float* dist, const 
     if (e != cudaSuccess) return fail((int)e, "zbuffer_splat: memset failed");
   }
   if (m > 0) {
-    zbuffer_raster_kernel<<<z_grid(m * kLanesPerPoint), 256, 0, st>>>(splat, dist, zbuf, m, (int)Hc, (int)crop_top);
+    zbuffer_raster_kernel<<<grid_cap(m * kLanesPerPoint, 256, 16), 256, 0, st>>>(splat, dist, zbuf, m, (int)Hc, (int)crop_top);
     rc = check_launch("zbuffer_raster");
     if (rc) return rc;
   }
-  zbuffer_resolve_kernel<<<z_grid(npix), 256, 0, st>>>(zbuf, idx_map, seen, npix, exact);
+  zbuffer_resolve_kernel<<<grid_cap(npix, 256, 16), 256, 0, st>>>(zbuf, idx_map, seen, npix, exact);
   rc = check_launch("zbuffer_resolve");
   if (rc) return rc;
   if (exact && m > 0) {
-    zbuffer_centres_kernel<<<z_grid(m), 256, 0, st>>>(seen, x_proj, y_proj, idx_map, m, (int)Hc, (int)crop_top);
+    zbuffer_centres_kernel<<<grid_cap(m, 256, 16), 256, 0, st>>>(seen, x_proj, y_proj, idx_map, m, (int)Hc, (int)crop_top);
     rc = check_launch("zbuffer_centres");
   }
   return rc;
