@@ -72,6 +72,7 @@ SIGNATURES = {
     "dva_mapping_build": (_i32, [_vp, _vp, _vp, _i32, _vp, _vp, _vp, _i64, _i64, _i64, _i32, _vp, _vp, _vp, _vp, _vp, _vp,
                                  _vp, _vp, _sz, _vp]),
     "dva_view_cat_sorting": (_i32, [_vp, _vp, _i64, _i64, _vp, _vp, _vp]),
+    "dva_linear_gemm_skinny": (_i32, [_i64, _i64, _i64, _i32]),
     "dva_linear_gemm_workspace_bytes": (_sz, [_i64, _i64, _i64, _i32, _i32]),
     "dva_linear_gemm": (_i32, [_vp, _vp, _vp, _i64, _i64, _i64, _i32, _i32, _vp, _sz, _vp]),
     "dva_linear_bnstats_supported": (_i32, [_i64, _i64, _i64]),

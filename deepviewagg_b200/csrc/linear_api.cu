@@ -33,6 +33,12 @@ static bool use_skinny(int64_t M, int64_t N, int64_t K, int layout) {
   return !(N > 32 && K > 32 && N % 4 == 0 && K % 4 == 0);
 }
 
+// 1 when dva_linear_gemm serves the shape with the skinny kernels, which accept any alignment (scalar loads);
+// the wgmma kernels need 16-byte aligned operands
+extern "C" int dva_linear_gemm_skinny(int64_t M, int64_t N, int64_t K, int layout) {
+  return M > 0 && use_skinny(M, N, K, layout) ? 1 : 0;
+}
+
 static bool gemm_shape_ok(int64_t M, int64_t N, int64_t K) {
   return M >= 1 && N >= 4 && K >= 4 && N % 4 == 0 && K % 4 == 0 && M < (1ll << 40) && N <= 65536 && K <= 65536;
 }

@@ -630,6 +630,12 @@ def set_gemm_precision(mode):
     _GEMM_PRECISION["mode"] = {"fp32": 0, "tf32": 1}[mode]
 
 
+def _aligned16(t):
+    """t, or a copy of it when its data does not start on a 16-byte boundary (e.g. a contiguous view at an odd
+    storage offset): the wgmma, bnstats and fused-layer kernels read their rows with TMA / 16-byte loads."""
+    return t if t is None or t.data_ptr() % 16 == 0 else t.clone()
+
+
 def _tc_gemm(a, b, layout, n_out):
     """layout 0: D[M,n_out] = a[M,K] . b[n_out,K]^T;  1: D[M,n_out] = a[M,K] . b[K,n_out];
     2: D[N,n_out] = a[M,N]^T . b[M,n_out]  -- through dva_linear_gemm."""
@@ -642,7 +648,10 @@ def _tc_gemm(a, b, layout, n_out):
         M, K = a.shape
         N = n_out
         out = torch.empty((M, N), dtype=torch.float32, device=a.device)
-    ws = _lib.workspace(_lib.load().dva_linear_gemm_workspace_bytes(M, N, K, layout, prec), a.device)
+    lib = _lib.load()
+    if (a.data_ptr() | b.data_ptr()) % 16 and not lib.dva_linear_gemm_skinny(M, N, K, layout):
+        a, b = _aligned16(a), _aligned16(b)                    # the skinny kernels take any alignment
+    ws = _lib.workspace(lib.dva_linear_gemm_workspace_bytes(M, N, K, layout, prec), a.device)
     launch("dva_linear_gemm", a.device, a, b, out, M, N, K, layout, prec, ws, ws.numel())
     return out
 
@@ -662,6 +671,7 @@ def _linear_bnstats(x, w, running_mean, running_var, momentum, eps):
     (dva_linear_bnstats_fwd), which also updates the running buffers: returns (z, mean, invstd)."""
     M, K = x.shape
     N = w.shape[0]
+    x, w = _aligned16(x), _aligned16(w)
     z = torch.empty((M, N), dtype=torch.float32, device=x.device)
     mean = torch.empty(N, dtype=torch.float32, device=x.device)
     invstd = torch.empty(N, dtype=torch.float32, device=x.device)
@@ -705,7 +715,8 @@ class _LinearStats(torch.autograd.Function):
     @_fwd_f32
     def forward(ctx, x, weight, running_mean, running_var, momentum, eps):
         require_cuda(x, weight)
-        x, w = x.float().contiguous(), weight.float().contiguous()
+        # aligned before saving, so that the backward's wgmma dW reads the same copy
+        x, w = _aligned16(x.float().contiguous()), _aligned16(weight.float().contiguous())
         z, mean, invstd = _linear_bnstats(x, w, running_mean, running_var, momentum, eps)
         ctx.save_for_backward(x, w)
         ctx.mark_non_differentiable(mean, invstd)
@@ -727,7 +738,8 @@ class _MLPLayer(torch.autograd.Function):
     @_fwd_f32
     def forward(ctx, x, weight, gamma, beta, running_mean, running_var, momentum, eps, slope):
         require_cuda(x, weight, gamma, beta)
-        x, w = x.float().contiguous(), weight.float().contiguous()
+        # aligned before saving: dva_mlp_layer_bwd reads the saved x with 16-byte loads too
+        x, w = _aligned16(x.float().contiguous()), _aligned16(weight.float().contiguous())
         g = gamma.detach().float().contiguous() if gamma is not None else None
         b = beta.detach().float().contiguous() if beta is not None else None
         z, mean, invstd = _linear_bnstats(x, w, running_mean, running_var, momentum, eps)
@@ -745,7 +757,7 @@ class _MLPLayer(torch.autograd.Function):
         slope, has_g, has_b, pdt, wdt = ctx.cfg
         M, K = x.shape
         N = w.shape[0]
-        dy = dy.float().contiguous()
+        dy = _aligned16(dy.float().contiguous())
         dx = torch.empty_like(x) if ctx.needs_input_grad[0] else None
         dw = torch.empty_like(w)
         sums = torch.empty((2, N), dtype=torch.float32, device=x.device)

@@ -277,8 +277,10 @@ int dva_neighborhood_features(const float* xyz, const int64_t* neighbors, int km
  *       per-CTA partial tiles reduced in a fixed order): operands 16-byte aligned, N % 4 == 0 and
  *       K % 4 == 0 (else DVA_EUNSUPPORTED; ops.linear zero-pads such widths).
  *   `precision` is accepted for ABI stability (0 or 1) and ignored: every path is fp32-grade.
- *   workspace: dva_linear_gemm_workspace_bytes().
+ *   workspace: dva_linear_gemm_workspace_bytes().  dva_linear_gemm_skinny(): 1 when the skinny kernels
+ *   serve the shape (any operand alignment), 0 when the wgmma kernels do (16-byte aligned operands).
  * ------------------------------------------------------------------------------------------ */
+int dva_linear_gemm_skinny(int64_t M, int64_t N, int64_t K, int layout);
 size_t dva_linear_gemm_workspace_bytes(int64_t M, int64_t N, int64_t K, int layout, int precision);
 int dva_linear_gemm(const float* A, const float* B, float* D, int64_t M, int64_t N, int64_t K, int layout,
                     int precision, void* workspace, size_t workspace_bytes, void* stream);

@@ -22,8 +22,19 @@ RED_NAMES = ("sum", "mean", "max", "min")
 RECORD_ATTEMPTS = 8
 
 
-def record(fn, want=()):
+def _lead_in():
+    """A few sacrificial launches and a short pause at the start of a profiler session, before the kernels under
+    test."""
+    t = torch.zeros(1, device="cuda")
+    for _ in range(16):
+        t.add_(1)
+    torch.cuda.synchronize()
+    time.sleep(0.05)
+
+
+def record(fn, want=(), canon=canonical, seen=SEEN):
     """Run fn() under the profiler; returns (fn's result, set of canonical dva kernel names that ran).
+    canon: demangled name -> canonical name of a listed family, or None; seen: the set every recorded name joins.
 
     The profiler is a lossy observer: under host CPU load, about 1 - 2 % of short sessions come back with
     some or all of their kernel records missing (measured on an H100 over 300-session runs; pausing before
@@ -31,7 +42,11 @@ def record(fn, want=()):
     can come several sessions in a row.  So fn() is run again, after a growing pause, while a name in `want`
     is missing, at most RECORD_ATTEMPTS times.  The dispatch is deterministic and a name is only recorded
     when its kernel ran, so the union over the runs never reports a kernel that did not run: a silent
-    fallback is missing from every run and still fails."""
+    fallback is missing from every run and still fails.  fn() must therefore give the same result every time it
+    runs (a body that updates state in place restores it first).
+
+    Every session starts with a lead-in (_lead_in): late in a long test process the profiler was seen to drop
+    the records of the kernels launched first in a session, in every retry, while keeping the later ones."""
     from torch.profiler import ProfilerActivity, profile
     names, active = set(), False
     for attempt in range(RECORD_ATTEMPTS):
@@ -39,16 +54,17 @@ def record(fn, want=()):
             time.sleep(0.05 * attempt)
         torch.cuda.synchronize()
         with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            _lead_in()
             res = fn()
             torch.cuda.synchronize()
         evs = [e for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA]
         active |= bool(evs)
-        names |= {k for k in (canonical(e.name) for e in evs) if k is not None}
+        names |= {k for k in (canon(e.name) for e in evs) if k is not None}
         if all(w in names for w in want):
             break
     if not active:
         pytest.fail("the profiler recorded no CUDA activity: kernel names cannot be checked")
-    SEEN.update(names)
+    seen.update(names)
     return res, names
 
 

@@ -82,9 +82,9 @@ def kname(family, *args):
         else family
 
 
-def canonical(name):
+def canonical(name, families=FAMILIES):
     p = parse_kernel(name)
-    if p is None or p[0] not in FAMILIES:
+    if p is None or p[0] not in families:
         return None
     return kname(p[0], *p[1])
 
@@ -153,13 +153,13 @@ CASES = _va_cases() + _seg_cases() + _qk_cases()
 CASE_IDS = [c["kernel"] for c in CASES]
 
 
-def library_kernels(lib_path):
+def library_kernels(lib_path, families=FAMILIES):
     """Canonical names of the listed families compiled into `lib_path` (cuobjdump -symbols | c++filt)."""
     cuobjdump = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
     out = subprocess.run([cuobjdump, "-symbols", lib_path], capture_output=True, text=True, check=True).stdout
     mangled = [ln.split()[-1] for ln in out.splitlines() if "STT_FUNC" in ln]
     dem = subprocess.run(["c++filt"], input="\n".join(mangled), capture_output=True, text=True, check=True).stdout
-    return {k for k in (canonical(n) for n in dem.splitlines()) if k is not None}
+    return {k for k in (canonical(n, families) for n in dem.splitlines()) if k is not None}
 
 
 # ------------------------------------------------------------------------------------------------
