@@ -47,8 +47,10 @@ csr_nll_fwd_kernel(const T* __restrict__ logits, const int64_t* __restrict__ lab
       float m = -INFINITY, s = 0.f, xy = 0.f;
       for (int j = 0; j < K; ++j) {
         const float x = Cvt<T>::to_f(row[j]);
+        // a -inf logit adds exp(-inf) = 0; skipping it keeps exp(-inf - -inf) = NaN out of s while m is
+        // still -inf, so a row with one finite logit has a finite lse (a row of -inf only stays NaN, as in torch)
         if (x > m) { s = s * expf(m - x) + 1.f; m = x; }
-        else s += expf(x - m);
+        else if (x != -INFINITY) s += expf(x - m);
         if (j == y) xy = x;
       }
       const float ls = logf(s);

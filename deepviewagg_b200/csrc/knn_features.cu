@@ -69,8 +69,11 @@ knn_grid_kernel(const float* __restrict__ xyz_q, const int64_t* __restrict__ cel
     const int64_t c = cell_q[q];
     const int cx = (int)(c % gx), cy = (int)((c / gx) % gy), cz = (int)(c / ((int64_t)gx * gy));
     // distance from the query to the nearest face of its own cell (shell r adds r * cs); 0 for a
-    // query outside the grid (clamped into a border cell), which keeps the bound conservative
-    const float fx = px - (ox + cx * cs), fy = py - (oy + cy * cs), fz = pz - (oz + cz * cs);
+    // query outside the grid (clamped into a border cell), which keeps the bound conservative.  Faces
+    // are measured from the same p - o the cell assignment used: o + cx * cs rounded at the ulp of |o|,
+    // far more than the margin below once the cloud sits far from the origin (|o| ~ 1e5 m, 5 cm cells)
+    const float rx = px - ox, ry = py - oy, rz = pz - oz;
+    const float fx = rx - cx * cs, fy = ry - cy * cs, fz = rz - cz * cs;
     const float inner = fmaxf(fminf(fminf(fminf(fx, cs - fx), fminf(fy, cs - fy)), fminf(fz, cs - fz)), 0.f);
     int cnt = 0;
     auto offer = [&](float d2, int64_t id) {
@@ -130,6 +133,7 @@ knn_grid_kernel(const float* __restrict__ xyz_q, const int64_t* __restrict__ cel
         const int Rmax = max(GX, max(GY, GZ));
         // lower bound of the distance from the query to [lo, lo + bs) on one axis, shrunk by the
         // cell-assignment margin and by a relative 1e-5 for the rounding of far distances
+        // (p and lo relative to the grid origin, as the fine level's faces)
         auto gap = [&](float p, float lo) {
           const float g = fmaxf(fmaxf(lo - p, p - (lo + bs)), 0.f);
           return fmaxf(g - 1e-5f * g - margin, 0.f);
@@ -145,7 +149,7 @@ knn_grid_kernel(const float* __restrict__ xyz_q, const int64_t* __restrict__ cel
                 if (bx < 0 || bx >= GX) continue;
                 if (blk_cnt[((int64_t)bz * GY + by) * GX + bx] == 0) continue;
                 if (cnt == k) {
-                  const float ax = gap(px, ox + bx * bs), ay = gap(py, oy + by * bs), az = gap(pz, oz + bz * bs);
+                  const float ax = gap(rx, bx * bs), ay = gap(ry, by * bs), az = gap(rz, bz * bs);
                   if (__fadd_rn(__fadd_rn(__fmul_rn(ax, ax), __fmul_rn(ay, ay)), __fmul_rn(az, az)) > bd[k - 1])
                     continue;
                 }
@@ -158,12 +162,12 @@ knn_grid_kernel(const float* __restrict__ xyz_q, const int64_t* __restrict__ cel
           if (cnt == k) {
             // nearest face of the visited block cube that has blocks beyond it
             float reach = INFINITY;
-            if (Cx - R > 0) reach = fminf(reach, px - (ox + (Cx - R) * bs));
-            if (Cx + R + 1 < GX) reach = fminf(reach, (ox + (Cx + R + 1) * bs) - px);
-            if (Cy - R > 0) reach = fminf(reach, py - (oy + (Cy - R) * bs));
-            if (Cy + R + 1 < GY) reach = fminf(reach, (oy + (Cy + R + 1) * bs) - py);
-            if (Cz - R > 0) reach = fminf(reach, pz - (oz + (Cz - R) * bs));
-            if (Cz + R + 1 < GZ) reach = fminf(reach, (oz + (Cz + R + 1) * bs) - pz);
+            if (Cx - R > 0) reach = fminf(reach, rx - (Cx - R) * bs);
+            if (Cx + R + 1 < GX) reach = fminf(reach, (Cx + R + 1) * bs - rx);
+            if (Cy - R > 0) reach = fminf(reach, ry - (Cy - R) * bs);
+            if (Cy + R + 1 < GY) reach = fminf(reach, (Cy + R + 1) * bs - ry);
+            if (Cz - R > 0) reach = fminf(reach, rz - (Cz - R) * bs);
+            if (Cz + R + 1 < GZ) reach = fminf(reach, (Cz + R + 1) * bs - rz);
             if (reach == INFINITY) break;                        // every block visited
             reach = fmaxf(reach - 1e-5f * reach - margin, 0.f);
             if (bd[k - 1] <= reach * reach) break;
