@@ -111,7 +111,15 @@ SIGNATURES = {
     "dva_csr_nll_fwd_workspace_bytes": (_sz, [_i64]),
     "dva_csr_nll_fwd": (_i32, [_vp, _i32, _vp, _vp, _i64, _i64, _i32, _i64, _vp, _vp, _vp, _vp, _sz, _vp]),
     "dva_csr_nll_bwd": (_i32, [_vp, _i32, _vp, _vp, _i64, _i64, _i32, _i64, _vp, _vp, _vp, _vp, _vp]),
-    "dva_csr_pointers_from_sorted": (_i32, [_vp, _vp, _i64, _i64, _vp]),
+    "dva_csr_nll_weighted_fwd_workspace_bytes": (_sz, [_i64]),
+    "dva_csr_nll_weighted_fwd": (_i32, [_vp, _i32, _vp, _vp, _i64, _i64, _i32, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _sz,
+                                        _vp]),
+    "dva_csr_nll_weighted_bwd": (_i32, [_vp, _i32, _vp, _vp, _i64, _i64, _i32, _i64, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "dva_lovasz_keys": (_i32, [_vp, _i32, _i32, _vp, _i64, _i32, _i64, _vp, _vp]),
+    "dva_lovasz_fwd_workspace_bytes": (_sz, [_i64, _i32]),
+    "dva_lovasz_fwd": (_i32, [_vp, _vp, _vp, _i64, _i32, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "dva_lovasz_bwd": (_i32, [_vp, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i32, _vp, _vp]),
+    "dva_csr_pointers_from_sorted":(_i32, [_vp, _vp, _i64, _i64, _vp]),
     "dva_csr_select_values": (_i32, [_vp, _vp, _vp, _vp, _i64, _i64, _vp]),
 }
 

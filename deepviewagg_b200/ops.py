@@ -1096,16 +1096,23 @@ CSR_NLL_MAX_CLASSES = 64
 class _CSRNLLLoss(torch.autograd.Function):
     @staticmethod
     @_fwd
-    def forward(ctx, logits, labels, csr_idx, ignore_index):
+    def forward(ctx, logits, labels, csr_idx, ignore_index, weight):
         V, K = logits.shape
         N = labels.shape[0]
         need_grad = ctx.needs_input_grad[0]
         loss = torch.empty((), dtype=torch.float32, device=logits.device)
         stats = torch.empty(3, dtype=torch.int64, device=logits.device)
         lse = torch.empty(V, dtype=torch.float32, device=logits.device) if need_grad else None
-        ws = _lib.workspace(_lib.load().dva_csr_nll_fwd_workspace_bytes(N), logits.device)
-        launch("dva_csr_nll_fwd", logits.device, logits, dtype_code(logits), labels, csr_idx, V, N, K, int(ignore_index),
-               lse, loss, stats, ws, ws.numel())
+        wsum = None
+        if weight is None:
+            ws = _lib.workspace(_lib.load().dva_csr_nll_fwd_workspace_bytes(N), logits.device)
+            launch("dva_csr_nll_fwd", logits.device, logits, dtype_code(logits), labels, csr_idx, V, N, K,
+                   int(ignore_index), lse, loss, stats, ws, ws.numel())
+        else:
+            wsum = torch.empty(1, dtype=torch.float64, device=logits.device)
+            ws = _lib.workspace(_lib.load().dva_csr_nll_weighted_fwd_workspace_bytes(N), logits.device)
+            launch("dva_csr_nll_weighted_fwd", logits.device, logits, dtype_code(logits), labels, csr_idx, V, N, K,
+                   int(ignore_index), weight, lse, loss, wsum, stats, ws, ws.numel())
         _, bad, bad_csr = stats.tolist()
         if bad:
             raise ValueError(f"csr_nll_loss: {bad} view(s) have a label outside [0, {K}) that is not "
@@ -1113,33 +1120,42 @@ class _CSRNLLLoss(torch.autograd.Function):
         if bad_csr:
             raise ValueError(f"csr_nll_loss: csr_idx must run from 0 to the number of views ({V})")
         ctx.cfg = (V, N, K, int(ignore_index))
-        ctx.save_for_backward(logits, labels, csr_idx, lse, stats)
+        ctx.save_for_backward(logits, labels, csr_idx, lse, stats, weight, wsum)
         return loss
 
     @staticmethod
     @_bwd
     @torch.autograd.function.once_differentiable
     def backward(ctx, grad_loss):
-        logits, labels, csr_idx, lse, stats = ctx.saved_tensors
+        logits, labels, csr_idx, lse, stats, weight, wsum = ctx.saved_tensors
         V, N, K, ignore_index = ctx.cfg
         grad = torch.empty_like(logits)
         g = grad_loss.detach().float().contiguous().view(1)
-        launch("dva_csr_nll_bwd", logits.device, logits, dtype_code(logits), labels, csr_idx, V, N, K, ignore_index,
-               lse, g, stats, grad)
-        return grad, None, None, None
+        if weight is None:
+            launch("dva_csr_nll_bwd", logits.device, logits, dtype_code(logits), labels, csr_idx, V, N, K,
+                   ignore_index, lse, g, stats, grad)
+        else:
+            launch("dva_csr_nll_weighted_bwd", logits.device, logits, dtype_code(logits), labels, csr_idx, V, N, K,
+                   ignore_index, weight, lse, g, wsum, grad)
+        return grad, None, None, None, None
 
 
-def csr_nll_loss(logits, labels, csr_idx=None, ignore_index=-1):
+def csr_nll_loss(logits, labels, csr_idx=None, ignore_index=-1, weight=None):
     """F.nll_loss(F.log_softmax(logits, -1), repeat_interleave(labels, csr_idx.diff()),
-    ignore_index=ignore_index) with the mean reduction (no3d.py:144-154), without the [V] target
-    and [V, K] log-prob tensors: view v takes the label of its point through the CSR.
+    ignore_index=ignore_index, weight=weight) with the mean reduction (no3d.py:144-154,
+    models/segmentation/sparseconv3d.py:41-58), without the [V] target and [V, K] log-prob tensors:
+    view v takes the label of its point through the CSR.
 
     logits [V, K] fp32 / bf16 / fp16 (fp32 math, K <= 64), labels [N] int64, csr_idx [N+1] int64 or
     None for one view per point (V == N, the point-level loss).  Returns a float32 scalar: the mean
     over views whose label is in [0, K) (NaN when there is none, as F.nll_loss); the sum is taken in
     fp64 in a fixed order, so two calls give the same bits.  A label outside [0, K) that is not
-    ignore_index raises ValueError (read back after the forward; no device assert)."""
-    require_cuda(logits, labels, csr_idx)
+    ignore_index raises ValueError (read back after the forward; no device assert).
+
+    weight: optional [K] float32 class weights on the logits' device.  The loss is then
+    sum w[y] (lse - x[y]) / sum w[y] over the counted views (NaN when the weights sum to 0, as in
+    torch), on separate kernels; weight=None runs the unweighted ones."""
+    require_cuda(logits, labels, csr_idx, weight)
     if logits.dim() != 2:
         raise ValueError(f"csr_nll_loss: logits must be [V, K], got shape {tuple(logits.shape)}")
     if logits.dtype not in DTYPE_CODES:
@@ -1157,4 +1173,100 @@ def csr_nll_loss(logits, labels, csr_idx=None, ignore_index=-1):
         csr_idx = _check_csr(csr_idx, logits.device)
         if csr_idx.numel() != labels.shape[0] + 1:
             raise ValueError("csr_nll_loss: csr_idx must have one more entry than labels")
-    return _CSRNLLLoss.apply(logits.contiguous(), labels.contiguous(), csr_idx, ignore_index)
+    if weight is not None:
+        if weight.dtype != torch.float32 or weight.dim() != 1 or weight.shape[0] != K:
+            raise ValueError(f"csr_nll_loss: weight must be a [{K}] float32 tensor, got {weight.dtype} "
+                             f"{tuple(weight.shape)}")
+        if weight.device != logits.device:
+            raise RuntimeError("csr_nll_loss: weight must live on the device of the logits")
+        weight = weight.detach().contiguous()
+    return _CSRNLLLoss.apply(logits.contiguous(), labels.contiguous(), csr_idx, ignore_index, weight)
+
+
+# --------------------------------------------------------------------------------------------
+# Lovász-softmax (metrics/lovasz_loss.py:155-230; csrc/lovasz.cu)
+# --------------------------------------------------------------------------------------------
+LOVASZ_MAX_CLASSES = 64
+
+
+class _LovaszSoftmax(torch.autograd.Function):
+    @staticmethod
+    @_fwd
+    def forward(ctx, probas, labels, class_mult, present, ignore, log_probs):
+        P, K = probas.shape
+        dev = probas.device
+        keys = torch.empty((K, P), dtype=torch.float32, device=dev)
+        launch("dva_lovasz_keys", dev, probas, dtype_code(probas), int(log_probs), labels, P, K, int(ignore), keys)
+        # stable, descending: ties keep point order; ignored points (key -1) go after every valid one
+        skeys, perm = torch.sort(keys, dim=1, descending=True, stable=True)
+        del keys
+        need_grad = ctx.needs_input_grad[0]
+        fgs = torch.empty((K, P), dtype=torch.uint8, device=dev)
+        gsorted = torch.empty((K, P), dtype=torch.float32, device=dev) if need_grad else None
+        loss = torch.empty((), dtype=torch.float32, device=dev)
+        scale = torch.empty(K, dtype=torch.float32, device=dev)
+        ws = _lib.workspace(_lib.load().dva_lovasz_fwd_workspace_bytes(P, K), dev)
+        launch("dva_lovasz_fwd", dev, skeys, perm, labels, P, K, class_mult, int(present), fgs, gsorted, loss, scale,
+               ws, ws.numel())
+        ctx.log_probs = bool(log_probs)
+        if need_grad:
+            ctx.save_for_backward(probas, skeys, perm, fgs, gsorted, scale)
+        return loss
+
+    @staticmethod
+    @_bwd
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_loss):
+        probas, skeys, perm, fgs, gsorted, scale = ctx.saved_tensors
+        P, K = probas.shape
+        grad = torch.empty_like(probas)
+        g = grad_loss.detach().float().contiguous().view(1)
+        launch("dva_lovasz_bwd", probas.device, probas, dtype_code(probas), int(ctx.log_probs), skeys, perm, fgs,
+               gsorted, scale, g, P, K, grad)
+        return grad, None, None, None, None, None
+
+
+def lovasz_softmax(probas, labels, classes="present", ignore=-1, log_probs=False, per_image=False):
+    """Multi-class Lovász-softmax loss: lovasz_softmax_flat(*flatten_probas(probas, labels, ignore),
+    classes) of metrics/lovasz_loss.py:155-230 for [P, K] inputs (per_image=False).
+
+    probas [P, K] fp32 / bf16 / fp16 class probabilities (fp32 math, 2 <= K <= 64), or
+    log-probabilities with log_probs=True (exp taken in the kernel, the gradient chained through it);
+    labels [P] int64; points labelled `ignore` are left out.  classes: 'present' (classes with a
+    valid point), 'all', or a list of class ids (a repeated id counts twice, as in the reference).
+    Returns a float32 scalar, the mean over the kept classes of sum_j e_j g_j (errors sorted
+    descending, g the Jaccard differences); fp64 partials in a fixed order, so two calls give the
+    same bits.  The sort is torch's stable sort: tied errors are ordered by point index (the
+    reference's CPU torch.sort is unstable; the loss does not depend on the order of ties, the
+    gradient of one element of a tied block does).  With no valid point, or no kept class, the loss
+    is 0 and the gradient 0."""
+    if per_image:
+        raise NotImplementedError("lovasz_softmax(per_image=True) is not supported")
+    require_cuda(probas, labels)
+    if probas.dim() != 2:
+        raise ValueError(f"lovasz_softmax: probas must be [P, K], got shape {tuple(probas.shape)}")
+    if probas.dtype not in DTYPE_CODES:
+        raise TypeError(f"lovasz_softmax: unsupported probas dtype {probas.dtype}; expected float32/bfloat16/float16")
+    P, K = probas.shape
+    if K == 1:
+        raise NotImplementedError("lovasz_softmax: the single-class (sigmoid) branch is not supported")
+    if not 2 <= K <= LOVASZ_MAX_CLASSES:
+        raise ValueError(f"lovasz_softmax: {K} classes; this kernel supports 2 to {LOVASZ_MAX_CLASSES}")
+    if labels.dim() != 1 or labels.dtype != torch.int64 or labels.shape[0] != P:
+        raise TypeError(f"lovasz_softmax: labels must be a [{P}] int64 tensor")
+    if labels.device != probas.device:
+        raise RuntimeError("lovasz_softmax: labels must live on the device of probas")
+    if isinstance(classes, str):
+        if classes not in ("all", "present"):
+            raise ValueError(f"lovasz_softmax: classes must be 'all', 'present' or a list, got {classes!r}")
+        mult = [1] * K
+    else:
+        mult = [0] * K
+        for c in classes:
+            c = int(c)
+            if not 0 <= c < K:
+                raise ValueError(f"lovasz_softmax: class {c} outside [0, {K})")
+            mult[c] += 1
+    class_mult = torch.tensor(mult, dtype=torch.int32, device=probas.device)
+    return _LovaszSoftmax.apply(probas.contiguous(), labels.contiguous(), class_mult, classes == "present",
+                                int(ignore), bool(log_probs))

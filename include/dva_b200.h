@@ -550,6 +550,48 @@ int dva_csr_nll_bwd(const void* logits, int dtype, const int64_t* labels, const 
                     int64_t N, int K, int64_t ignore_index, const float* lse, const float* grad_loss,
                     const int64_t* stats, void* grad_logits, void* stream);
 
+/* L2  class-weighted log-softmax NLL       replaces models/segmentation/sparseconv3d.py:41-58
+ *   F.nll_loss(F.log_softmax(logits), labels, ignore_index=-1, weight=dataset.weight_classes), mean reduction,
+ *   over the same inputs as L1 plus weight [K] float32 (device).  Separate kernels: L1 keeps its code and bits.
+ *   dva_csr_nll_weighted_fwd : loss[0] = sum_v w[y_v] (lse_v - x_v[y_v]) / W with W = sum_v w[y_v] over the
+ *                              counted views (fp64 per-CTA partials, dva_csr_nll_weighted_fwd_workspace_bytes(N)
+ *                              bytes, summed in a fixed order; NaN when W is 0, as in torch); wsum[0] = W (fp64)
+ *                              for the backward; lse and stats as L1.
+ *   dva_csr_nll_weighted_bwd : grad_logits = grad_loss[0] / W * w[y_v] * (exp(x - lse) - onehot), 0 on views that
+ *                              do not count.  With w = 1 both give L1's bits. */
+size_t dva_csr_nll_weighted_fwd_workspace_bytes(int64_t N);
+int dva_csr_nll_weighted_fwd(const void* logits, int dtype, const int64_t* labels, const int64_t* csr_idx, int64_t V,
+                             int64_t N, int K, int64_t ignore_index, const float* weight, float* lse, float* loss,
+                             double* wsum, int64_t* stats, void* workspace, size_t workspace_bytes, void* stream);
+int dva_csr_nll_weighted_bwd(const void* logits, int dtype, const int64_t* labels, const int64_t* csr_idx, int64_t V,
+                             int64_t N, int K, int64_t ignore_index, const float* weight, const float* lse,
+                             const float* grad_loss, const double* wsum, void* grad_logits, void* stream);
+
+/* L3  Lovász-softmax                        replaces metrics/lovasz_loss.py:155-230 (lovasz_softmax_flat after
+ *                                           flatten_probas, per_image=False), called by
+ *                                           models/segmentation/sparseconv3d.py:55-57 and
+ *                                           models/segmentation/multimodal/sparseconv3d.py:163-181
+ *   probas [P, K] (fp32 / bf16 / fp16 storage, fp32 math, 1 <= K <= 64), log-probabilities when log_probs (exp
+ *   taken in the kernel), labels [P] int64; a point whose label is ignore_index is left out.
+ *   dva_lovasz_keys : keys [K, P] fp32 = |fg - p| for valid points, -1 for ignored ones.  The caller sorts each
+ *                     row descending and stable into sorted_keys [K, P] and perm [K, P] int64.
+ *   dva_lovasz_fwd  : fgs [K, P] uint8 = fg in sorted order; gsorted [K, P] fp32 (nullable: no gradient) = the
+ *                     Jaccard differences (lovasz_grad) in sorted order, 0 for ignored points; loss[0] = the mean
+ *                     over kept classes of sum e_sorted g, kept_c = class_mult[c] (0 when present and class c
+ *                     has no valid point), 0 when nothing is kept; scale [K] = kept_c / sum kept.  fp64
+ *                     partials in a fixed order (dva_lovasz_fwd_workspace_bytes(P, K) bytes of workspace).
+ *   dva_lovasz_bwd  : grad [P, K] (probas' dtype) = -sign(fg - p) g scale_c grad_loss[0], times p when log_probs,
+ *                     0 for ignored points; every element written once through perm. */
+int dva_lovasz_keys(const void* probas, int dtype, int log_probs, const int64_t* labels, int64_t P, int K,
+                    int64_t ignore_index, float* keys, void* stream);
+size_t dva_lovasz_fwd_workspace_bytes(int64_t P, int K);
+int dva_lovasz_fwd(const float* sorted_keys, const int64_t* perm, const int64_t* labels, int64_t P, int K,
+                   const int* class_mult, int present, uint8_t* fgs, float* gsorted, float* loss, float* scale,
+                   void* workspace, size_t workspace_bytes, void* stream);
+int dva_lovasz_bwd(const void* probas, int dtype, int log_probs, const float* sorted_keys, const int64_t* perm,
+                   const uint8_t* fgs, const float* gsorted, const float* scale, const float* grad_loss, int64_t P,
+                   int K, void* grad, void* stream);
+
 /* C1  CSR pointers from sorted dense ids     replaces csr.py:158-172 + :197-229
  *   ids [n] int64 sorted ascending, values in [0,num_groups) -> ptr [num_groups+1] int64 with
  *   empty groups inserted (from_dense + insert_empty_groups, image.py:1787-1793). */
