@@ -1,4 +1,6 @@
-"""ctypes binding of libdva_b200.so (the C ABI declared in include/dva_b200.h).
+"""ctypes binding of libdva_b200.so (the C ABI declared in include/dva_b200.h) and of libdva_eval.so, the
+evaluation kernels (include/dva_eval.h), which links against the first and shares its error string and launch
+counter.
 
 There is NO fallback: if the shared library is missing or a call fails, a RuntimeError is
 raised.  PyTorch is used above this layer only for device memory and streams.
@@ -13,6 +15,8 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # DVA_B200_LIB: developer knob to load a tuning variant of the same library (bench sweeps)
 LIB_PATH = os.environ.get("DVA_B200_LIB") or os.path.join(_HERE, "libdva_b200.so")
 CSRC_DIR = os.path.join(_HERE, "csrc")
+# libdva_eval.so loads the libdva_b200.so next to it (rpath $ORIGIN), whatever DVA_B200_LIB names
+EVAL_LIB_PATH = os.path.join(_HERE, "libdva_eval.so")
 
 DVA_OK, DVA_EINVAL, DVA_EALIGN, DVA_EUNSUPPORTED = 0, -1, -2, -3
 DVA_F32, DVA_BF16, DVA_F16 = 0, 1, 2
@@ -123,7 +127,19 @@ SIGNATURES = {
     "dva_csr_select_values": (_i32, [_vp, _vp, _vp, _vp, _i64, _i64, _vp]),
 }
 
+# name -> (restype, argtypes); mirrors include/dva_eval.h one to one
+EVAL_SIGNATURES = {
+    "dva_eval_confusion_scores": (_i32, [_vp, _i32, _vp, _vp, _i64, _i32, _i64, _i32, _vp, _vp, _vp]),
+    "dva_eval_confusion_pred": (_i32, [_vp, _vp, _i64, _i32, _i64, _i32, _vp, _vp, _vp]),
+    "dva_eval_vote": (_i32, [_vp, _i32, _vp, _i64, _i64, _i32, _vp, _vp, _vp, _vp, _vp]),
+    "dva_eval_nn_vote": (_i32, [_vp, _vp, _vp, _i64, _i32, _vp, _i64, _vp, _vp, _i64, _i32, _vp, _i64, _i32, _vp,
+                                _vp, _vp, _vp]),
+}
+# status bits of the evaluation kernels (include/dva_eval.h)
+DVA_EVAL_BAD_LABEL, DVA_EVAL_BAD_PRED, DVA_EVAL_BAD_ID = 1, 2, 4
+
 _lib = None
+_eval_lib = None
 
 
 def build(verbose=False):
@@ -158,6 +174,34 @@ def load():
     return lib
 
 
+def load_eval():
+    """Load libdva_eval.so (once), after libdva_b200.so.  Raises if it has not been built."""
+    global _eval_lib
+    if _eval_lib is not None:
+        return _eval_lib
+    if os.path.realpath(LIB_PATH) != os.path.realpath(os.path.join(_HERE, "libdva_b200.so")):
+        # libdva_eval.so would load a second libdva_b200.so, whose error string and launch counter last_error()
+        # and launch_count() do not read
+        raise RuntimeError(f"libdva_eval.so links against {os.path.join(_HERE, 'libdva_b200.so')}; it cannot run "
+                           f"beside the variant DVA_B200_LIB={LIB_PATH}")
+    load()
+    if not os.path.exists(EVAL_LIB_PATH):
+        raise RuntimeError(f"{EVAL_LIB_PATH} not found: build it with `make -C deepviewagg_b200/csrc` "
+                           f"(the same build as libdva_b200.so). deepviewagg_b200 has no CPU fallback.")
+    lib = ctypes.CDLL(EVAL_LIB_PATH)
+    for name, (res, args) in EVAL_SIGNATURES.items():
+        fn = getattr(lib, name)
+        fn.restype = res
+        fn.argtypes = args
+    _eval_lib = lib
+    return lib
+
+
+def entry(name):
+    """The entry point `name`, from whichever library declares it."""
+    return getattr(load_eval() if name in EVAL_SIGNATURES else load(), name)
+
+
 def last_error():
     return load().dva_last_error().decode()
 
@@ -187,7 +231,7 @@ def launch(name, device, *args):
     passed as their device pointer and None as NULL.  `args` holds every tensor, temporaries made in
     the caller's argument list included, until the call returns: a temporary freed before the call
     would hand its block to the next one, and two arguments would alias."""
-    fn = getattr(load(), name)
+    fn = entry(name)
     with torch.cuda.device(device):
         check(fn(*[ptr(a) if isinstance(a, torch.Tensor) else a for a in args], stream_ptr()), name)
 

@@ -51,6 +51,20 @@ class _SparseConvModel(nn.Module):
         y = getattr(data, 'y', None)
         self.labels = (y.to(device) if device is not None else y) if y is not None else None
 
+    # the tracker interface of the reference's BaseModel (metrics/*_tracker.py read these)
+    def get_input(self):
+        return self.input
+
+    def get_output(self):
+        return self.output
+
+    def get_labels(self):
+        return self.labels
+
+    @property
+    def is_multimodal(self):
+        return bool(self._modalities)
+
     def _nll(self, logits, weight=None):
         return ops.csr_nll_loss(logits, self.labels, None, ignore_index=IGNORE_LABEL, weight=weight)
 

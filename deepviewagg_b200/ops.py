@@ -1270,3 +1270,147 @@ def lovasz_softmax(probas, labels, classes="present", ignore=-1, log_probs=False
     class_mult = torch.tensor(mult, dtype=torch.int32, device=probas.device)
     return _LovaszSoftmax.apply(probas.contiguous(), labels.contiguous(), class_mult, classes == "present",
                                 int(ignore), bool(log_probs))
+
+
+# ------------------------------------------------------------------------------------------------
+# segmentation evaluation (libdva_eval.so, include/dva_eval.h): confusion update, vote accumulation,
+# full-resolution nearest-neighbour prediction.  No host read: range errors go to a device status word
+# (int32 [1], bits _lib.DVA_EVAL_BAD_*) that the caller reads when it wants the metrics.
+# ------------------------------------------------------------------------------------------------
+EVAL_MAX_CLASSES = 64
+_NN_MODES = {"interpolate": 0, "interpolate_mean": 1, "own_votes": 2}
+
+
+def eval_status(device):
+    """A fresh device status word for the evaluation operators."""
+    return torch.zeros(1, dtype=torch.int32, device=device)
+
+
+def _eval_classes(K, what):
+    if not 1 <= K <= EVAL_MAX_CLASSES:
+        raise ValueError(f"{what}: {K} classes; the evaluation kernels support 1 to {EVAL_MAX_CLASSES}")
+
+
+def _ignore_args(ignore_label):
+    return (0, 0) if ignore_label is None else (int(ignore_label), 1)
+
+
+def _check_vec(t, n, dtype, what, name):
+    if t.dim() != 1 or t.shape[0] != n or t.dtype != dtype:
+        raise TypeError(f"{what}: {name} must be a [{n}] {dtype} tensor, got {tuple(t.shape)} {t.dtype}")
+
+
+def confusion_update(cm, scores_or_pred, labels, ignore_label=None, counts=None, status=None):
+    """cm += the confusion of (labels, prediction) in place: np.bincount(K * gt + argmax(outputs, 1)) of
+    metrics/segmentation_tracker.py:76-85 without the host copy.
+
+    cm int64 [K, K] (row = ground truth, column = prediction), K <= 64; scores_or_pred either scores [n, K]
+    fp32 / bf16 / fp16, whose argmax is taken in the kernel with numpy's rule (first index of the maximum,
+    the first NaN wins), or int64 predictions [n]; labels int64 [n].  Rows labelled `ignore_label` are
+    skipped, and with counts (int32 [n], scores only) the rows whose count is 0.  A label (or prediction)
+    outside [0, K) is not counted; it sets a bit of `status` (int32 [1]), which is returned."""
+    require_cuda(cm, scores_or_pred, labels, counts, status)
+    if cm.dim() != 2 or cm.shape[0] != cm.shape[1] or cm.dtype != torch.int64 or not cm.is_contiguous():
+        raise TypeError("confusion_update: cm must be a contiguous [K, K] int64 tensor")
+    K = cm.shape[0]
+    _eval_classes(K, "confusion_update")
+    n = scores_or_pred.shape[0]
+    _check_vec(labels, n, torch.int64, "confusion_update", "labels")
+    status = eval_status(cm.device) if status is None else status
+    ign, has_ign = _ignore_args(ignore_label)
+    if scores_or_pred.is_floating_point():
+        if scores_or_pred.dim() != 2 or scores_or_pred.shape[1] != K:
+            raise ValueError(f"confusion_update: scores must be [n, {K}], got {tuple(scores_or_pred.shape)}")
+        if counts is not None:
+            _check_vec(counts, n, torch.int32, "confusion_update", "counts")
+        launch("dva_eval_confusion_scores", cm.device, scores_or_pred.contiguous(), dtype_code(scores_or_pred),
+               labels.contiguous(), None if counts is None else counts.contiguous(), n, K, ign, has_ign, cm, status)
+    else:
+        _check_vec(scores_or_pred, n, torch.int64, "confusion_update", "predictions")
+        if counts is not None:
+            raise ValueError("confusion_update: counts applies to scores, not to predictions")
+        launch("dva_eval_confusion_pred", cm.device, scores_or_pred.contiguous(), labels.contiguous(), n, K, ign,
+               has_ign, cm, status)
+    return status
+
+
+def vote(votes, counts, stamp, ids, outputs, status=None):
+    """votes[ids] += outputs; counts[ids] += 1 in place (metrics/s3dis_tracker.py:76-80).
+
+    votes fp32 [N, K] (K <= 64), counts int32 [N], stamp int32 [N] all -1 (kept by the caller with the
+    table; it is -1 again on return), ids int64 [n], outputs [n, K] fp32 / bf16 / fp16, added in fp32 with one
+    rounding per element (torch's votes + outputs).  A duplicated id takes its last occurrence (torch's
+    index_put_ leaves it undefined); an id outside [0, N) is skipped and sets a bit of `status`, returned."""
+    require_cuda(votes, counts, stamp, ids, outputs, status)
+    if votes.dim() != 2 or votes.dtype != torch.float32 or not votes.is_contiguous():
+        raise TypeError("vote: votes must be a contiguous [N, K] float32 tensor")
+    N, K = votes.shape
+    _eval_classes(K, "vote")
+    for t, name in ((counts, "counts"), (stamp, "stamp")):
+        _check_vec(t, N, torch.int32, "vote", name)
+        if not t.is_contiguous():
+            raise TypeError(f"vote: {name} must be contiguous")
+    n = ids.shape[0]
+    _check_vec(ids, n, torch.int64, "vote", "ids")
+    if outputs.dim() != 2 or tuple(outputs.shape) != (n, K):
+        raise ValueError(f"vote: outputs must be [{n}, {K}], got {tuple(outputs.shape)}")
+    status = eval_status(votes.device) if status is None else status
+    try:
+        launch("dva_eval_vote", votes.device, outputs.contiguous(), dtype_code(outputs), ids.contiguous(), n, N, K,
+               votes, counts, stamp, status)
+    except RuntimeError:
+        stamp.fill_(-1)     # a failed add launch leaves claims behind; a stale claim would drop a later vote
+        raise
+    return status
+
+
+def full_res_predict(votes, counts, pos, labels=None, cm=None, ignore_label=None, mode="interpolate", status=None):
+    """Full-resolution predictions from a vote table: knn_interpolate(votes[voted], pos[voted], pos, k=1)
+    followed by argmax (and the confusion update), fused, without the [N, K] interpolated tensor.
+
+    votes fp32 [N, K], counts int32 [N], pos [N, 3]; voted = the points with counts > 0, in index order.
+    The nearest voted point comes from mapping.knn_query (ties to the lower index); the row is weighted in
+    torch_geometric's fp32 order.  mode:
+      'interpolate'       every point from its nearest voted point (s3dis_tracker.py:94-118);
+      'interpolate_mean'  the same, the voted rows divided by their counts first
+                          (scannet_segmentation_tracker.py:122-135; the table is not modified);
+      'own_votes'         a voted point keeps the argmax of its own votes, the others are interpolated
+                          (kitti360_tracker.py:219-222).
+    With labels (int64 [N]) and cm (int64 [K, K]) also cm += confusion(labels, pred), skipping
+    `ignore_label`.  Returns (pred int64 [N], status)."""
+    from .core.multimodal.mapping import knn_query
+    require_cuda(votes, counts, pos, labels, cm, status)
+    if mode not in _NN_MODES:
+        raise ValueError(f"full_res_predict: mode must be one of {sorted(_NN_MODES)}, got {mode!r}")
+    if votes.dim() != 2 or votes.dtype != torch.float32 or not votes.is_contiguous():
+        raise TypeError("full_res_predict: votes must be a contiguous [N, K] float32 tensor")
+    N, K = votes.shape
+    _eval_classes(K, "full_res_predict")
+    _check_vec(counts, N, torch.int32, "full_res_predict", "counts")
+    if pos.dim() != 2 or tuple(pos.shape) != (N, 3):
+        raise ValueError(f"full_res_predict: pos must be [{N}, 3], got {tuple(pos.shape)}")
+    if (labels is None) != (cm is None):
+        raise ValueError("full_res_predict: labels and cm go together")
+    if labels is not None:
+        _check_vec(labels, N, torch.int64, "full_res_predict", "labels")
+        if tuple(cm.shape) != (K, K) or cm.dtype != torch.int64 or not cm.is_contiguous():
+            raise TypeError(f"full_res_predict: cm must be a contiguous [{K}, {K}] int64 tensor")
+    pos = pos.float().contiguous()
+    counts = counts.contiguous()
+    has = counts > 0
+    voted = torch.nonzero(has).squeeze(1)
+    if voted.numel() == 0:
+        raise ValueError("full_res_predict: no point has a vote (empty search set)")
+    query = torch.arange(N, dtype=torch.int64, device=votes.device)
+    if mode == "own_votes":
+        unvoted = torch.nonzero(~has).squeeze(1)
+        nbr = torch.zeros(N, dtype=torch.int64, device=votes.device)
+        nbr[unvoted] = knn_query(pos[unvoted], pos[voted], 1).squeeze(1)
+    else:
+        nbr = knn_query(pos, pos[voted], 1).squeeze(1)
+    status = eval_status(votes.device) if status is None else status
+    pred = torch.empty(N, dtype=torch.int64, device=votes.device)
+    ign, has_ign = _ignore_args(ignore_label)
+    launch("dva_eval_nn_vote", votes.device, votes, counts, pos, N, K, voted, voted.numel(), query, nbr, N,
+           _NN_MODES[mode], None if labels is None else labels.contiguous(), ign, has_ign, pred, cm, status)
+    return pred, status
