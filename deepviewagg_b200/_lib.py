@@ -1,6 +1,6 @@
-"""ctypes binding of libdva_b200.so (the C ABI declared in include/dva_b200.h) and of libdva_eval.so, the
-evaluation kernels (include/dva_eval.h), which links against the first and shares its error string and launch
-counter.
+"""ctypes binding of libdva_b200.so (the C ABI declared in include/dva_b200.h), of libdva_eval.so, the
+evaluation kernels (include/dva_eval.h), and of libdva_conv2d.so, the image encoder's convolutions
+(include/dva_conv2d.h); the last two link against the first and share its error string and launch counter.
 
 There is NO fallback: if the shared library is missing or a call fails, a RuntimeError is
 raised.  PyTorch is used above this layer only for device memory and streams.
@@ -17,6 +17,7 @@ LIB_PATH = os.environ.get("DVA_B200_LIB") or os.path.join(_HERE, "libdva_b200.so
 CSRC_DIR = os.path.join(_HERE, "csrc")
 # libdva_eval.so loads the libdva_b200.so next to it (rpath $ORIGIN), whatever DVA_B200_LIB names
 EVAL_LIB_PATH = os.path.join(_HERE, "libdva_eval.so")
+CONV_LIB_PATH = os.path.join(_HERE, "libdva_conv2d.so")
 
 DVA_OK, DVA_EINVAL, DVA_EALIGN, DVA_EUNSUPPORTED = 0, -1, -2, -3
 DVA_F32, DVA_BF16, DVA_F16 = 0, 1, 2
@@ -138,8 +139,28 @@ EVAL_SIGNATURES = {
 # status bits of the evaluation kernels (include/dva_eval.h)
 DVA_EVAL_BAD_LABEL, DVA_EVAL_BAD_PRED, DVA_EVAL_BAD_ID = 1, 2, 4
 
+# name -> (restype, argtypes); mirrors include/dva_conv2d.h one to one
+CONV_SIGNATURES = {
+    "dva_conv2d_weight_prep": (_i32, [_vp, _i32, _i32, _i32, _i32, _vp, _vp, _vp]),
+    "dva_conv2d_weight_prep_bwd": (_i32, [_vp, _vp, _i32, _i32, _i32, _vp, _vp]),
+    "dva_conv2d_fwd_workspace_bytes": (_sz, [_i64, _i64, _i64, _i32, _i32]),
+    "dva_conv2d_fwd": (_i32, [_vp, _i64, _i64, _i64, _i32, _vp, _vp, _i32, _i32, _i32, _f32, _vp, _vp, _vp, _vp, _sz,
+                              _vp]),
+    "dva_conv2d_dgrad": (_i32, [_vp, _i64, _i64, _i64, _i32, _i32, _vp, _i32, _vp, _vp, _vp]),
+    "dva_conv2d_wgrad_workspace_bytes": (_sz, [_i64, _i64, _i64, _i32, _i32, _i32]),
+    "dva_conv2d_wgrad": (_i32, [_vp, _vp, _i64, _i64, _i64, _i32, _i32, _i32, _vp, _vp, _vp, _sz, _vp]),
+    "dva_conv2d_gn_apply": (_i32, [_vp, _i64, _i64, _i32, _i32, _vp, _vp, _vp, _vp, _f32, _vp, _vp, _vp, _vp, _vp,
+                                   _vp, _vp, _vp]),
+    "dva_conv2d_gn_bwd_workspace_bytes": (_sz, [_i64, _i64, _i32, _i32]),
+    "dva_conv2d_gn_bwd": (_i32, [_vp, _vp, _i64, _i64, _i32, _i32, _vp, _vp, _vp, _vp, _f32, _vp, _vp, _vp, _vp, _sz,
+                                 _vp]),
+}
+# convolution kinds (include/dva_conv2d.h)
+DVA_CONV_3X3_REFLECT, DVA_CONV_2X2_S2, DVA_CONV_1X1 = 0, 1, 2
+
 _lib = None
 _eval_lib = None
+_conv_lib = None
 
 
 def build(verbose=False):
@@ -174,32 +195,50 @@ def load():
     return lib
 
 
+def _load_linked(path, signatures):
+    """Load a library that links against libdva_b200.so (rpath $ORIGIN), after it.  Raises if it has not been
+    built."""
+    name = os.path.basename(path)
+    if os.path.realpath(LIB_PATH) != os.path.realpath(os.path.join(_HERE, "libdva_b200.so")):
+        # the library would load a second libdva_b200.so, whose error string and launch counter last_error()
+        # and launch_count() do not read
+        raise RuntimeError(f"{name} links against {os.path.join(_HERE, 'libdva_b200.so')}; it cannot run "
+                           f"beside the variant DVA_B200_LIB={LIB_PATH}")
+    load()
+    if not os.path.exists(path):
+        raise RuntimeError(f"{path} not found: build it with `make -C deepviewagg_b200/csrc` "
+                           f"(the same build as libdva_b200.so). deepviewagg_b200 has no CPU fallback.")
+    lib = ctypes.CDLL(path)
+    for fname, (res, args) in signatures.items():
+        fn = getattr(lib, fname)
+        fn.restype = res
+        fn.argtypes = args
+    return lib
+
+
 def load_eval():
     """Load libdva_eval.so (once), after libdva_b200.so.  Raises if it has not been built."""
     global _eval_lib
-    if _eval_lib is not None:
-        return _eval_lib
-    if os.path.realpath(LIB_PATH) != os.path.realpath(os.path.join(_HERE, "libdva_b200.so")):
-        # libdva_eval.so would load a second libdva_b200.so, whose error string and launch counter last_error()
-        # and launch_count() do not read
-        raise RuntimeError(f"libdva_eval.so links against {os.path.join(_HERE, 'libdva_b200.so')}; it cannot run "
-                           f"beside the variant DVA_B200_LIB={LIB_PATH}")
-    load()
-    if not os.path.exists(EVAL_LIB_PATH):
-        raise RuntimeError(f"{EVAL_LIB_PATH} not found: build it with `make -C deepviewagg_b200/csrc` "
-                           f"(the same build as libdva_b200.so). deepviewagg_b200 has no CPU fallback.")
-    lib = ctypes.CDLL(EVAL_LIB_PATH)
-    for name, (res, args) in EVAL_SIGNATURES.items():
-        fn = getattr(lib, name)
-        fn.restype = res
-        fn.argtypes = args
-    _eval_lib = lib
-    return lib
+    if _eval_lib is None:
+        _eval_lib = _load_linked(EVAL_LIB_PATH, EVAL_SIGNATURES)
+    return _eval_lib
+
+
+def load_conv():
+    """Load libdva_conv2d.so (once), after libdva_b200.so.  Raises if it has not been built."""
+    global _conv_lib
+    if _conv_lib is None:
+        _conv_lib = _load_linked(CONV_LIB_PATH, CONV_SIGNATURES)
+    return _conv_lib
 
 
 def entry(name):
     """The entry point `name`, from whichever library declares it."""
-    return getattr(load_eval() if name in EVAL_SIGNATURES else load(), name)
+    if name in EVAL_SIGNATURES:
+        return getattr(load_eval(), name)
+    if name in CONV_SIGNATURES:
+        return getattr(load_conv(), name)
+    return getattr(load(), name)
 
 
 def last_error():

@@ -1414,3 +1414,224 @@ def full_res_predict(votes, counts, pos, labels=None, cm=None, ignore_label=None
     launch("dva_eval_nn_vote", votes.device, votes, counts, pos, N, K, voted, voted.numel(), query, nbr, N,
            _NN_MODES[mode], None if labels is None else labels.contiguous(), ign, has_ign, pred, cm, status)
     return pred, status
+
+
+# --------------------------------------------------------------------------------------------
+# from-scratch image encoder (libdva_conv2d.so, include/dva_conv2d.h): the Conv2dWS -> GroupNorm -> ReLUWS units
+# of ResNetDown and ResBlock (modalities/image.py:39-340), each one autograd node.  Maps are channels-last
+# [B, H, W, C] fp32; products are 3xTF32 on tensor cores, also under autocast (the inputs are cast to fp32).
+# --------------------------------------------------------------------------------------------
+RELU_WS_SCALE = math.sqrt(2 / (1 - 1 / math.pi))   # ReLUWS._SCALE (image.py:119)
+# (kernel_size, stride, padding) -> convolution kind; the only shapes of the shipped configs
+CONV_KINDS = {(3, 1, 1): _lib.DVA_CONV_3X3_REFLECT, (2, 2, 0): _lib.DVA_CONV_2X2_S2, (1, 1, 0): _lib.DVA_CONV_1X1}
+_TAPS = {_lib.DVA_CONV_3X3_REFLECT: 3, _lib.DVA_CONV_2X2_S2: 2, _lib.DVA_CONV_1X1: 1}
+
+
+def conv_out_hw(kind, H, W):
+    """Spatial size of a convolution of `kind`, raising ValueError where torch's reflect pad or conv2d raises."""
+    if kind != _lib.DVA_CONV_1X1 and (H < 2 or W < 2):
+        what = "reflect padding" if kind == _lib.DVA_CONV_3X3_REFLECT else "a 2x2 convolution"
+        raise ValueError(f"{what} needs every spatial side >= 2, got {H}x{W}")
+    return (H // 2, W // 2) if kind == _lib.DVA_CONV_2X2_S2 else (H, W)
+
+
+def _conv_weights(w, kind, standardize):
+    """(wf, wd): the filter the forward reads ([Co][R][S][Ci]) and the one the data gradient reads."""
+    Co, Ci = w.shape[:2]
+    wf = torch.empty(w.numel(), dtype=torch.float32, device=w.device)
+    wd = torch.empty_like(wf)
+    launch("dva_conv2d_weight_prep", w.device, w, Co, Ci, kind, int(standardize), wf, wd)
+    return wf, wd
+
+
+def _weight_grad(w, dwf, kind, standardize):
+    if not standardize:     # 1x1: [Co][1][1][Ci] is the torch layout
+        return dwf.view_as(w)
+    dw = torch.empty_like(w)
+    launch("dva_conv2d_weight_prep_bwd", w.device, w, dwf, w.shape[0], w.shape[1], kind, dw)
+    return dw
+
+
+def _conv_fwd(x, wf, bias, Co, kind, G, eps):
+    B, H, W, Ci = x.shape
+    Ho, Wo = conv_out_hw(kind, H, W)
+    z = torch.empty(B, Ho, Wo, Co, dtype=torch.float32, device=x.device)
+    mean = torch.empty(B, G, dtype=torch.float32, device=x.device)
+    invstd = torch.empty_like(mean)
+    ws = _lib.workspace(_lib.load_conv().dva_conv2d_fwd_workspace_bytes(B, Ho, Wo, Co, G), x.device)
+    launch("dva_conv2d_fwd", x.device, x, B, H, W, Ci, wf, bias, Co, kind, G, float(eps), z, mean, invstd, ws,
+           ws.numel())
+    return z, mean, invstd
+
+
+def _gn_apply(z, gn, relu, skip=None, ds=None):
+    """act(GN(z)) [+ skip] [+ GN_ds(z_ds)]; gn = (G, mean, invstd, gamma, beta), ds = (z_ds, G, mean, ...)."""
+    B, Ho, Wo, C = z.shape
+    G, mean, invstd, gamma, beta = gn
+    zs, _, ms, iss, gs, bs = ds if ds is not None else (None,) * 6
+    y = torch.empty_like(z)
+    launch("dva_conv2d_gn_apply", z.device, z, B, Ho * Wo, C, G, mean, invstd, gamma, beta,
+           RELU_WS_SCALE if relu else 0.0, skip, zs, ms, iss, gs, bs, y)
+    return y
+
+
+def _gn_bwd(dy, z, gn, relu):
+    B, Ho, Wo, C = z.shape
+    G, mean, invstd, gamma, beta = gn
+    dz = torch.empty_like(z)
+    dgamma = torch.empty(C, dtype=torch.float32, device=z.device)
+    dbeta = torch.empty_like(dgamma)
+    ws = _lib.workspace(_lib.load_conv().dva_conv2d_gn_bwd_workspace_bytes(B, Ho * Wo, C, G), z.device)
+    launch("dva_conv2d_gn_bwd", z.device, dy, z, B, Ho * Wo, C, G, mean, invstd, gamma, beta,
+           RELU_WS_SCALE if relu else 0.0, dz, dgamma, dbeta, ws, ws.numel())
+    return dz, dgamma, dbeta
+
+
+def _wgrad(dz, x, kind):
+    B, H, W, Ci = x.shape
+    Co, T = dz.shape[-1], _TAPS[kind]
+    dwf = torch.empty(Co * T * T * Ci, dtype=torch.float32, device=x.device)
+    dbias = torch.empty(Co, dtype=torch.float32, device=x.device)
+    ws = _lib.workspace(_lib.load_conv().dva_conv2d_wgrad_workspace_bytes(B, H, W, Ci, Co, kind), x.device)
+    launch("dva_conv2d_wgrad", x.device, dz, x, B, H, W, Ci, Co, kind, dwf, dbias, ws, ws.numel())
+    return dwf, dbias
+
+
+def _dgrad(dz, x_shape, wd, kind, add=None, out=None):
+    """conv^T(dz) [+ add] into out (a new tensor when None; out may be add)."""
+    B, H, W, Ci = x_shape
+    dx = out if out is not None else torch.empty(B, H, W, Ci, dtype=torch.float32, device=dz.device)
+    launch("dva_conv2d_dgrad", dz.device, dz, B, H, W, Ci, dz.shape[-1], wd, kind, add, dx)
+    return dx
+
+
+def _f32(*ts):
+    return [None if t is None else t.detach().float().contiguous() for t in ts]
+
+
+def _encoder_input(x, weight):
+    """x as the kernels read it: channels-last rows [B, H, W, C_in], fp32, contiguous (a copy for any other dtype
+    or layout; outside autocast custom_fwd casts nothing)."""
+    if x.dim() != 4 or x.shape[3] != weight.shape[1]:
+        raise ValueError(f"expected channels-last rows [B, H, W, {weight.shape[1]}], got shape {tuple(x.shape)}")
+    if not x.is_floating_point():
+        raise TypeError(f"expected a floating-point feature map, got {x.dtype}")
+    return x.float().contiguous()
+
+
+def _as_dtypes(grads, dtypes):
+    """Each gradient in the dtype of its input (the kernels compute in fp32)."""
+    return tuple(None if g is None else g.to(d) for g, d in zip(grads, dtypes))
+
+
+class _ConvGNAct(torch.autograd.Function):
+    """ReLUWS(GroupNorm(Conv2dWS(x))), ResNetDown.conv_in (image.py:302-312), as one node.  Saves x, z and the
+    per-(image, group) statistics."""
+
+    @staticmethod
+    @_fwd_f32
+    def forward(ctx, x, weight, bias, gamma, beta, kind, G, eps):
+        require_cuda(x, weight, bias, gamma, beta)
+        ctx.dtypes = [t.dtype for t in (x, weight, bias, gamma, beta)]
+        x = _encoder_input(x, weight)
+        w, b, g, be = _f32(weight, bias, gamma, beta)
+        wf, wd = _conv_weights(w, kind, True)
+        z, mean, invstd = _conv_fwd(x, wf, b, w.shape[0], kind, G, eps)
+        ctx.save_for_backward(x, w, wd, g, be, z, mean, invstd)
+        ctx.cfg = (kind, G)
+        return _gn_apply(z, (G, mean, invstd, g, be), True)
+
+    @staticmethod
+    @_bwd
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, dy):
+        x, w, wd, g, be, z, mean, invstd = ctx.saved_tensors
+        kind, G = ctx.cfg
+        dz, dg, dbe = _gn_bwd(dy.float().contiguous(), z, (G, mean, invstd, g, be), True)
+        dwf, db = _wgrad(dz, x, kind)
+        dx = _dgrad(dz, x.shape, wd, kind) if ctx.needs_input_grad[0] else None
+        return (*_as_dtypes((dx, _weight_grad(w, dwf, kind, True), db, dg, dbe), ctx.dtypes), None, None, None)
+
+
+class _ResBlock(torch.autograd.Function):
+    """ResBlock (image.py:128-189) as one node: h = ReLUWS(GN1(conv1(x))), y = ReLUWS(GN2(conv2(h))) + skip, skip =
+    x or GN_ds(conv1x1(x)), the residual added after the second activation.  Saves x, z1, z2, z_ds and the
+    statistics; h is recomputed in the backward."""
+
+    @staticmethod
+    @_fwd_f32
+    def forward(ctx, x, w1, b1, g1, be1, w2, b2, g2, be2, wd, bd, gd, bed, cfg):
+        require_cuda(x, w1, b1, g1, be1, w2, b2, g2, be2, wd, bd, gd, bed)
+        (G1, eps1), (G2, eps2), (Gd, epsd) = cfg
+        ctx.dtypes = [None if t is None else t.dtype for t in (x, w1, b1, g1, be1, w2, b2, g2, be2, wd, bd, gd, bed)]
+        x = _encoder_input(x, w1)
+        w1, b1, g1, be1, w2, b2, g2, be2, wd, bd, gd, bed = _f32(w1, b1, g1, be1, w2, b2, g2, be2, wd, bd, gd, bed)
+        k3 = _lib.DVA_CONV_3X3_REFLECT
+        wf1, wd1 = _conv_weights(w1, k3, True)
+        z1, m1, i1 = _conv_fwd(x, wf1, b1, w1.shape[0], k3, G1, eps1)
+        h = _gn_apply(z1, (G1, m1, i1, g1, be1), True)
+        wf2, wd2 = _conv_weights(w2, k3, True)
+        z2, m2, i2 = _conv_fwd(h, wf2, b2, w2.shape[0], k3, G2, eps2)
+        del h
+        ds = None
+        wdd = zd = md = idd = None
+        if wd is not None:
+            wfd, wdd = _conv_weights(wd, _lib.DVA_CONV_1X1, False)
+            zd, md, idd = _conv_fwd(x, wfd, bd, wd.shape[0], _lib.DVA_CONV_1X1, Gd, epsd)
+            ds = (zd, Gd, md, idd, gd, bed)
+        y = _gn_apply(z2, (G2, m2, i2, g2, be2), True, skip=x if ds is None else None, ds=ds)
+        ctx.save_for_backward(x, w1, wd1, g1, be1, z1, m1, i1, w2, wd2, g2, be2, z2, m2, i2, wd, wdd, gd, bed, zd,
+                              md, idd)
+        ctx.cfg = cfg
+        return y
+
+    @staticmethod
+    @_bwd
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, dy):
+        (x, w1, wd1, g1, be1, z1, m1, i1, w2, wd2, g2, be2, z2, m2, i2, wd, wdd, gd, bed, zd, md,
+         idd) = ctx.saved_tensors
+        (G1, _), (G2, _), (Gd, _) = ctx.cfg
+        k3, k1 = _lib.DVA_CONV_3X3_REFLECT, _lib.DVA_CONV_1X1
+        dy = dy.float().contiguous()
+        gn1, gn2 = (G1, m1, i1, g1, be1), (G2, m2, i2, g2, be2)
+        dz2, dg2, dbe2 = _gn_bwd(dy, z2, gn2, True)
+        h = _gn_apply(z1, gn1, True)
+        dwf2, db2 = _wgrad(dz2, h, k3)
+        dh = _dgrad(dz2, h.shape, wd2, k3)
+        del h
+        dz1, dg1, dbe1 = _gn_bwd(dh, z1, gn1, True)
+        del dh
+        dwf1, db1 = _wgrad(dz1, x, k3)
+        grads_ds = (None,) * 4
+        dx = None
+        if wd is not None:
+            dzd, dgd, dbed = _gn_bwd(dy, zd, (Gd, md, idd, gd, bed), False)
+            dwfd, dbd = _wgrad(dzd, x, k1)
+            grads_ds = (_weight_grad(wd, dwfd, k1, False), dbd, dgd, dbed)
+            if ctx.needs_input_grad[0]:
+                dx = _dgrad(dzd, x.shape, wdd, k1)
+        if ctx.needs_input_grad[0]:
+            dx = _dgrad(dz1, x.shape, wd1, k3, add=dy if dx is None else dx, out=dx)
+        grads = (dx, _weight_grad(w1, dwf1, k3, True), db1, dg1, dbe1, _weight_grad(w2, dwf2, k3, True), db2, dg2,
+                 dbe2, *grads_ds)
+        return (*_as_dtypes(grads, ctx.dtypes), None)
+
+
+def conv_gn_relu_ws(x, conv, norm, kind):
+    """ReLUWS(norm(conv(x))) for channels-last x [B, H, W, C_in] (conv a Conv2dWS, norm an nn.GroupNorm): fp32
+    [B, H', W', C_out], computed from fp32 operands whatever the dtype and layout of x."""
+    return _ConvGNAct.apply(x, conv.weight, conv.bias, norm.weight, norm.bias, kind, norm.num_groups, norm.eps)
+
+
+def res_block(x, block):
+    """A ResBlock on channels-last x [B, H, W, C_in]: fp32 [B, H, W, C_out], computed from fp32 operands whatever the
+    dtype and layout of x."""
+    c1, n1, _, c2, n2, _ = block.block
+    ds = block.downsample
+    cd, nd = (ds[0], ds[1]) if ds is not None else (None, None)
+    cfg = ((n1.num_groups, n1.eps), (n2.num_groups, n2.eps),
+           (nd.num_groups, nd.eps) if nd is not None else (1, 1e-5))
+    return _ResBlock.apply(x, c1.weight, c1.bias, n1.weight, n1.bias, c2.weight, c2.bias, n2.weight, n2.bias,
+                           cd.weight if cd is not None else None, cd.bias if cd is not None else None,
+                           nd.weight if nd is not None else None, nd.bias if nd is not None else None, cfg)
