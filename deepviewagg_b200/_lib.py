@@ -1,6 +1,7 @@
 """ctypes binding of libdva_b200.so (the C ABI declared in include/dva_b200.h), of libdva_eval.so, the
-evaluation kernels (include/dva_eval.h), and of libdva_conv2d.so, the image encoder's convolutions
-(include/dva_conv2d.h); the last two link against the first and share its error string and launch counter.
+evaluation kernels (include/dva_eval.h), of libdva_conv2d.so, the image encoder's convolutions
+(include/dva_conv2d.h), and of libdva_unet.so, the image decoder's transposed convolutions (include/dva_unet.h); the
+last three link against the first and share its error string and launch counter.
 
 There is NO fallback: if the shared library is missing or a call fails, a RuntimeError is
 raised.  PyTorch is used above this layer only for device memory and streams.
@@ -18,6 +19,7 @@ CSRC_DIR = os.path.join(_HERE, "csrc")
 # libdva_eval.so loads the libdva_b200.so next to it (rpath $ORIGIN), whatever DVA_B200_LIB names
 EVAL_LIB_PATH = os.path.join(_HERE, "libdva_eval.so")
 CONV_LIB_PATH = os.path.join(_HERE, "libdva_conv2d.so")
+UNET_LIB_PATH = os.path.join(_HERE, "libdva_unet.so")
 
 DVA_OK, DVA_EINVAL, DVA_EALIGN, DVA_EUNSUPPORTED = 0, -1, -2, -3
 DVA_F32, DVA_BF16, DVA_F16 = 0, 1, 2
@@ -158,9 +160,26 @@ CONV_SIGNATURES = {
 # convolution kinds (include/dva_conv2d.h)
 DVA_CONV_3X3_REFLECT, DVA_CONV_2X2_S2, DVA_CONV_1X1 = 0, 1, 2
 
+# name -> (restype, argtypes); mirrors include/dva_unet.h one to one
+UNET_SIGNATURES = {
+    "dva_unet_weight_prep": (_i32, [_vp, _i32, _i32, _i32, _vp, _vp, _vp]),
+    "dva_unet_weight_prep_bwd": (_i32, [_vp, _vp, _i32, _i32, _i32, _vp, _vp]),
+    "dva_unet_fwd_workspace_bytes": (_sz, [_i64, _i64, _i64, _i32, _i32, _i32]),
+    "dva_unet_fwd": (_i32, [_vp, _i64, _i64, _i64, _i32, _vp, _vp, _i32, _i32, _i32, _f32, _vp, _vp, _vp, _vp, _sz,
+                            _vp]),
+    "dva_unet_dgrad": (_i32, [_vp, _i64, _i64, _i64, _i32, _i32, _vp, _i32, _vp, _vp, _vp]),
+    "dva_unet_wgrad_workspace_bytes": (_sz, [_i64, _i64, _i64, _i32, _i32, _i32]),
+    "dva_unet_wgrad": (_i32, [_vp, _vp, _i64, _i64, _i64, _i32, _i32, _i32, _vp, _vp, _vp, _sz, _vp]),
+    "dva_unet_act": (_i32, [_vp, _i64, _f32, _vp, _vp]),
+    "dva_unet_act_bwd": (_i32, [_vp, _vp, _i64, _f32, _vp, _vp]),
+}
+# transposed convolution kinds (include/dva_unet.h)
+DVA_UNET_UP_2X2, DVA_UNET_T_3X3 = 0, 1
+
 _lib = None
 _eval_lib = None
 _conv_lib = None
+_unet_lib = None
 
 
 def build(verbose=False):
@@ -232,8 +251,18 @@ def load_conv():
     return _conv_lib
 
 
+def load_unet():
+    """Load libdva_unet.so (once), after libdva_b200.so.  Raises if it has not been built."""
+    global _unet_lib
+    if _unet_lib is None:
+        _unet_lib = _load_linked(UNET_LIB_PATH, UNET_SIGNATURES)
+    return _unet_lib
+
+
 def entry(name):
     """The entry point `name`, from whichever library declares it."""
+    if name in UNET_SIGNATURES:
+        return getattr(load_unet(), name)
     if name in EVAL_SIGNATURES:
         return getattr(load_eval(), name)
     if name in CONV_SIGNATURES:

@@ -1,6 +1,7 @@
-"""The from-scratch image encoder of the reference (torch_points3d/modules/multimodal/modalities/image.py:26-340):
-ResNetDown built from ResBlock, Conv2dWS, GroupNorm and ReLUWS, with the reference's names, constructor arguments
-and module tree, so a reference state_dict loads with strict=True.
+"""The from-scratch image network of the reference (torch_points3d/modules/multimodal/modalities/image.py:26-627):
+the encoder ResNetDown built from ResBlock, Conv2dWS, GroupNorm and ReLUWS, and the decoder (ResNetUp,
+ConvTranspose2dWS, UnaryConv, Dropout2d, PersistentDropout2d) that UNet joins to it, with the reference's names,
+constructor arguments and module tree, so a reference state_dict loads with strict=True.
 
 ResNetDown.forward and ResBlock.forward run on the sm_90a kernels of libdva_conv2d.so (ops.conv_gn_relu_ws,
 ops.res_block): each Conv2dWS -> GroupNorm -> ReLUWS unit, and each ResBlock, is one autograd node; Conv2dWS,
@@ -12,11 +13,16 @@ autocast).
 Supported: block='ResBlock', normalization='GroupNorm', weight_standardization=True, padding_mode='reflect',
 dilation=1, and (kernel_size, stride, padding) of conv_in in {(3, 1, 1), (2, 2, 0)} -- every layer of the shipped
 GroupNorm configs.  Anything else raises NotImplementedError naming the argument.
+
+The decoder runs on the transposed convolutions of libdva_unet.so (ops.convt_gn_relu_ws, ops.res_block_t) with the
+same rules; ResNetUp takes padding_mode='zeros' and (kernel_size, stride, padding) in {(2, 2, 0), (3, 1, 1)}, and
+UnaryConv normalization=None.  UNet(opt) builds the network from the compact config format of the reference.
 """
 from math import pi, sqrt
 
 import torch
 import torch.nn as nn
+import torch.nn.functional as F
 
 from .... import ops
 from ...._lib import require_cuda
@@ -105,21 +111,41 @@ def _out_dtype(x):
     return torch.float32 if torch.is_autocast_enabled("cuda") else x.dtype
 
 
+class ConvTranspose2dWS(nn.ConvTranspose2d):
+    """Parameters of a weight-standardised transposed convolution (image.py:76-107); the weight is [C_in, C_out, R,
+    S] and is standardised per input channel.  It runs inside ResNetUp / ResBlock."""
+
+    def __init__(self, in_channels, out_channels, kernel_size, stride=1, padding=0, output_padding=0, dilation=1,
+                 groups=1, bias=True, padding_mode='zeros', scaled=True):
+        super().__init__(in_channels, out_channels, kernel_size, stride=stride, padding=padding,
+                         output_padding=output_padding, dilation=dilation, groups=groups, bias=bias,
+                         padding_mode=padding_mode)
+        self.scaled = scaled
+
+    def forward(self, x, *args, output_size=None, **kwargs):
+        raise NotImplementedError("ConvTranspose2dWS runs fused with its GroupNorm and ReLUWS: call the ResNetUp or "
+                                  "ResBlock that holds it")
+
+
 class ResBlock(nn.Module):
     """Basic ResNet block (image.py:128-189): conv3x3-GN-ReLUWS-conv3x3-GN-ReLUWS, plus the block input or a 1x1
-    nn.Conv2d + GN downsample when the widths differ, added after the second activation."""
+    nn.Conv2d + GN downsample when the widths differ, added after the second activation.  The convolutions are
+    Conv2dWS with reflect padding (the encoder) or ConvTranspose2dWS with zero padding (the decoder)."""
 
     def __init__(self, input_nc, output_nc, convolution, normalization, activation):
         super().__init__()
-        if convolution is not Conv2dWS:
-            raise NotImplementedError(f"convolution={getattr(convolution, '__name__', convolution)}: only Conv2dWS")
+        if convolution is not Conv2dWS and convolution is not ConvTranspose2dWS:
+            raise NotImplementedError(f"convolution={getattr(convolution, '__name__', convolution)}: only Conv2dWS "
+                                      f"and ConvTranspose2dWS")
         if activation is not ReLUWS:
             raise NotImplementedError(f"activation={getattr(activation, '__name__', activation)}: only ReLUWS")
+        self._transposed = convolution is ConvTranspose2dWS
+        padding_mode = 'zeros' if self._transposed else 'reflect'
         self.block = (
-            Seq().append(convolution(input_nc, output_nc, kernel_size=3, stride=1, padding=1, padding_mode='reflect'))
+            Seq().append(convolution(input_nc, output_nc, kernel_size=3, stride=1, padding=1, padding_mode=padding_mode))
             .append(normalization(output_nc))
             .append(activation())
-            .append(convolution(output_nc, output_nc, kernel_size=3, stride=1, padding=1, padding_mode='reflect'))
+            .append(convolution(output_nc, output_nc, kernel_size=3, stride=1, padding=1, padding_mode=padding_mode))
             .append(normalization(output_nc))
             .append(activation()))
         if not isinstance(self.block[1], nn.GroupNorm):
@@ -133,6 +159,8 @@ class ResBlock(nn.Module):
 
     def forward_rows(self, x):
         """The block on channels-last rows [B, H, W, C_in] -> [B, H, W, C_out]."""
+        if self._transposed:
+            return ops.res_block_t(x, self)
         ops.conv_out_hw(ops.CONV_KINDS[(3, 1, 1)], x.shape[1], x.shape[2])
         return ops.res_block(x, self)
 
@@ -226,4 +254,308 @@ class ResNetDown(nn.Module):
         if self.blocks is not None:
             for blk in self.blocks:
                 h = ops.res_block(h, blk)
+        return h.to(_out_dtype(x)).permute(0, 3, 1, 2)
+
+
+class ResNetUp(ResNetDown):
+    """in -- strided transposed conv -- [concatenate skip] -- N x ResBlock (image.py:343-405), the decoder stage, on
+    the sm_90a kernels of libdva_unet.so.  skip_first=True concatenates the skip before the strided convolution."""
+
+    CONVOLUTION = "ConvTranspose2d"
+
+    def __init__(self, up_conv_nn=[], kernel_size=2, dilation=1, stride=2, N=1, padding=0, padding_mode='zeros',
+                 normalization='BatchNorm2d', weight_standardization=False, skip_first=False, block="ResBlock",
+                 **kwargs):
+        nn.Module.__init__(self)
+        self.skip_first = skip_first
+        if len(up_conv_nn) < 2 or any([x < 0 for x in up_conv_nn]):
+            self.conv_in = None
+            self.blocks = None
+            return
+        if block != "ResBlock":
+            raise NotImplementedError(f"block={block!r}: only 'ResBlock' is supported")
+        if normalization != "GroupNorm":
+            raise NotImplementedError(f"normalization={normalization!r}: only 'GroupNorm' is supported")
+        if not weight_standardization:
+            raise NotImplementedError("weight_standardization=False: only weight-standardised convolutions are "
+                                      "supported")
+        if padding_mode != "zeros":
+            raise NotImplementedError(f"padding_mode={padding_mode!r}: only 'zeros' is supported")
+        if _single(dilation, "dilation") != 1:
+            raise NotImplementedError(f"dilation={dilation}: only 1 is supported")
+        shape = (_single(kernel_size, "kernel_size"), _single(stride, "stride"), _single(padding, "padding"))
+        if shape not in ops.CONVT_KINDS:
+            raise NotImplementedError(f"(kernel_size, stride, padding)={shape}: only (2, 2, 0) and (3, 1, 1) are "
+                                      f"supported")
+        if N < 0:
+            raise NotImplementedError(f"N={N}: only N >= 0 is supported")
+        self._kind = ops.CONVT_KINDS[shape]
+
+        nc_in, nc_stride_out, nc_block_in, nc_out = self._parse_conv_nn(up_conv_nn, stride, N)
+        self.conv_in = (
+            Seq().append(ConvTranspose2dWS(in_channels=nc_in, out_channels=nc_stride_out, kernel_size=kernel_size,
+                                           stride=stride, dilation=dilation, padding=padding,
+                                           padding_mode=padding_mode))
+            .append(_group_norm(nc_stride_out))
+            .append(ReLUWS()))
+        if N > 0:
+            self.blocks = Seq()
+            for _ in range(N):
+                self.blocks.append(ResBlock(nc_block_in, nc_out, ConvTranspose2dWS, _group_norm, ReLUWS))
+                nc_block_in = nc_out
+        else:
+            self.blocks = None
+
+    def _parse_conv_nn(self, up_conv_nn, stride, N):
+        if _is_list(up_conv_nn[0]):
+            up_conv_nn = up_conv_nn[0]
+        expected = 2 if self.skip_first else 3
+        assert len(up_conv_nn) == expected, \
+            f"ResNetUp with skip_first={self.skip_first} expects up_conv_nn to have length of {expected} but got " \
+            f"len(up_conv_nn)={len(up_conv_nn)}."
+        if self.skip_first:
+            nc_in, nc_out = up_conv_nn
+            nc_skip_in = 0
+        else:
+            nc_in, nc_skip_in, nc_out = up_conv_nn
+        nc_stride_out = nc_in if _single(stride, "stride") > 1 and N > 0 else nc_out
+        nc_block_in = nc_stride_out if self.skip_first else nc_stride_out + nc_skip_in
+        return nc_in, nc_stride_out, nc_block_in, nc_out
+
+    def output_hw(self, H, W):
+        """Spatial size of the output for an H x W input."""
+        if self.conv_in is None:
+            return H, W
+        return ops.convt_out_hw(self._kind, H, W)
+
+    def _skip_hw(self, H, W, skip_hw, where="ResNetUp"):
+        """The size the skip connection must have: the input's (skip_first) or the upsampled map's."""
+        hw = (H, W) if self.skip_first or self.conv_in is None else self.output_hw(H, W)
+        if skip_hw is not None and tuple(skip_hw) != tuple(hw):
+            raise ValueError(f"{where}: the skip connection is {skip_hw[0]}x{skip_hw[1]} but the map it joins is "
+                             f"{hw[0]}x{hw[1]}; the image sides must be multiples of 2 ** (number of strided "
+                             f"stages)")
+
+    def forward_rows(self, x, skip):
+        """The stage on channels-last rows: x [B, H, W, C_in], skip [B, H', W', C_skip] or None."""
+        self._skip_hw(x.shape[1], x.shape[2], None if skip is None else skip.shape[1:3])
+        if self.skip_first and skip is not None:
+            x = torch.cat((x.float(), skip.float()), dim=3)
+        if self.conv_in is not None:
+            conv, norm, _ = self.conv_in
+            x = ops.convt_gn_relu_ws(x, conv, norm, self._kind)
+        if not self.skip_first and skip is not None:
+            x = torch.cat((x.float(), skip.float()), dim=3)
+        if self.blocks is not None:
+            for blk in self.blocks:
+                x = ops.res_block_t(x, blk)
+        return x
+
+    def forward(self, x, skip, *args, **kwargs):
+        h = _rows(x)
+        return self.forward_rows(h, None if skip is None else _rows(skip)).to(_out_dtype(x)).permute(0, 3, 1, 2)
+
+    def extra_repr(self) -> str:
+        return f"skip_first={self.skip_first}"
+
+
+class Dropout2d(nn.Dropout2d):
+    """Dropout2d with kwargs support (image.py:479-482): F.dropout2d, one Bernoulli draw per (image, channel)."""
+
+    def forward(self, input, *args, **kwargs):
+        return super().forward(input)
+
+    def draw_mask(self, x, reset=True):
+        """The [B, C, 1, 1] mask F.dropout2d draws for x [B, C, H, W] (the same torch RNG calls), or None when it is
+        the identity."""
+        if not self.training or not self.p:
+            return None
+        return x.new_empty(x.shape[0], x.shape[1], 1, 1).bernoulli_(1 - self.p).div_(1 - self.p)
+
+
+class PersistentDropout2d(nn.Module):
+    """Dropout2d whose [1, C, 1, 1] mask is kept across calls until reset (image.py:485-525); the identity, and no
+    mask, in eval mode."""
+
+    def __init__(self, input_nc, p=0.5):
+        self.input_nc = input_nc
+        self.p = p
+        self.mask = None
+        super().__init__()
+
+    def draw_mask(self, x, reset=True):
+        if not self.training or not self.p:
+            self.mask = None
+            return None
+        if self.mask is None or reset:
+            mask = x.new_empty(1, self.input_nc, 1, 1, requires_grad=False)
+            mask = mask.bernoulli_(1 - self.p)
+            self.mask = mask.div_(1 - self.p)
+        return self.mask
+
+    def forward(self, x, reset, *args, **kwargs):
+        mask = self.draw_mask(x, reset)
+        return x if mask is None else x * mask.expand_as(x)
+
+    def extra_repr(self) -> str:
+        return f"input_nc={self.input_nc}, p={self.p}"
+
+
+class UnaryConv(nn.Module):
+    """Dropout -- 1x1 convolution -- activation -- dropout on images (image.py:408-476), the last convolution of
+    UNet.  The 1x1 runs on libdva_conv2d.so (weight-standardised or not); the dropout masks multiply the channels-last
+    rows.  normalization must be None (the reference's own norm path cannot run: it calls the normalization class
+    on the tensor)."""
+
+    def __init__(self, input_nc, output_nc, normalization=None, activation=None, weight_standardization=False,
+                 in_drop=0, out_drop=0, persistent_drop=False):
+        super().__init__()
+        if normalization is not None:
+            raise NotImplementedError(f"normalization={normalization!r}: only None is supported")
+        if activation not in (None, "ReLU"):
+            raise NotImplementedError(f"activation={activation!r}: only None and 'ReLU' are supported")
+        if in_drop is None or in_drop <= 0:
+            self.input_dropout = None
+        elif persistent_drop:
+            self.input_dropout = PersistentDropout2d(input_nc, p=in_drop)
+        else:
+            self.input_dropout = Dropout2d(p=in_drop, inplace=True)
+        self.norm = None
+        if weight_standardization:
+            self.conv = Conv2dWS(input_nc, output_nc, stride=1, kernel_size=1)
+            self.activation = ReLUWS if activation is not None else None
+        else:
+            self.conv = nn.Conv2d(input_nc, output_nc, stride=1, kernel_size=1)
+            self.activation = nn.ReLU if activation is not None else None
+        self._standardize = bool(weight_standardization)
+        if out_drop is None or out_drop <= 0:
+            self.output_dropout = None
+        elif persistent_drop:
+            self.output_dropout = PersistentDropout2d(output_nc, p=out_drop)
+        else:
+            self.output_dropout = Dropout2d(p=out_drop, inplace=True)
+
+    @staticmethod
+    def _drop(h, dropout, reset):
+        """h [B, H, W, C] times the mask of `dropout` (drawn for the NCHW view of h), or h."""
+        if dropout is None:
+            return h
+        mask = dropout.draw_mask(h.permute(0, 3, 1, 2), reset)
+        return h if mask is None else h * mask.reshape(mask.shape[0], 1, 1, mask.shape[1])
+
+    def forward_rows(self, h, reset=True):
+        h = self._drop(h, self.input_dropout, reset)
+        scale = 0.0 if self.activation is None else (ReLUWS._SCALE if self.activation is ReLUWS else 1.0)
+        h = ops.unary_conv(h, self.conv, self._standardize, scale)
+        return self._drop(h, self.output_dropout, reset)
+
+    def forward(self, x, *args, **kwargs):
+        reset = kwargs.get("reset", args[0] if args else True)
+        return self.forward_rows(_rows(x), bool(reset)).to(_out_dtype(x)).permute(0, 3, 1, 2)
+
+
+SPECIAL_NAMES = ["block_names"]
+
+
+def fetch_arguments_from_list(opt, index, special_names):
+    """The arguments of layer `index` from a compact config (torch_points3d/utils/config.py:78-103): a list-valued
+    key gives its index-th entry under the key without a trailing 's' (except special_names), a string entry is
+    eval'ed where it parses (config arithmetic), and any other key is passed as it is."""
+    args = {}
+    for o, v in opt.items():
+        name = str(o)
+        if _is_list(v) and len(v) > 0:
+            if name[-1] == "s" and name not in special_names:
+                name = name[:-1]
+            v_index = v[index]
+            if _is_list(v_index):
+                v_index = list(v_index)
+            try:
+                v_index = eval(v_index)
+            except Exception:
+                pass
+            args[name] = v_index
+        else:
+            if _is_list(v):
+                v = list(v)
+            args[name] = v
+    return args
+
+
+def _opt(opt, key):
+    """opt[key] for an omegaconf DictConfig, a dict or an attribute dict; None when absent."""
+    if hasattr(opt, "get"):
+        return opt.get(key)
+    return getattr(opt, key, None)
+
+
+class UNet(nn.Module):
+    """The image UNet of the reference (image.py:531-627): ResNetDown stages, ResNetUp stages joined by symmetric
+    skip connections, and an optional UnaryConv, built from the compact config format (down_conv.down_conv_nn,
+    up_conv.up_conv_nn, optional last_conv).  Input [B, C, H, W] on CUDA; output [B, C', H', W'] with channels-last
+    strides in the input's dtype (fp32 under autocast).  Called as conv(x, reset): reset (default True) draws a new
+    persistent dropout mask in last_conv."""
+
+    def __init__(self, opt):
+        super().__init__()
+        down, up = _opt(opt, "down_conv"), _opt(opt, "up_conv")
+        if down is None or up is None or _is_list(down) or "down_conv_nn" not in down or _is_list(up) \
+                or "up_conv_nn" not in up:
+            raise NotImplementedError("UNet: only the compact format (down_conv.down_conv_nn and up_conv.up_conv_nn) "
+                                      "is supported")
+        self._init_from_compact_format(opt)
+
+    def _init_from_compact_format(self, opt):
+        down, up = _opt(opt, "down_conv"), _opt(opt, "up_conv")
+        self.down_modules = nn.ModuleList()
+        for i in range(len(down["down_conv_nn"])):
+            self.down_modules.append(self._build_module(down, i, "DOWN"))
+        if _opt(opt, "innermost") is not None:
+            raise NotImplementedError("innermost: the BottleneckBlock inner module is not supported")
+        self.inner_modules = None
+        self.up_modules = nn.ModuleList()
+        for i in range(len(up["up_conv_nn"])):
+            self.up_modules.append(self._build_module(up, i, "UP"))
+        last = _opt(opt, "last_conv")
+        self.last = self._build_module(last, 0, "LAST") if last is not None else None
+
+    def _build_module(self, opt, index, flow):
+        module_cls = {"down": ResNetDown, "up": ResNetUp, "last": UnaryConv}.get(flow.lower())
+        if module_cls is None:
+            raise NotImplementedError(f"flow={flow!r}")
+        return module_cls(**fetch_arguments_from_list(opt, index, SPECIAL_NAMES))
+
+    def check_sizes(self, H, W):
+        """The spatial size of the output for an H x W input; ValueError, naming the stage and both shapes, where a
+        skip connection would not match the map it joins (the sides are not multiples of 2 ** strided stages)."""
+        sizes = []
+        for m in self.down_modules:
+            H, W = m.output_hw(H, W)
+            sizes.append((H, W))
+        stack = sizes[:-1]
+        if self.up_modules[0].skip_first:
+            stack.append(None)
+        for i, m in enumerate(self.up_modules):
+            skip = stack.pop(-1) if stack else None
+            m._skip_hw(H, W, skip, where=f"UNet up stage {i}")
+            H, W = m.output_hw(H, W)
+        return H, W
+
+    def forward(self, x, *args, **kwargs):
+        reset = kwargs.get("reset", args[0] if args else True)
+        self.check_sizes(x.shape[2], x.shape[3])
+        h = x.float() if x.is_floating_point() else x
+        stack = []
+        for m in self.down_modules[:-1]:
+            h = m(h)
+            stack.append(h)
+        h = self.down_modules[-1](h)
+        if self.up_modules[0].skip_first:
+            stack.append(None)
+        h = _rows(h)
+        for m in self.up_modules:
+            skip = stack.pop(-1) if stack else None
+            h = m.forward_rows(h, None if skip is None else _rows(skip))
+        if self.last is not None:
+            h = self.last.forward_rows(h, bool(reset))
         return h.to(_out_dtype(x)).permute(0, 3, 1, 2)

@@ -1635,3 +1635,233 @@ def res_block(x, block):
     return _ResBlock.apply(x, c1.weight, c1.bias, n1.weight, n1.bias, c2.weight, c2.bias, n2.weight, n2.bias,
                            cd.weight if cd is not None else None, cd.bias if cd is not None else None,
                            nd.weight if nd is not None else None, nd.bias if nd is not None else None, cfg)
+
+
+# --------------------------------------------------------------------------------------------
+# from-scratch image decoder (libdva_unet.so, include/dva_unet.h): the ConvTranspose2dWS -> GroupNorm -> ReLUWS
+# units of ResNetUp and the transposed ResBlocks (modalities/image.py), each one autograd node, and UnaryConv's 1x1
+# convolution.  GroupNorm, ReLUWS, the residual and the 1x1 convolutions run on libdva_conv2d.so.  Same rules as
+# the encoder: channels-last [B, H, W, C] fp32 maps, 3xTF32 products, inputs cast to fp32 under autocast, gradients
+# in each input's dtype.
+# --------------------------------------------------------------------------------------------
+# (kernel_size, stride, padding) of a zero-padded ConvTranspose2d -> kind; the only shapes of the shipped configs
+CONVT_KINDS = {(2, 2, 0): _lib.DVA_UNET_UP_2X2, (3, 1, 1): _lib.DVA_UNET_T_3X3}
+
+
+def convt_out_hw(kind, H, W):
+    """Spatial size of a transposed convolution of `kind` (output_padding 0)."""
+    if H < 1 or W < 1:
+        raise ValueError(f"a transposed convolution needs a non-empty map, got {H}x{W}")
+    return (2 * H, 2 * W) if kind == _lib.DVA_UNET_UP_2X2 else (H, W)
+
+
+def _convt_weights(w, kind):
+    """(wf, wd): the standardised filter as the forward reads it and as the data gradient reads it."""
+    Ci, Co = w.shape[:2]
+    wf = torch.empty(w.numel(), dtype=torch.float32, device=w.device)
+    wd = torch.empty_like(wf)
+    launch("dva_unet_weight_prep", w.device, w, Ci, Co, kind, wf, wd)
+    return wf, wd
+
+
+def _convt_weight_grad(w, dwf, kind):
+    dw = torch.empty_like(w)
+    launch("dva_unet_weight_prep_bwd", w.device, w, dwf, w.shape[0], w.shape[1], kind, dw)
+    return dw
+
+
+def _convt_fwd(x, wf, bias, Co, kind, G, eps):
+    B, H, W, Ci = x.shape
+    Ho, Wo = convt_out_hw(kind, H, W)
+    z = torch.empty(B, Ho, Wo, Co, dtype=torch.float32, device=x.device)
+    mean = torch.empty(B, G, dtype=torch.float32, device=x.device)
+    invstd = torch.empty_like(mean)
+    ws = _lib.workspace(_lib.load_unet().dva_unet_fwd_workspace_bytes(B, H, W, Co, G, kind), x.device)
+    launch("dva_unet_fwd", x.device, x, B, H, W, Ci, wf, bias, Co, kind, G, float(eps), z, mean, invstd, ws,
+           ws.numel())
+    return z, mean, invstd
+
+
+def _convt_wgrad(dz, x, kind):
+    B, H, W, Ci = x.shape
+    Co = dz.shape[-1]
+    dwf = torch.empty(Ci * Co * (4 if kind == _lib.DVA_UNET_UP_2X2 else 9), dtype=torch.float32, device=x.device)
+    dbias = torch.empty(Co, dtype=torch.float32, device=x.device)
+    ws = _lib.workspace(_lib.load_unet().dva_unet_wgrad_workspace_bytes(B, H, W, Ci, Co, kind), x.device)
+    launch("dva_unet_wgrad", x.device, dz, x, B, H, W, Ci, Co, kind, dwf, dbias, ws, ws.numel())
+    return dwf, dbias
+
+
+def _convt_dgrad(dz, x_shape, wd, kind, add=None, out=None):
+    """The data gradient of the transposed convolution [+ add] into out (a new tensor when None; out may be add)."""
+    B, H, W, Ci = x_shape
+    dx = out if out is not None else torch.empty(B, H, W, Ci, dtype=torch.float32, device=dz.device)
+    launch("dva_unet_dgrad", dz.device, dz, B, H, W, Ci, dz.shape[-1], wd, kind, add, dx)
+    return dx
+
+
+def _decoder_input(x, c_in):
+    """x as the kernels read it: channels-last rows [B, H, W, c_in], fp32, contiguous."""
+    if x.dim() != 4 or x.shape[3] != c_in:
+        raise ValueError(f"expected channels-last rows [B, H, W, {c_in}], got shape {tuple(x.shape)}")
+    if not x.is_floating_point():
+        raise TypeError(f"expected a floating-point feature map, got {x.dtype}")
+    return x.float().contiguous()
+
+
+class _ConvTGNAct(torch.autograd.Function):
+    """ReLUWS(GroupNorm(ConvTranspose2dWS(x))), ResNetUp.conv_in, as one node.  Saves x, z and the per-(image,
+    group) statistics."""
+
+    @staticmethod
+    @_fwd_f32
+    def forward(ctx, x, weight, bias, gamma, beta, kind, G, eps):
+        require_cuda(x, weight, bias, gamma, beta)
+        ctx.dtypes = [t.dtype for t in (x, weight, bias, gamma, beta)]
+        x = _decoder_input(x, weight.shape[0])
+        w, b, g, be = _f32(weight, bias, gamma, beta)
+        wf, wd = _convt_weights(w, kind)
+        z, mean, invstd = _convt_fwd(x, wf, b, w.shape[1], kind, G, eps)
+        ctx.save_for_backward(x, w, wd, g, be, z, mean, invstd)
+        ctx.cfg = (kind, G)
+        return _gn_apply(z, (G, mean, invstd, g, be), True)
+
+    @staticmethod
+    @_bwd
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, dy):
+        x, w, wd, g, be, z, mean, invstd = ctx.saved_tensors
+        kind, G = ctx.cfg
+        dz, dg, dbe = _gn_bwd(dy.float().contiguous(), z, (G, mean, invstd, g, be), True)
+        dwf, db = _convt_wgrad(dz, x, kind)
+        dx = _convt_dgrad(dz, x.shape, wd, kind) if ctx.needs_input_grad[0] else None
+        return (*_as_dtypes((dx, _convt_weight_grad(w, dwf, kind), db, dg, dbe), ctx.dtypes), None, None, None)
+
+
+class _ResBlockT(torch.autograd.Function):
+    """A ResBlock of ConvTranspose2dWS (3x3, stride 1, zero padding 1) as one node: h = ReLUWS(GN1(convT1(x))),
+    y = ReLUWS(GN2(convT2(h))) + skip, skip = x or GN_ds(conv1x1(x)) (a plain nn.Conv2d with bias).  Saves x, z1,
+    z2, z_ds and the statistics; h is recomputed in the backward."""
+
+    @staticmethod
+    @_fwd_f32
+    def forward(ctx, x, w1, b1, g1, be1, w2, b2, g2, be2, wd, bd, gd, bed, cfg):
+        require_cuda(x, w1, b1, g1, be1, w2, b2, g2, be2, wd, bd, gd, bed)
+        (G1, eps1), (G2, eps2), (Gd, epsd) = cfg
+        ctx.dtypes = [None if t is None else t.dtype for t in (x, w1, b1, g1, be1, w2, b2, g2, be2, wd, bd, gd, bed)]
+        x = _decoder_input(x, w1.shape[0])
+        w1, b1, g1, be1, w2, b2, g2, be2, wd, bd, gd, bed = _f32(w1, b1, g1, be1, w2, b2, g2, be2, wd, bd, gd, bed)
+        k3 = _lib.DVA_UNET_T_3X3
+        wf1, wd1 = _convt_weights(w1, k3)
+        z1, m1, i1 = _convt_fwd(x, wf1, b1, w1.shape[1], k3, G1, eps1)
+        h = _gn_apply(z1, (G1, m1, i1, g1, be1), True)
+        wf2, wd2 = _convt_weights(w2, k3)
+        z2, m2, i2 = _convt_fwd(h, wf2, b2, w2.shape[1], k3, G2, eps2)
+        del h
+        ds = None
+        wdd = zd = md = idd = None
+        if wd is not None:
+            wfd, wdd = _conv_weights(wd, _lib.DVA_CONV_1X1, False)
+            zd, md, idd = _conv_fwd(x, wfd, bd, wd.shape[0], _lib.DVA_CONV_1X1, Gd, epsd)
+            ds = (zd, Gd, md, idd, gd, bed)
+        y = _gn_apply(z2, (G2, m2, i2, g2, be2), True, skip=x if ds is None else None, ds=ds)
+        ctx.save_for_backward(x, w1, wd1, g1, be1, z1, m1, i1, w2, wd2, g2, be2, z2, m2, i2, wd, wdd, gd, bed, zd,
+                              md, idd)
+        ctx.cfg = cfg
+        return y
+
+    @staticmethod
+    @_bwd
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, dy):
+        (x, w1, wd1, g1, be1, z1, m1, i1, w2, wd2, g2, be2, z2, m2, i2, wd, wdd, gd, bed, zd, md,
+         idd) = ctx.saved_tensors
+        (G1, _), (G2, _), (Gd, _) = ctx.cfg
+        k3, k1 = _lib.DVA_UNET_T_3X3, _lib.DVA_CONV_1X1
+        dy = dy.float().contiguous()
+        gn1, gn2 = (G1, m1, i1, g1, be1), (G2, m2, i2, g2, be2)
+        dz2, dg2, dbe2 = _gn_bwd(dy, z2, gn2, True)
+        h = _gn_apply(z1, gn1, True)
+        dwf2, db2 = _convt_wgrad(dz2, h, k3)
+        dh = _convt_dgrad(dz2, h.shape, wd2, k3)
+        del h
+        dz1, dg1, dbe1 = _gn_bwd(dh, z1, gn1, True)
+        del dh
+        dwf1, db1 = _convt_wgrad(dz1, x, k3)
+        grads_ds = (None,) * 4
+        dx = None
+        if wd is not None:
+            dzd, dgd, dbed = _gn_bwd(dy, zd, (Gd, md, idd, gd, bed), False)
+            dwfd, dbd = _wgrad(dzd, x, k1)
+            grads_ds = (_weight_grad(wd, dwfd, k1, False), dbd, dgd, dbed)
+            if ctx.needs_input_grad[0]:
+                dx = _dgrad(dzd, x.shape, wdd, k1)
+        if ctx.needs_input_grad[0]:
+            dx = _convt_dgrad(dz1, x.shape, wd1, k3, add=dy if dx is None else dx, out=dx)
+        grads = (dx, _convt_weight_grad(w1, dwf1, k3), db1, dg1, dbe1, _convt_weight_grad(w2, dwf2, k3), db2, dg2,
+                 dbe2, *grads_ds)
+        return (*_as_dtypes(grads, ctx.dtypes), None)
+
+
+class _UnaryConv(torch.autograd.Function):
+    """UnaryConv's act(conv1x1(x)) (the 1x1 on libdva_conv2d.so, weight-standardised or not; act = relu * scale or
+    the identity when scale is 0) as one node.  Saves x and z."""
+
+    @staticmethod
+    @_fwd_f32
+    def forward(ctx, x, weight, bias, standardize, scale):
+        require_cuda(x, weight, bias)
+        ctx.dtypes = [t.dtype for t in (x, weight, bias)]
+        x = _encoder_input(x, weight)
+        w, b = _f32(weight, bias)
+        k1 = _lib.DVA_CONV_1X1
+        wf, wd = _conv_weights(w, k1, standardize)
+        z, _, _ = _conv_fwd(x, wf, b, w.shape[0], k1, 1, 1e-5)
+        ctx.save_for_backward(x, w, wd, z)
+        ctx.cfg = (standardize, scale)
+        if not scale:
+            return z
+        y = torch.empty_like(z)
+        launch("dva_unet_act", z.device, z, z.numel(), float(scale), y)
+        return y
+
+    @staticmethod
+    @_bwd
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, dy):
+        x, w, wd, z = ctx.saved_tensors
+        standardize, scale = ctx.cfg
+        k1 = _lib.DVA_CONV_1X1
+        dz = dy.float().contiguous()
+        if scale:
+            dz_act = torch.empty_like(z)
+            launch("dva_unet_act_bwd", z.device, dz, z, z.numel(), float(scale), dz_act)
+            dz = dz_act
+        dwf, db = _wgrad(dz, x, k1)
+        dx = _dgrad(dz, x.shape, wd, k1) if ctx.needs_input_grad[0] else None
+        return (*_as_dtypes((dx, _weight_grad(w, dwf, k1, standardize), db), ctx.dtypes), None, None)
+
+
+def convt_gn_relu_ws(x, conv, norm, kind):
+    """ReLUWS(norm(conv(x))) for channels-last x [B, H, W, C_in] (conv a ConvTranspose2dWS, norm an nn.GroupNorm):
+    fp32 [B, H', W', C_out], computed from fp32 operands whatever the dtype and layout of x."""
+    return _ConvTGNAct.apply(x, conv.weight, conv.bias, norm.weight, norm.bias, kind, norm.num_groups, norm.eps)
+
+
+def res_block_t(x, block):
+    """A ResBlock of ConvTranspose2dWS on channels-last x [B, H, W, C_in]: fp32 [B, H, W, C_out], computed from fp32
+    operands whatever the dtype and layout of x."""
+    c1, n1, _, c2, n2, _ = block.block
+    ds = block.downsample
+    cd, nd = (ds[0], ds[1]) if ds is not None else (None, None)
+    cfg = ((n1.num_groups, n1.eps), (n2.num_groups, n2.eps),
+           (nd.num_groups, nd.eps) if nd is not None else (1, 1e-5))
+    return _ResBlockT.apply(x, c1.weight, c1.bias, n1.weight, n1.bias, c2.weight, c2.bias, n2.weight, n2.bias,
+                            cd.weight if cd is not None else None, cd.bias if cd is not None else None,
+                            nd.weight if nd is not None else None, nd.bias if nd is not None else None, cfg)
+
+
+def unary_conv(x, conv, standardize, scale):
+    """act(conv(x)) for channels-last x [B, H, W, C_in] and a 1x1 conv (nn.Conv2d or Conv2dWS with bias): fp32
+    [B, H, W, C_out]; act = relu(.) * scale, or none when scale is 0."""
+    return _UnaryConv.apply(x, conv.weight, conv.bias, bool(standardize), float(scale))
