@@ -1,7 +1,8 @@
 """ctypes binding of libdva_b200.so (the C ABI declared in include/dva_b200.h), of libdva_eval.so, the
 evaluation kernels (include/dva_eval.h), of libdva_conv2d.so, the image encoder's convolutions
-(include/dva_conv2d.h), and of libdva_unet.so, the image decoder's transposed convolutions (include/dva_unet.h); the
-last three link against the first and share its error string and launch counter.
+(include/dva_conv2d.h), of libdva_unet.so, the image decoder's transposed convolutions (include/dva_unet.h), and of
+libdva_resnet.so, the ADE20K ResNet-18 encoder (include/dva_resnet.h); the last four link against the first and share
+its error string and launch counter.
 
 There is NO fallback: if the shared library is missing or a call fails, a RuntimeError is
 raised.  PyTorch is used above this layer only for device memory and streams.
@@ -20,6 +21,7 @@ CSRC_DIR = os.path.join(_HERE, "csrc")
 EVAL_LIB_PATH = os.path.join(_HERE, "libdva_eval.so")
 CONV_LIB_PATH = os.path.join(_HERE, "libdva_conv2d.so")
 UNET_LIB_PATH = os.path.join(_HERE, "libdva_unet.so")
+RESNET_LIB_PATH = os.path.join(_HERE, "libdva_resnet.so")
 
 DVA_OK, DVA_EINVAL, DVA_EALIGN, DVA_EUNSUPPORTED = 0, -1, -2, -3
 DVA_F32, DVA_BF16, DVA_F16 = 0, 1, 2
@@ -176,10 +178,29 @@ UNET_SIGNATURES = {
 # transposed convolution kinds (include/dva_unet.h)
 DVA_UNET_UP_2X2, DVA_UNET_T_3X3 = 0, 1
 
+# name -> (restype, argtypes); mirrors include/dva_resnet.h one to one
+RESNET_SIGNATURES = {
+    "dva_resnet_weight_prep": (_i32, [_vp, _i32, _i32, _i32, _vp, _vp, _vp]),
+    "dva_resnet_fwd_workspace_bytes": (_sz, [_i64, _i64, _i64, _i32]),
+    "dva_resnet_conv_bn_fwd": (_i32, [_vp, _i64, _i64, _i64, _i32, _vp, _i32, _i32, _i32, _i32, _i32, _f32, _f32, _vp,
+                                      _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "dva_resnet_conv_dgrad": (_i32, [_vp, _i64, _i64, _i64, _i32, _i32, _vp, _i32, _i32, _i32, _vp, _vp, _vp]),
+    "dva_resnet_wgrad_workspace_bytes": (_sz, [_i64, _i64, _i64, _i32, _i32, _i32, _i32, _i32]),
+    "dva_resnet_conv_wgrad": (_i32, [_vp, _vp, _i64, _i64, _i64, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _sz, _vp]),
+    "dva_resnet_bn_apply": (_i32, [_vp, _i64, _i32] + [_vp] * 11 + [_vp]),
+    "dva_resnet_bn_bwd_workspace_bytes": (_sz, [_i64, _i32]),
+    "dva_resnet_bn_bwd": (_i32, [_vp, _vp, _vp, _i64, _i32, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "dva_resnet_maxpool": (_i32, [_vp, _i64, _i64, _i64, _i32, _vp, _vp, _vp]),
+    "dva_resnet_maxpool_bwd": (_i32, [_vp, _vp, _i64, _i64, _i64, _i32, _vp, _vp]),
+    "dva_resnet_resize": (_i32, [_vp, _i64, _i64, _i64, _i32, _i64, _i64, _f32, _f32, _vp, _i64, _i64, _vp]),
+    "dva_resnet_resize_bwd": (_i32, [_vp, _i64, _i64, _i64, _i64, _i64, _i32, _i64, _i64, _f32, _f32, _vp, _vp]),
+}
+
 _lib = None
 _eval_lib = None
 _conv_lib = None
 _unet_lib = None
+_resnet_lib = None
 
 
 def build(verbose=False):
@@ -259,8 +280,18 @@ def load_unet():
     return _unet_lib
 
 
+def load_resnet():
+    """Load libdva_resnet.so (once), after libdva_b200.so.  Raises if it has not been built."""
+    global _resnet_lib
+    if _resnet_lib is None:
+        _resnet_lib = _load_linked(RESNET_LIB_PATH, RESNET_SIGNATURES)
+    return _resnet_lib
+
+
 def entry(name):
     """The entry point `name`, from whichever library declares it."""
+    if name in RESNET_SIGNATURES:
+        return getattr(load_resnet(), name)
     if name in UNET_SIGNATURES:
         return getattr(load_unet(), name)
     if name in EVAL_SIGNATURES:

@@ -559,3 +559,302 @@ class UNet(nn.Module):
         if self.last is not None:
             h = self.last.forward_rows(h, bool(reset))
         return h.to(_out_dtype(x)).permute(0, 3, 1, 2)
+
+
+# --------------------------------------------------------------------------------------------------------------------
+# ResNet-18 pretrained on ADE20K (mit_semseg's resnet18dilated) behind the reference's wrappers (image.py:793-956), on
+# the sm_90a kernels of libdva_resnet.so.  The module tree, parameter and buffer names are the reference's, so a
+# reference DeepViewAgg checkpoint loads with strict=True; the convolutions and BatchNorms only hold the parameters.
+# --------------------------------------------------------------------------------------------------------------------
+class SynchronizedBatchNorm2d(nn.BatchNorm2d):
+    """Parameters and buffers of mit_semseg's SynchronizedBatchNorm2d.  On one device its forward is
+    F.batch_norm(x, running_mean, running_var, weight, bias, training, momentum, eps): num_batches_tracked never moves
+    and the momentum is 0.001.  The three extra buffers are in the state dict and never touched on one device."""
+
+    def __init__(self, num_features, eps=1e-5, momentum=0.001, affine=True):
+        super().__init__(num_features, eps=eps, momentum=momentum, affine=affine)
+        self.register_buffer('_tmp_running_mean', torch.zeros(num_features))
+        self.register_buffer('_tmp_running_var', torch.ones(num_features))
+        self.register_buffer('_running_iter', torch.ones(1))
+
+    def forward(self, input):
+        raise NotImplementedError("SynchronizedBatchNorm2d runs fused with its convolution: call the "
+                                  "ADE20KResNet18* module that holds it")
+
+
+class FusedConv2d(nn.Conv2d):
+    """Parameters of a bias-free convolution of the ResNet-18 trunk; it runs fused with its BatchNorm and ReLU."""
+
+    def forward(self, input):
+        raise NotImplementedError("FusedConv2d runs fused with its BatchNorm: call the ADE20KResNet18* module that "
+                                  "holds it")
+
+
+class FusedReLU(nn.ReLU):
+    """ReLU of the ResNet-18 trunk; fused into the BatchNorm pass."""
+
+    def forward(self, input):
+        raise NotImplementedError("FusedReLU runs fused with its BatchNorm: call the ADE20KResNet18* module that "
+                                  "holds it")
+
+
+class FusedMaxPool2d(nn.MaxPool2d):
+    """MaxPool2d(3, stride 2, padding 1) of the stem; run by the ADE20KResNet18* module that holds it."""
+
+    def __init__(self):
+        super().__init__(kernel_size=3, stride=2, padding=1)
+
+    def forward(self, input):
+        raise NotImplementedError("FusedMaxPool2d is run by the ADE20KResNet18* module that holds it")
+
+
+def _conv3x3(c_in, c_out, stride=1, dilation=1):
+    return FusedConv2d(c_in, c_out, kernel_size=3, stride=stride, padding=dilation, dilation=dilation, bias=False)
+
+
+class BasicBlock(nn.Module):
+    """mit_semseg's BasicBlock: relu(bn2(conv2(relu(bn1(conv1 x)))) + residual), the residual x or
+    downsample = (1x1 conv, BN).  Runs as one node (ops.rn_basic_block)."""
+
+    def __init__(self, inplanes, planes, stride=1, dilation=(1, 1), downsample=None):
+        super().__init__()
+        self.conv1 = _conv3x3(inplanes, planes, stride, dilation[0])
+        self.bn1 = SynchronizedBatchNorm2d(planes)
+        self.relu = FusedReLU(inplace=True)
+        self.conv2 = _conv3x3(planes, planes, 1, dilation[1])
+        self.bn2 = SynchronizedBatchNorm2d(planes)
+        self.downsample = downsample
+        self.stride = stride
+
+    def forward(self, x):
+        return ops.rn_basic_block(x, self)
+
+
+def _make_layer(inplanes, planes, stride, dilations):
+    """Two BasicBlocks as resnet18dilated has them after _nostride_dilate: dilations of (block 0 conv1, every other
+    3x3); the downsample 1x1 has the block's stride."""
+    ds = None
+    if stride != 1 or inplanes != planes:
+        ds = nn.Sequential(FusedConv2d(inplanes, planes, kernel_size=1, stride=stride, bias=False),
+                           SynchronizedBatchNorm2d(planes))
+    d0, d = dilations
+    return nn.Sequential(BasicBlock(inplanes, planes, stride, (d0, d), ds), BasicBlock(planes, planes, 1, (d, d)))
+
+
+def _make_trunk_layer(name):
+    if name == 'layer0':
+        return nn.Sequential(_conv3x3(3, 64, stride=2), SynchronizedBatchNorm2d(64), FusedReLU(inplace=True),
+                             _conv3x3(64, 64), SynchronizedBatchNorm2d(64), FusedReLU(inplace=True),
+                             _conv3x3(64, 128), SynchronizedBatchNorm2d(128), FusedReLU(inplace=True),
+                             FusedMaxPool2d())
+    return {'layer1': lambda: _make_layer(128, 64, 1, (1, 1)), 'layer2': lambda: _make_layer(64, 128, 2, (1, 1)),
+            'layer3': lambda: _make_layer(128, 256, 1, (1, 2)), 'layer4': lambda: _make_layer(256, 512, 1, (2, 4))}[name]()
+
+
+def _mit_semseg_init(module):
+    """mit_semseg's initialisation: conv weights normal with std sqrt(2 / (k^2 C_out)), BN weight 1 and bias 0."""
+    for m in module.modules():
+        if isinstance(m, nn.Conv2d):
+            n = m.kernel_size[0] * m.kernel_size[1] * m.out_channels
+            m.weight.data.normal_(0, sqrt(2. / n))
+        elif isinstance(m, nn.BatchNorm2d):
+            m.weight.data.fill_(1.)
+            m.bias.data.zero_()
+
+
+# positions of mit_semseg's stem modules in layer0
+_STEM_KEYS = {'conv1': '0', 'bn1': '1', 'conv2': '3', 'bn2': '4', 'conv3': '6', 'bn3': '7'}
+_TRUNK_LAYERS = ['layer0', 'layer1', 'layer2', 'layer3', 'layer4']
+
+
+def _mit_semseg_keys():
+    """Every key of mit_semseg's encoder_epoch_20.pth -> (layer, key inside that layer of the wrapper)."""
+    keys = {}
+    inverse = {v: k for k, v in _STEM_KEYS.items()}
+    for name in _TRUNK_LAYERS:
+        for k in _make_trunk_layer(name).state_dict():
+            if name == 'layer0':
+                head, rest = k.split('.', 1)
+                keys[f"{inverse[head]}.{rest}"] = (name, k)
+            else:
+                keys[f"{name}.{k}"] = (name, k)
+    return keys
+
+
+def load_mit_semseg_encoder(module, state_dict):
+    """Load mit_semseg's resnet18dilated encoder state dict (encoder_epoch_20.pth: conv1, bn1, ..., layer4.1.bn2.*)
+    into the layers an ADE20KResNet18* module holds (its conv.<i>.*).  The state dict must have exactly the
+    checkpoint's keys; a missing or extra key raises KeyError."""
+    mapping = _mit_semseg_keys()
+    missing = sorted(set(mapping) - set(state_dict))
+    extra = sorted(set(state_dict) - set(mapping))
+    if missing or extra:
+        raise KeyError(f"not a mit_semseg resnet18dilated encoder state dict: missing {missing[:5]}"
+                       f"{' ...' if len(missing) > 5 else ''}, unexpected {extra[:5]}{' ...' if len(extra) > 5 else ''}")
+    position = {name: i for i, name in enumerate(module._LAYERS)}
+    ours = {f"conv.{position[layer]}.{k}": state_dict[key] for key, (layer, k) in mapping.items() if layer in position}
+    module.load_state_dict(ours, strict=True)
+    return module
+
+
+class ADE20KResNet18TruncatedLayer4(nn.Module):
+    """ResNet-18 encoder pretrained on ADE20K (mit_semseg's resnet18dilated), truncated after `_LAYERS`
+    (image.py:793-898), on the sm_90a kernels of libdva_resnet.so.
+
+    weights: None (mit_semseg's random initialisation), a path to mit_semseg's encoder_epoch_20.pth or its state
+    dict (load_mit_semseg_encoder).  The reference always loads that checkpoint from its own tree.
+    Input [B, 3, H, W] on CUDA (input_nc channels), NCHW or channels-last; output [B, output_nc, H', W'] in the
+    input's dtype (fp32 under autocast) with channels-last strides.  Each BatchNorm runs in its own mode (its
+    .training): batch statistics and a running-stat update (momentum 0.001) in training mode, the running stats in
+    eval mode."""
+    _LAYERS = ['layer0', 'layer1', 'layer2', 'layer3', 'layer4']
+    _LAYERS_IN = {k: v for k, v in zip(_TRUNK_LAYERS, [3, 128, 64, 128, 256])}
+    _LAYERS_OUT = {k: v for k, v in zip(_TRUNK_LAYERS, [128, 64, 128, 256, 512])}
+    _LAYERS_SCALE = {k: v for k, v in zip(_TRUNK_LAYERS, [4, 1, 2, 1, 1])}
+
+    def __init__(self, frozen=False, scale_factor=None, weights=None, **kwargs):
+        super().__init__()
+        self.conv = nn.Sequential(*[_make_trunk_layer(layer) for layer in self._LAYERS])
+        _mit_semseg_init(self.conv)
+        if weights is not None:
+            if not isinstance(weights, dict):
+                weights = torch.load(weights, map_location='cpu')
+            load_mit_semseg_encoder(self, weights)
+
+        # If the model is frozen, it will always remain in eval mode and the parameters will have requires_grad=False
+        self.frozen = frozen
+        if self.frozen:
+            self.training = False
+
+        # scale_factor < 0: resize by conv_scale_factor
+        if scale_factor is not None and scale_factor < 0:
+            scale_factor = self.conv_scale_factor
+        self.scale_factor = scale_factor
+
+    def _check_input(self, x):
+        require_cuda(x)
+        if x.dim() != 4 or x.shape[1] != self.input_nc:
+            raise ValueError(f"{type(self).__name__} expects [B, {self.input_nc}, H, W] images, got shape "
+                             f"{tuple(x.shape)}")
+        B, _, H, W = x.shape
+        for bn, H, W in self._bn_sizes(H, W):
+            if bn.training and B * H * W <= 1:
+                raise ValueError(f"Expected more than 1 value per channel when training, got input size "
+                                 f"{[B, bn.num_features, H, W]}")
+
+    def _bn_sizes(self, H, W):
+        """Yields (BatchNorm, H, W of the map it normalises) along the trunk for an H x W input."""
+        for layer in self.conv:
+            if isinstance(layer[0], BasicBlock):
+                for block in layer:
+                    H, W = ops.rn_out(H, block.conv1.stride[0]), ops.rn_out(W, block.conv1.stride[0])
+                    yield block.bn1, H, W
+                    yield block.bn2, H, W
+                    if block.downsample is not None:
+                        yield block.downsample[1], H, W
+            else:
+                for i in (0, 3, 6):
+                    H, W = ops.rn_out(H, layer[i].stride[0]), ops.rn_out(W, layer[i].stride[0])
+                    yield layer[i + 1], H, W
+                H, W = ops.rn_out(H, 2), ops.rn_out(W, 2)
+
+    def _layers(self, h):
+        """Yields the channels-last output of each layer of self.conv for channels-last rows h."""
+        for layer in self.conv:
+            if isinstance(layer[0], BasicBlock):
+                for block in layer:
+                    h = ops.rn_basic_block(h, block)
+            else:
+                for i in (0, 3, 6):
+                    h = ops.rn_conv_bn_relu(h, layer[i], layer[i + 1])
+                h = ops.rn_maxpool(h)
+            yield h
+
+    def forward(self, x, *args, **kwargs):
+        self._check_input(x)
+        for h in self._layers(_rows(x)):
+            pass
+        if self.scale_factor is not None:
+            size = (int(h.shape[1] * float(self.scale_factor)), int(h.shape[2] * float(self.scale_factor)))
+            h = ops.rn_resize([h], size, scale_factor=float(self.scale_factor))
+        return h.to(_out_dtype(x)).permute(0, 3, 1, 2)
+
+    @property
+    def input_nc(self):
+        return self._LAYERS_IN[self._LAYERS[0]]
+
+    @property
+    def output_nc(self):
+        return self._LAYERS_OUT[self._LAYERS[-1]]
+
+    @property
+    def conv_scale_factor(self):
+        return torch.prod(torch.LongTensor([self._LAYERS_SCALE[s] for s in self._LAYERS])).item()
+
+    @property
+    def frozen(self):
+        return self._frozen
+
+    @frozen.setter
+    def frozen(self, frozen):
+        if isinstance(frozen, bool):
+            self._frozen = frozen
+        for p in self.parameters():
+            p.requires_grad = not self.frozen
+
+    def train(self, mode=True):
+        return super().train(mode and not self.frozen)
+
+    def extra_repr(self) -> str:
+        return f"scale_factor={self.scale_factor}" if self.scale_factor is not None else ""
+
+
+class ADE20KResNet18TruncatedLayer0(ADE20KResNet18TruncatedLayer4):
+    _LAYERS = ['layer0']
+
+
+class ADE20KResNet18TruncatedLayer1(ADE20KResNet18TruncatedLayer4):
+    _LAYERS = ['layer0', 'layer1']
+
+
+class ADE20KResNet18TruncatedLayer2(ADE20KResNet18TruncatedLayer4):
+    _LAYERS = ['layer0', 'layer1', 'layer2']
+
+
+class ADE20KResNet18TruncatedLayer3(ADE20KResNet18TruncatedLayer4):
+    _LAYERS = ['layer0', 'layer1', 'layer2', 'layer3']
+
+
+class ADE20KResNet18Layer0(ADE20KResNet18TruncatedLayer4):
+    _LAYERS = ['layer0']
+
+
+class ADE20KResNet18Layer1(ADE20KResNet18TruncatedLayer4):
+    _LAYERS = ['layer1']
+
+
+class ADE20KResNet18Layer2(ADE20KResNet18TruncatedLayer4):
+    _LAYERS = ['layer2']
+
+
+class ADE20KResNet18Layer3(ADE20KResNet18TruncatedLayer4):
+    _LAYERS = ['layer3']
+
+
+class ADE20KResNet18Layer4(ADE20KResNet18TruncatedLayer4):
+    _LAYERS = ['layer4']
+
+
+class ADE20KResNet18Pyramid(ADE20KResNet18TruncatedLayer4):
+    """Every layer's output resized to int(side * scale_factor / conv_scale_factor) of the input sides (a size-based
+    bilinear resize) and concatenated: 128 + 64 + 128 + 256 + 512 = 1088 channels, written into one buffer."""
+
+    def __init__(self, frozen=False, scale_factor=-1, **kwargs):
+        assert scale_factor is not None, f'scale_factor cannot be None for feature pyramid.'
+        super().__init__(frozen=frozen, scale_factor=scale_factor, **kwargs)
+
+    def forward(self, x, *args, **kwargs):
+        self._check_input(x)
+        size = [int(s * self.scale_factor / self.conv_scale_factor) for s in x.shape[2:4]]
+        h = ops.rn_resize(list(self._layers(_rows(x))), size)
+        return h.to(_out_dtype(x)).permute(0, 3, 1, 2)

@@ -1865,3 +1865,304 @@ def unary_conv(x, conv, standardize, scale):
     """act(conv(x)) for channels-last x [B, H, W, C_in] and a 1x1 conv (nn.Conv2d or Conv2dWS with bias): fp32
     [B, H, W, C_out]; act = relu(.) * scale, or none when scale is 0."""
     return _UnaryConv.apply(x, conv.weight, conv.bias, bool(standardize), float(scale))
+
+
+# --------------------------------------------------------------------------------------------
+# ADE20K ResNet-18 encoder (libdva_resnet.so, include/dva_resnet.h): mit_semseg's resnet18dilated behind the
+# reference's ADE20KResNet18* wrappers (modalities/image.py:793-956).  One autograd node per stem unit (conv -> BN ->
+# ReLU), per BasicBlock (its hidden activation recomputed in the backward), for the max pool and for a (multi-map)
+# bilinear resize.  BatchNorm is F.batch_norm on one device: in training mode the batch statistics normalise and the
+# running stats are updated inside the forward (a second call, such as the recompute of a reentrant checkpoint,
+# updates them again).  Maps are channels-last [B, H, W, C] fp32; products are 3xTF32 on tensor cores, also under
+# autocast (the inputs are cast to fp32); gradients come back in each input's dtype.
+# --------------------------------------------------------------------------------------------
+def rn_out(n, stride):
+    """Output side of a stride-`stride` convolution or max pool of the trunk: ceil(n / stride)."""
+    return (n - 1) // stride + 1
+
+
+def _rn_weights(w):
+    """(wf, wd): the filter the forward reads ([Co][T][T][Ci]) and the one the data gradient reads ([Ci][T][T][Co])."""
+    Co, Ci, T = w.shape[0], w.shape[1], w.shape[2]
+    wf = torch.empty(w.numel(), dtype=torch.float32, device=w.device)
+    wd = torch.empty_like(wf)
+    launch("dva_resnet_weight_prep", w.device, w, Co, Ci, T, wf, wd)
+    return wf, wd
+
+
+def _rn_running(t):
+    """A running-stat buffer as the kernel updates it in place: itself when fp32 and contiguous, else a copy."""
+    return t if t.dtype == torch.float32 and t.is_contiguous() else t.detach().float().contiguous()
+
+
+def _rn_conv_bn(x, wf, Co, geo, bn):
+    """z = conv(x) and the BatchNorm statistics of z; bn = (running_mean, running_var, training, momentum, eps)."""
+    T, stride, dil = geo
+    rm, rv, training, momentum, eps = bn
+    B, H, W, Ci = x.shape
+    Ho, Wo = rn_out(H, stride), rn_out(W, stride)
+    z = torch.empty(B, Ho, Wo, Co, dtype=torch.float32, device=x.device)
+    mean = torch.empty(Co, dtype=torch.float32, device=x.device)
+    invstd = torch.empty_like(mean)
+    ws = _lib.workspace(_lib.load_resnet().dva_resnet_fwd_workspace_bytes(B, Ho, Wo, Co) if training else 0, x.device)
+    rm32, rv32 = _rn_running(rm), _rn_running(rv)
+    launch("dva_resnet_conv_bn_fwd", x.device, x, B, H, W, Ci, wf, Co, T, stride, dil, int(training), float(momentum),
+           float(eps), rm32, rv32, z, mean, invstd, ws, ws.numel())
+    if training:
+        for buf, b32 in ((rm, rm32), (rv, rv32)):
+            if b32 is not buf:
+                buf.copy_(b32)
+    return z, mean, invstd
+
+
+def _rn_apply(z, mean, invstd, gamma, beta, skip=None, ds=None):
+    """relu(BN(z) [+ skip] [+ BN_ds(z_ds)]); ds = (z_ds, mean, invstd, gamma, beta)."""
+    B, H, W, C = z.shape
+    zs, ms, iss, gs, bs = ds if ds is not None else (None,) * 5
+    y = torch.empty_like(z)
+    launch("dva_resnet_bn_apply", z.device, z, B * H * W, C, mean, invstd, gamma, beta, skip, zs, ms, iss, gs, bs, y)
+    return y
+
+
+def _rn_bn_bwd(dy, y, z, mean, invstd, gamma, training, want_g=False):
+    """(dz, g, dgamma, dbeta) of y = relu(BN(z) + r); g, the gradient reaching r, only when want_g."""
+    B, H, W, C = z.shape
+    M = B * H * W
+    dz = torch.empty_like(z)
+    g = torch.empty_like(z) if want_g else None
+    dgamma = torch.empty(C, dtype=torch.float32, device=z.device)
+    dbeta = torch.empty_like(dgamma)
+    ws = _lib.workspace(_lib.load_resnet().dva_resnet_bn_bwd_workspace_bytes(M, C), z.device)
+    launch("dva_resnet_bn_bwd", z.device, dy, y, z, M, C, mean, invstd, gamma, int(training), dz, g, dgamma, dbeta,
+           ws, ws.numel())
+    return dz, g, dgamma, dbeta
+
+
+def _rn_wgrad(dz, x, Co, geo):
+    T, stride, dil = geo
+    B, H, W, Ci = x.shape
+    dw = torch.empty(Co, Ci, T, T, dtype=torch.float32, device=x.device)
+    ws = _lib.workspace(_lib.load_resnet().dva_resnet_wgrad_workspace_bytes(B, H, W, Ci, Co, T, stride, dil), x.device)
+    launch("dva_resnet_conv_wgrad", x.device, dz, x, B, H, W, Ci, Co, T, stride, dil, dw, ws, ws.numel())
+    return dw
+
+
+def _rn_dgrad(dz, x_shape, wd, geo, add=None, out=None):
+    """conv^T(dz) [+ add] into out (a new tensor when None; out may be add)."""
+    T, stride, dil = geo
+    B, H, W, Ci = x_shape
+    dx = out if out is not None else torch.empty(B, H, W, Ci, dtype=torch.float32, device=dz.device)
+    launch("dva_resnet_conv_dgrad", dz.device, dz, B, H, W, Ci, dz.shape[-1], wd, T, stride, dil, add, dx)
+    return dx
+
+
+def _rn_input(x, c_in):
+    if x.dim() != 4 or x.shape[3] != c_in:
+        raise ValueError(f"expected channels-last rows [B, H, W, {c_in}], got shape {tuple(x.shape)}")
+    if not x.is_floating_point():
+        raise TypeError(f"expected a floating-point feature map, got {x.dtype}")
+    return x.float().contiguous()
+
+
+def _bn_cfg(bn):
+    return (bn.training, bn.momentum, bn.eps)
+
+
+class _RNConvBNReLU(torch.autograd.Function):
+    """relu(BN(conv(x))), a unit of the deep stem, as one node.  Saves x, z, the statistics and the output (the
+    ReLU mask)."""
+
+    @staticmethod
+    @_fwd_f32
+    def forward(ctx, x, weight, gamma, beta, running_mean, running_var, geo, bn_cfg):
+        require_cuda(x, weight, gamma, beta)
+        ctx.dtypes = [t.dtype for t in (x, weight, gamma, beta)]
+        x = _rn_input(x, weight.shape[1])
+        w, g, b = _f32(weight, gamma, beta)
+        training, momentum, eps = bn_cfg
+        wf, wd = _rn_weights(w)
+        z, mean, invstd = _rn_conv_bn(x, wf, w.shape[0], geo, (running_mean, running_var, training, momentum, eps))
+        y = _rn_apply(z, mean, invstd, g, b)
+        ctx.save_for_backward(x, wd, g, z, mean, invstd, y)
+        ctx.cfg = (geo, training, w.shape[0])
+        return y
+
+    @staticmethod
+    @_bwd
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, dy):
+        x, wd, g, z, mean, invstd, y = ctx.saved_tensors
+        geo, training, Co = ctx.cfg
+        dz, _, dg, db = _rn_bn_bwd(dy.float().contiguous(), y, z, mean, invstd, g, training)
+        dw = _rn_wgrad(dz, x, Co, geo) if ctx.needs_input_grad[1] else None
+        dx = _rn_dgrad(dz, x.shape, wd, geo) if ctx.needs_input_grad[0] else None
+        return (*_as_dtypes((dx, dw, dg, db), ctx.dtypes), None, None, None, None)
+
+
+class _RNBasicBlock(torch.autograd.Function):
+    """mit_semseg's BasicBlock as one node: h = relu(bn1(conv1(x))), y = relu(bn2(conv2(h)) + r), r = x or
+    bn_ds(conv1x1(x)).  Saves x, z1, z2, z_ds, the statistics and y; h is recomputed in the backward."""
+
+    @staticmethod
+    @_fwd_f32
+    def forward(ctx, x, w1, g1, b1, w2, g2, b2, wd, gd, bd, rm1, rv1, rm2, rv2, rmd, rvd, cfg):
+        require_cuda(x, w1, g1, b1, w2, g2, b2, wd, gd, bd)
+        (stride, dil1, dil2), bn1, bn2, bnd = cfg
+        ctx.dtypes = [None if t is None else t.dtype for t in (x, w1, g1, b1, w2, g2, b2, wd, gd, bd)]
+        x = _rn_input(x, w1.shape[1])
+        w1, g1, b1, w2, g2, b2, wd, gd, bd = _f32(w1, g1, b1, w2, g2, b2, wd, gd, bd)
+        geo1, geo2, geod = (3, stride, dil1), (3, 1, dil2), (1, stride, 1)
+        wf1, wd1 = _rn_weights(w1)
+        z1, m1, i1 = _rn_conv_bn(x, wf1, w1.shape[0], geo1, (rm1, rv1, *bn1))
+        h = _rn_apply(z1, m1, i1, g1, b1)
+        wf2, wd2 = _rn_weights(w2)
+        z2, m2, i2 = _rn_conv_bn(h, wf2, w2.shape[0], geo2, (rm2, rv2, *bn2))
+        del h
+        wdd = zd = md = idd = None
+        if wd is not None:
+            wfd, wdd = _rn_weights(wd)
+            zd, md, idd = _rn_conv_bn(x, wfd, wd.shape[0], geod, (rmd, rvd, *bnd))
+            y = _rn_apply(z2, m2, i2, g2, b2, ds=(zd, md, idd, gd, bd))
+        else:
+            y = _rn_apply(z2, m2, i2, g2, b2, skip=x)
+        ctx.save_for_backward(x, wd1, g1, b1, z1, m1, i1, wd2, g2, z2, m2, i2, wdd, gd, zd, md, idd, y)
+        ctx.cfg = (geo1, geo2, geod, bn1[0], bn2[0], bnd[0] if bnd is not None else False, w1.shape[0])
+        return y
+
+    @staticmethod
+    @_bwd
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, dy):
+        x, wd1, g1, b1, z1, m1, i1, wd2, g2, z2, m2, i2, wdd, gd, zd, md, idd, y = ctx.saved_tensors
+        geo1, geo2, geod, t1, t2, td, Co = ctx.cfg
+        need = ctx.needs_input_grad
+        dy = dy.float().contiguous()
+        dz2, gr, dg2, db2 = _rn_bn_bwd(dy, y, z2, m2, i2, g2, t2, want_g=zd is None)
+        h = _rn_apply(z1, m1, i1, g1, b1)
+        dw2 = _rn_wgrad(dz2, h, Co, geo2) if need[4] else None
+        dh = _rn_dgrad(dz2, h.shape, wd2, geo2)
+        dz1, _, dg1, db1 = _rn_bn_bwd(dh, h, z1, m1, i1, g1, t1)
+        del h, dh
+        dw1 = _rn_wgrad(dz1, x, Co, geo1) if need[1] else None
+        grads_ds = (None,) * 3
+        dx = None
+        if zd is not None:
+            dzd, _, dgd, dbd = _rn_bn_bwd(dy, y, zd, md, idd, gd, td)
+            grads_ds = (_rn_wgrad(dzd, x, Co, geod) if need[7] else None, dgd, dbd)
+            if need[0]:
+                dx = _rn_dgrad(dzd, x.shape, wdd, geod)
+        if need[0]:
+            dx = _rn_dgrad(dz1, x.shape, wd1, geo1, add=gr if dx is None else dx, out=dx)
+        grads = (dx, dw1, dg1, db1, dw2, dg2, db2, *grads_ds)
+        return (*_as_dtypes(grads, ctx.dtypes), *([None] * 7))
+
+
+class _RNMaxPool(torch.autograd.Function):
+    """MaxPool2d(3, stride 2, padding 1) with the window position of the max saved for the backward."""
+
+    @staticmethod
+    @_fwd_f32
+    def forward(ctx, x):
+        require_cuda(x)
+        ctx.dtype = x.dtype
+        x = x.float().contiguous()
+        B, H, W, C = x.shape
+        y = torch.empty(B, rn_out(H, 2), rn_out(W, 2), C, dtype=torch.float32, device=x.device)
+        arg = torch.empty(y.shape, dtype=torch.uint8, device=x.device)
+        launch("dva_resnet_maxpool", x.device, x, B, H, W, C, y, arg)
+        ctx.save_for_backward(arg)
+        ctx.shape = (B, H, W, C)
+        ctx.mark_non_differentiable(arg)
+        return y
+
+    @staticmethod
+    @_bwd
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, dy):
+        (arg,) = ctx.saved_tensors
+        B, H, W, C = ctx.shape
+        dx = torch.empty(B, H, W, C, dtype=torch.float32, device=dy.device)
+        launch("dva_resnet_maxpool_bwd", dy.device, dy.float().contiguous(), arg, B, H, W, C, dx)
+        return dx.to(ctx.dtype)
+
+
+def resize_scale(n_in, n_out, scale_factor=None):
+    """The scale of torch's bilinear source index (align_corners=False): float32(1 / scale_factor) when a factor is
+    given, float32(n_in) / n_out when a size is."""
+    if scale_factor is not None and scale_factor > 0:
+        return float(np.float32(1.0 / scale_factor))
+    return float(np.float32(n_in) / np.float32(n_out))
+
+
+class _RNResize(torch.autograd.Function):
+    """Bilinear resizes (align_corners=False) of several maps [B, H_i, W_i, C_i] to one size, concatenated along the
+    channels: each map is written into its own column slice of the [B, Ho, Wo, sum C_i] output."""
+
+    @staticmethod
+    @_fwd_f32
+    def forward(ctx, size, scales, *xs):
+        require_cuda(*xs)
+        Ho, Wo = size
+        ctx.dtypes = [x.dtype for x in xs]
+        xs = [x.float().contiguous() for x in xs]
+        B, ld = xs[0].shape[0], sum(x.shape[3] for x in xs)
+        y = torch.empty(B, Ho, Wo, ld, dtype=torch.float32, device=xs[0].device)
+        col = 0
+        for x, (sh, sw) in zip(xs, scales):
+            _, H, W, C = x.shape
+            launch("dva_resnet_resize", x.device, x, B, H, W, C, Ho, Wo, sh, sw, y, ld, col)
+            col += C
+        ctx.shapes = [tuple(x.shape) for x in xs]
+        ctx.cfg = (size, scales, ld)
+        return y
+
+    @staticmethod
+    @_bwd
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, dy):
+        (Ho, Wo), scales, ld = ctx.cfg
+        dy = dy.float().contiguous()
+        grads, col = [], 0
+        for (B, H, W, C), (sh, sw), need in zip(ctx.shapes, scales, ctx.needs_input_grad[2:]):
+            if need:
+                dx = torch.empty(B, H, W, C, dtype=torch.float32, device=dy.device)
+                launch("dva_resnet_resize_bwd", dy.device, dy, ld, col, B, H, W, C, Ho, Wo, sh, sw, dx)
+                grads.append(dx)
+            else:
+                grads.append(None)
+            col += C
+        return (None, None, *_as_dtypes(grads, ctx.dtypes))
+
+
+def rn_conv_bn_relu(x, conv, bn):
+    """relu(bn(conv(x))) for channels-last x [B, H, W, C_in] (conv an nn.Conv2d without bias, bn a BatchNorm2d):
+    fp32 [B, H', W', C_out]; in training mode bn's running stats are updated."""
+    geo = (conv.kernel_size[0], conv.stride[0], conv.dilation[0])
+    return _RNConvBNReLU.apply(x, conv.weight, bn.weight, bn.bias, bn.running_mean, bn.running_var, geo, _bn_cfg(bn))
+
+
+def rn_basic_block(x, block):
+    """A BasicBlock (conv1, bn1, conv2, bn2, downsample) on channels-last x [B, H, W, C_in]: fp32 [B, H', W', C_out]."""
+    ds = block.downsample
+    cd, nd = (ds[0], ds[1]) if ds is not None else (None, None)
+    cfg = ((block.conv1.stride[0], block.conv1.dilation[0], block.conv2.dilation[0]), _bn_cfg(block.bn1),
+           _bn_cfg(block.bn2), _bn_cfg(nd) if nd is not None else None)
+    return _RNBasicBlock.apply(x, block.conv1.weight, block.bn1.weight, block.bn1.bias, block.conv2.weight,
+                               block.bn2.weight, block.bn2.bias, cd.weight if cd is not None else None,
+                               nd.weight if nd is not None else None, nd.bias if nd is not None else None,
+                               block.bn1.running_mean, block.bn1.running_var, block.bn2.running_mean,
+                               block.bn2.running_var, nd.running_mean if nd is not None else None,
+                               nd.running_var if nd is not None else None, cfg)
+
+
+def rn_maxpool(x):
+    """MaxPool2d(3, 2, 1) of channels-last x [B, H, W, C]: fp32 [B, ceil(H/2), ceil(W/2), C]."""
+    return _RNMaxPool.apply(x)
+
+
+def rn_resize(xs, size, scale_factor=None):
+    """Bilinear resizes (align_corners=False) of the channels-last maps xs to size (Ho, Wo), concatenated along the
+    channels; scale_factor, when given, sets torch's source scale 1 / scale_factor (F.interpolate(scale_factor=))."""
+    scales = [(resize_scale(x.shape[1], size[0], scale_factor), resize_scale(x.shape[2], size[1], scale_factor))
+              for x in xs]
+    return _RNResize.apply(tuple(int(s) for s in size), scales, *xs)
