@@ -57,8 +57,7 @@ template <int MODE>
 __global__ void __launch_bounds__(kThreads) conv_gemm_kernel(GemmArgs a) {
   __shared__ __align__(16) float smem[2 * (BM + BN) * LDS];
   __shared__ double2 colst[2][BN];
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int wm = warp >> 1, wn = warp & 1, g = lane >> 2, tq = lane & 3;
+  const int tid = threadIdx.x;
   const int64_t b = blockIdx.x / a.tiles;
   const int t = (int)(blockIdx.x - b * a.tiles);
   const int64_t P = a.Ho * a.Wo, p0 = (int64_t)t * BM;
@@ -66,12 +65,7 @@ __global__ void __launch_bounds__(kThreads) conv_gemm_kernel(GemmArgs a) {
   const int64_t img = b * a.H * a.W;   // first source pixel of image b (gathering modes)
   const int64_t row0 = b * P + p0;     // first GEMM row of the tile
   int oh[8], ow[8];
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    const int64_t p = p0 + (tid >> 4) + 8 * i;
-    oh[i] = p < P ? (int)(p / a.Wo) : -1;
-    ow[i] = p < P ? (int)(p - (p / a.Wo) * a.Wo) : 0;
-  }
+  tile_pixels(p0, P, a.Wo, oh, ow);
   const int H = (int)a.H, W = (int)a.W, Cs = a.Cs, K = a.K;
   auto fa = [&](int i, int row, int64_t k64) -> float {
     if (oh[i] < 0) return 0.f;
@@ -117,58 +111,39 @@ __global__ void __launch_bounds__(kThreads) conv_gemm_kernel(GemmArgs a) {
 #pragma unroll
   for (int m = 0; m < 2; ++m)
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int64_t p = p0 + wm * 32 + m * 16 + g + 8 * h;
-      if (p >= P) continue;
-#pragma unroll
-      for (int n = 0; n < 4; ++n)
-#pragma unroll
-        for (int j = 0; j < 2; ++j) {
-          const int col = n0 + wn * 32 + n * 8 + 2 * tq + j;
-          if (col >= a.N) continue;
-          float v = acc[m][n][2 * h + j];
-          if (MODE == kFwd3 || MODE == kFwd2 || MODE == kFwd1) {
-            v += __ldg(a.bias + col);
-            a.out[(b * P + p) * a.N + col] = v;
-            cs[n][j] += (double)v;
-            cq[n][j] += (double)v * (double)v;
-          } else if (MODE == kDgrad2) {
-            // col = (r * 2 + s) * Ci + c; dz row (oh, ow) reaches dx pixel (2 oh + r, 2 ow + s) only
-            const int Ci = a.N >> 2, rs = col / Ci, c = col - rs * Ci, r = rs >> 1, s = rs & 1;
-            const int64_t ohh = p / a.Wo, oww = p - ohh * a.Wo;
-            const int64_t ih = 2 * ohh + r, iw = 2 * oww + s;
-            const int64_t o = ((b * a.Hx + ih) * a.Wx + iw) * Ci + c;
-            a.out[o] = a.add ? v + a.add[o] : v;
-            // rows / columns the floor dropped: no tap reaches them
-            const bool lr = r == 1 && ohh == a.Ho - 1 && a.Hx > 2 * a.Ho;
-            const bool lc = s == 1 && oww == a.Wo - 1 && a.Wx > 2 * a.Wo;
-            if (lr) { const int64_t e = o + a.Wx * Ci; a.out[e] = a.add ? a.add[e] : 0.f; }
-            if (lc) { const int64_t e = o + Ci; a.out[e] = a.add ? a.add[e] : 0.f; }
-            if (lr && lc) { const int64_t e = o + (a.Wx + 1) * Ci; a.out[e] = a.add ? a.add[e] : 0.f; }
-          } else {
-            const int64_t o = (b * P + p) * a.N + col;
-            a.out[o] = a.add ? v + a.add[o] : v;
-          }
-        }
-    }
-  if (MODE == kFwd3 || MODE == kFwd2 || MODE == kFwd1) {
-    // column sums over the warp's 32 rows (lanes of equal tq), then over the two row halves, then per group
-#pragma unroll
     for (int n = 0; n < 4; ++n)
 #pragma unroll
-      for (int j = 0; j < 2; ++j)
-#pragma unroll
-        for (int o = 4; o < 32; o <<= 1) {
-          cs[n][j] += __shfl_xor_sync(0xffffffffu, cs[n][j], o);
-          cq[n][j] += __shfl_xor_sync(0xffffffffu, cq[n][j], o);
+      for (int q = 0; q < 4; ++q) {
+        const int64_t p = p0 + acc_row(m, q);
+        const int col = n0 + acc_col(n, q);
+        if (p >= P || col >= a.N) continue;
+        float v = acc[m][n][q];
+        if (MODE == kFwd3 || MODE == kFwd2 || MODE == kFwd1) {
+          v += __ldg(a.bias + col);
+          a.out[(b * P + p) * a.N + col] = v;
+          cs[n][q & 1] += (double)v;
+          cq[n][q & 1] += (double)v * (double)v;
+        } else if (MODE == kDgrad2) {
+          // col = (r * 2 + s) * Ci + c; dz row (oh, ow) reaches dx pixel (2 oh + r, 2 ow + s) only
+          const int Ci = a.N >> 2, rs = col / Ci, c = col - rs * Ci, r = rs >> 1, s = rs & 1;
+          const int64_t ohh = p / a.Wo, oww = p - ohh * a.Wo;
+          const int64_t ih = 2 * ohh + r, iw = 2 * oww + s;
+          const int64_t o = ((b * a.Hx + ih) * a.Wx + iw) * Ci + c;
+          a.out[o] = a.add ? v + a.add[o] : v;
+          // rows / columns the floor dropped: no tap reaches them
+          const bool lr = r == 1 && ohh == a.Ho - 1 && a.Hx > 2 * a.Ho;
+          const bool lc = s == 1 && oww == a.Wo - 1 && a.Wx > 2 * a.Wo;
+          if (lr) { const int64_t e = o + a.Wx * Ci; a.out[e] = a.add ? a.add[e] : 0.f; }
+          if (lc) { const int64_t e = o + Ci; a.out[e] = a.add ? a.add[e] : 0.f; }
+          if (lr && lc) { const int64_t e = o + (a.Wx + 1) * Ci; a.out[e] = a.add ? a.add[e] : 0.f; }
+        } else {
+          const int64_t o = (b * P + p) * a.N + col;
+          a.out[o] = a.add ? v + a.add[o] : v;
         }
-    if (g == 0) {
-#pragma unroll
-      for (int n = 0; n < 4; ++n)
-#pragma unroll
-        for (int j = 0; j < 2; ++j) colst[wm][wn * 32 + n * 8 + 2 * tq + j] = make_double2(cs[n][j], cq[n][j]);
-    }
-    __syncthreads();
+      }
+  if (MODE == kFwd3 || MODE == kFwd2 || MODE == kFwd1) {
+    // column sums over the two row halves, then per group
+    column_stats(cs, cq, colst);
     const int n_end = min(n0 + BN, a.N);
     const int g_lo = n0 / a.cpg, g_hi = (n_end - 1) / a.cpg;
     const int gg = g_lo + tid;
@@ -198,14 +173,7 @@ gn_stats_kernel(const double2* __restrict__ part, int tiles, int ntiles, int G, 
       s += d.x;
       q += d.y;
     }
-  s = block_sum(s, sh);
-  q = block_sum(q, sh);
-  if (threadIdx.x == 0) {
-    const double n = (double)P * cpg, mu = s / n;
-    const double var = fmax(q / n - mu * mu, 0.0);
-    mean[blockIdx.x] = (float)mu;
-    invstd[blockIdx.x] = (float)(1.0 / sqrt(var + (double)eps));
-  }
+  finish_stats(s, q, (double)P * cpg, eps, mean[blockIdx.x], invstd[blockIdx.x], sh);
 }
 
 struct WgradArgs {
@@ -220,12 +188,10 @@ struct WgradArgs {
 template <int KIND>
 __global__ void __launch_bounds__(kThreads) conv_wgrad_kernel(WgradArgs a) {
   __shared__ __align__(16) float smem[2 * (BM + BN) * LDS];
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int wm = warp >> 1, wn = warp & 1, g = lane >> 2, tq = lane & 3;
   const int i0 = blockIdx.x * BM, j0 = blockIdx.y * BN;
   const int64_t m_begin = (int64_t)blockIdx.z * a.rows_per_split;
   const int64_t m_end = min(a.M, m_begin + a.rows_per_split);
-  const int oc = i0 + (tid & 63), j = j0 + (tid & 63);
+  const int oc = i0 + (threadIdx.x & 63), j = j0 + (threadIdx.x & 63);
   constexpr int T = KIND == DVA_CONV_3X3_REFLECT ? 3 : (KIND == DVA_CONV_2X2_S2 ? 2 : 1);
   const int r = j / (T * a.Ci), rem = j - r * T * a.Ci, s = rem / a.Ci, c = rem - s * a.Ci;
   const int H = (int)a.H, W = (int)a.W;
@@ -243,21 +209,7 @@ __global__ void __launch_bounds__(kThreads) conv_wgrad_kernel(WgradArgs a) {
   float acc[2][4][4];
   gemm_mainloop<true, true>(fa, fb, m_begin, m_end, smem, acc);
   const int Kp = a.Kd + 1;
-  float* out = a.part + (int64_t)blockIdx.z * a.Co * Kp;
-#pragma unroll
-  for (int m = 0; m < 2; ++m)
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int o = i0 + wm * 32 + m * 16 + g + 8 * h;
-      if (o >= a.Co) continue;
-#pragma unroll
-      for (int n = 0; n < 4; ++n)
-#pragma unroll
-        for (int jj = 0; jj < 2; ++jj) {
-          const int col = j0 + wn * 32 + n * 8 + 2 * tq + jj;
-          if (col < Kp) out[(int64_t)o * Kp + col] = acc[m][n][2 * h + jj];
-        }
-    }
+  store_tile(acc, i0, j0, a.Co, Kp, Kp, a.part + (int64_t)blockIdx.z * a.Co * Kp);
 }
 
 // dwf[oc][j] (j < Kd) and dbias[oc] (j = Kd): the split partials summed in fp64, in split order
@@ -281,22 +233,14 @@ weight_prep_kernel(const float* __restrict__ w, int Co, int Ci, int T, int stand
   __shared__ double sh[kRedThreads];
   const int oc = blockIdx.x, n = Ci * T * T;
   const float* f = w + (int64_t)oc * n;
-  double mu = 0.0, a = 1.0;
-  if (standardize) {
-    double s = 0.0;
-    for (int i = threadIdx.x; i < n; i += kRedThreads) s += (double)f[i];
-    mu = block_sum(s, sh) / n;
-    double q = 0.0;
-    for (int i = threadIdx.x; i < n; i += kRedThreads) q += ((double)f[i] - mu) * ((double)f[i] - mu);
-    const double sd = sqrt(block_sum(q, sh) / (n - 1));
-    a = 1.0 / ((sd + 1e-5) * (double)sqrtf((float)Ci));
-  }
-  for (int i = threadIdx.x; i < n; i += kRedThreads) {
+  auto put = [&](int i, float v) {
     const int c = i / (T * T), rs = i - c * T * T;
-    const float v = standardize ? (float)(((double)f[i] - mu) * a) : f[i];
     wf[((int64_t)oc * T * T + rs) * Ci + c] = v;
     wd[T == 2 ? ((int64_t)rs * Ci + c) * Co + oc : ((int64_t)c * T * T + rs) * Co + oc] = v;
-  }
+  };
+  if (standardize) standardize_filter(f, n, Ci, sh, put);
+  else
+    for (int i = threadIdx.x; i < n; i += kRedThreads) put(i, f[i]);
 }
 
 // dw [Co][Ci][T][T] from dwf [Co][T][T][Ci], the gradient of the standardised filter
@@ -305,29 +249,9 @@ weight_prep_bwd_kernel(const float* __restrict__ w, const float* __restrict__ dw
                        float* __restrict__ dw) {
   __shared__ double sh[kRedThreads];
   const int oc = blockIdx.x, n = Ci * T * T;
-  const float* f = w + (int64_t)oc * n;
   const float* gf = dwf + (int64_t)oc * n;
   auto grad = [&](int i) { const int c = i / (T * T), rs = i - c * T * T; return (double)gf[rs * Ci + c]; };
-  double s = 0.0;
-  for (int i = threadIdx.x; i < n; i += kRedThreads) s += (double)f[i];
-  const double mu = block_sum(s, sh) / n;
-  double q = 0.0, g1 = 0.0, g2 = 0.0;
-  for (int i = threadIdx.x; i < n; i += kRedThreads) {
-    const double d = (double)f[i] - mu, gi = grad(i);
-    q += d * d;
-    g1 += gi;
-    g2 += gi * d;
-  }
-  q = block_sum(q, sh);
-  g1 = block_sum(g1, sh);
-  g2 = block_sum(g2, sh);
-  const double sd = sqrt(q / (n - 1)), den = sd + 1e-5;
-  const double a = 1.0 / (den * (double)sqrtf((float)Ci));
-  const double k2 = a / den * g2 / ((n - 1) * sd);
-  for (int i = threadIdx.x; i < n; i += kRedThreads) {
-    const double d = (double)f[i] - mu;
-    dw[(int64_t)oc * n + i] = (float)(a * (grad(i) - g1 / n) - k2 * d);
-  }
+  standardize_filter_bwd(w + (int64_t)oc * n, n, Ci, sh, grad, dw + (int64_t)oc * n);
 }
 
 __global__ void __launch_bounds__(kRedThreads)
@@ -360,15 +284,13 @@ __device__ __forceinline__ GnGrad gn_grad(float dy, float z, float mu, float is,
   return {zh, gu};
 }
 
-constexpr int kGnRows = 8;   // gn backward CTAs: 32 channels x 8 row lanes
-
 // per (image, chunk of pixels, channel): sums of gu and gu * zhat
-__global__ void __launch_bounds__(32 * kGnRows)
+__global__ void __launch_bounds__(32 * kRows)
 gn_bwd_partial_kernel(const float* __restrict__ dy, const float* __restrict__ z, int64_t P, int C, int G,
                       const float* __restrict__ mean, const float* __restrict__ invstd, const float* __restrict__ gamma,
                       const float* __restrict__ beta, float relu_scale, int64_t rows_per_chunk,
                       double2* __restrict__ part) {
-  __shared__ double2 sh[kGnRows][32];
+  __shared__ double2 sh[kRows][32];
   const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
   const int c = blockIdx.y * 32 + tx;
   const int64_t b = blockIdx.z, chunk = blockIdx.x, chunks = gridDim.x;
@@ -377,47 +299,31 @@ gn_bwd_partial_kernel(const float* __restrict__ dy, const float* __restrict__ z,
     const int64_t bg = b * G + c / (C / G);
     const float mu = mean[bg], is = invstd[bg], ga = gamma[c], be = beta[c];
     const int64_t p_end = min(P, (chunk + 1) * rows_per_chunk);
-    for (int64_t p = chunk * rows_per_chunk + ty; p < p_end; p += kGnRows) {
+    for (int64_t p = chunk * rows_per_chunk + ty; p < p_end; p += kRows) {
       const int64_t e = (b * P + p) * C + c;
       const GnGrad q = gn_grad(dy[e], z[e], mu, is, ga, be, relu_scale);
       s1 += (double)q.gu;
       s2 += (double)q.gu * (double)q.zh;
     }
   }
-  sh[ty][tx] = make_double2(s1, s2);
-  __syncthreads();
-  if (ty == 0 && c < C) {
-    for (int r = 1; r < kGnRows; ++r) {
-      s1 += sh[r][tx].x;
-      s2 += sh[r][tx].y;
-    }
-    part[(b * chunks + chunk) * C + c] = make_double2(s1, s2);
-  }
+  if (fold_rows(sh, tx, ty, c < C, s1, s2)) part[(b * chunks + chunk) * C + c] = make_double2(s1, s2);
 }
 
 // per (image, channel): the chunk partials in chunk order
-__global__ void __launch_bounds__(32 * kGnRows)
+__global__ void __launch_bounds__(32 * kRows)
 gn_bwd_sums_kernel(const double2* __restrict__ part, int64_t chunks, int C, double2* __restrict__ sums) {
-  __shared__ double2 sh[kGnRows][32];
+  __shared__ double2 sh[kRows][32];
   const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
   const int c = blockIdx.x * 32 + tx;
   const int64_t b = blockIdx.y;
   double s1 = 0.0, s2 = 0.0;
   if (c < C)
-    for (int64_t k = ty; k < chunks; k += kGnRows) {
+    for (int64_t k = ty; k < chunks; k += kRows) {
       const double2 d = part[(b * chunks + k) * C + c];
       s1 += d.x;
       s2 += d.y;
     }
-  sh[ty][tx] = make_double2(s1, s2);
-  __syncthreads();
-  if (ty == 0 && c < C) {
-    for (int r = 1; r < kGnRows; ++r) {
-      s1 += sh[r][tx].x;
-      s2 += sh[r][tx].y;
-    }
-    sums[b * C + c] = make_double2(s1, s2);
-  }
+  if (fold_rows(sh, tx, ty, c < C, s1, s2)) sums[b * C + c] = make_double2(s1, s2);
 }
 
 // dbeta, dgamma per channel (sum over images) and the per-(image, group) means of gamma * gu and gamma * gu * zhat
@@ -467,7 +373,6 @@ gn_bwd_dz_kernel(const float* __restrict__ dy, const float* __restrict__ z, int6
 
 // ---- host-side sizes
 inline int64_t out_size(int kind, int64_t n) { return kind == DVA_CONV_2X2_S2 ? n / 2 : n; }
-inline int64_t cdiv(int64_t a, int64_t b) { return (a + b - 1) / b; }
 
 inline int check_shape(const char* what, int64_t B, int64_t H, int64_t W, int Ci, int Co, int kind) {
   if (kind != DVA_CONV_3X3_REFLECT && kind != DVA_CONV_2X2_S2 && kind != DVA_CONV_1X1)
@@ -505,11 +410,9 @@ inline WgradPlan wgrad_plan(int64_t B, int64_t H, int64_t W, int Ci, int Co, int
   const int T = taps_of(kind);
   p.M = B * out_size(kind, H) * out_size(kind, W);
   p.Kd = T * T * Ci;
-  const int64_t tiles_mn = cdiv(Co, BM) * cdiv(p.Kd + 1, BN);
-  const int64_t want = std::max<int64_t>(1, cdiv(4 * kNumSMs, tiles_mn));
-  const int64_t splits = std::min<int64_t>(want, cdiv(p.M, 4 * BK));
-  p.rows_per_split = cdiv(cdiv(p.M, splits), BK) * BK;
-  p.splits = (int)cdiv(p.M, p.rows_per_split);
+  const SplitRows s = split_rows(p.M, cdiv(Co, BM) * cdiv(p.Kd + 1, BN));
+  p.rows_per_split = s.rows_per_split;
+  p.splits = s.splits;
   return p;
 }
 
@@ -530,8 +433,6 @@ template <int MODE> int launch_gemm(const GemmArgs& a, int64_t B, cudaStream_t s
   conv_gemm_kernel<MODE><<<grid, kThreads, 0, st>>>(a);
   return check_launch(what);
 }
-
-inline int elementwise_grid(int64_t n) { return grid_cap(n, kRedThreads, 8); }
 
 }  // namespace dva_conv2d
 
@@ -681,11 +582,11 @@ extern "C" int dva_conv2d_gn_bwd(const float* dy, const float* z, int64_t B, int
   double2* coef = (double2*)((uint8_t*)sums + round256((size_t)B * C * sizeof(double2)));
   cudaStream_t st = (cudaStream_t)stream;
   const int cb = (int)cdiv(C, 32);
-  gn_bwd_partial_kernel<<<dim3((unsigned)pl.chunks, cb, (unsigned)B), 32 * kGnRows, 0, st>>>(
+  gn_bwd_partial_kernel<<<dim3((unsigned)pl.chunks, cb, (unsigned)B), 32 * kRows, 0, st>>>(
       dy, z, P, C, G, mean, invstd, gamma, beta, relu_scale, pl.rows_per_chunk, part);
   int rc = check_launch("conv2d_gn_bwd_partial");
   if (rc != DVA_OK) return rc;
-  gn_bwd_sums_kernel<<<dim3(cb, (unsigned)B), 32 * kGnRows, 0, st>>>(part, pl.chunks, C, sums);
+  gn_bwd_sums_kernel<<<dim3(cb, (unsigned)B), 32 * kRows, 0, st>>>(part, pl.chunks, C, sums);
   rc = check_launch("conv2d_gn_bwd_sums");
   if (rc != DVA_OK) return rc;
   gn_bwd_coef_kernel<<<1, kRedThreads, 0, st>>>(sums, B, P, C, G, gamma, dgamma, dbeta, coef);

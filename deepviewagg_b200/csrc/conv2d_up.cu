@@ -54,8 +54,7 @@ __global__ void __launch_bounds__(kThreads) convt_gemm_kernel(ConvTArgs a) {
   __shared__ __align__(16) float smem[2 * (BM + BN) * LDS];
   __shared__ double2 colst[2][BN];
   constexpr bool kFwd = MODE == kUp2 || MODE == kFwdT3;
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int wm = warp >> 1, g = lane >> 2;
+  const int tid = threadIdx.x;
   const int64_t b = blockIdx.x / a.tiles;
   const int t = (int)(blockIdx.x - b * a.tiles);
   const int64_t P = a.Ho * a.Wo, p0 = (int64_t)t * BM;
@@ -63,12 +62,7 @@ __global__ void __launch_bounds__(kThreads) convt_gemm_kernel(ConvTArgs a) {
   const int64_t img = b * a.H * a.W;   // first source pixel of image b
   const int64_t row0 = b * P + p0;     // first GEMM row of the tile
   int oh[8], ow[8];
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    const int64_t p = p0 + (tid >> 4) + 8 * i;
-    oh[i] = p < P ? (int)(p / a.Wo) : -1;
-    ow[i] = p < P ? (int)(p - (p / a.Wo) * a.Wo) : 0;
-  }
+  tile_pixels(p0, P, a.Wo, oh, ow);
   const int H = (int)a.H, W = (int)a.W, Cs = a.Cs, K = a.K;
   auto fa = [&](int i, int row, int64_t k64) -> float {
     if (oh[i] < 0) return 0.f;
@@ -121,23 +115,8 @@ __global__ void __launch_bounds__(kThreads) convt_gemm_kernel(ConvTArgs a) {
         }
       }
   if (kFwd) {
-    // column sums over the warp's 32 rows (lanes of equal tq), then over the two row halves, then per group
-#pragma unroll
-    for (int n = 0; n < 4; ++n)
-#pragma unroll
-      for (int j = 0; j < 2; ++j)
-#pragma unroll
-        for (int o = 4; o < 32; o <<= 1) {
-          cs[n][j] += __shfl_xor_sync(0xffffffffu, cs[n][j], o);
-          cq[n][j] += __shfl_xor_sync(0xffffffffu, cq[n][j], o);
-        }
-    if (g == 0) {
-#pragma unroll
-      for (int n = 0; n < 4; ++n)
-#pragma unroll
-        for (int j = 0; j < 2; ++j) colst[wm][acc_col(n, j)] = make_double2(cs[n][j], cq[n][j]);
-    }
-    __syncthreads();
+    // column sums over the two row halves, then per group
+    column_stats(cs, cq, colst);
     // every group gets a partial (0 where the column tile has none of its columns): with kUp2 a column tile can
     // wrap around the channels
     if (tid < a.G) {
@@ -166,14 +145,7 @@ convt_stats_kernel(const double2* __restrict__ part, int tiles, int ntiles, int 
       s += d.x;
       q += d.y;
     }
-  s = block_sum(s, sh);
-  q = block_sum(q, sh);
-  if (threadIdx.x == 0) {
-    const double n = (double)n_group, mu = s / n;
-    const double var = fmax(q / n - mu * mu, 0.0);
-    mean[blockIdx.x] = (float)mu;
-    invstd[blockIdx.x] = (float)(1.0 / sqrt(var + (double)eps));
-  }
+  finish_stats(s, q, (double)n_group, eps, mean[blockIdx.x], invstd[blockIdx.x], sh);
 }
 
 struct ConvTWgradArgs {
@@ -216,16 +188,7 @@ __global__ void __launch_bounds__(kThreads) convt_wgrad_kernel(ConvTWgradArgs a)
   float acc[2][4][4];
   gemm_mainloop<true, true>(fa, fb, m_begin, m_end, smem, acc);
   const int Kp = a.Kd + 1;
-  float* out = a.part + (int64_t)blockIdx.z * a.Rw * Kp;
-#pragma unroll
-  for (int m = 0; m < 2; ++m)
-#pragma unroll
-    for (int n = 0; n < 4; ++n)
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        const int o = i0 + acc_row(m, q), col = j0 + acc_col(n, q);
-        if (o < a.Rw && col < Kp) out[(int64_t)o * Kp + col] = acc[m][n][q];
-      }
+  store_tile(acc, i0, j0, a.Rw, Kp, Kp, a.part + (int64_t)blockIdx.z * a.Rw * Kp);
 }
 
 // dwf [Rw][Kd] and dbias [Co]: the split partials summed in fp64, in split order; dbias folds the Rw / Co
@@ -262,20 +225,11 @@ convt_weight_prep_kernel(const float* __restrict__ w, int Ci, int Co, int T, flo
                          float* __restrict__ wd) {
   __shared__ double sh[kRedThreads];
   const int c = blockIdx.x, n = Co * T * T;
-  const float* f = w + (int64_t)c * n;
-  double s = 0.0;
-  for (int i = threadIdx.x; i < n; i += kRedThreads) s += (double)f[i];
-  const double mu = block_sum(s, sh) / n;
-  double q = 0.0;
-  for (int i = threadIdx.x; i < n; i += kRedThreads) q += ((double)f[i] - mu) * ((double)f[i] - mu);
-  const double sd = sqrt(block_sum(q, sh) / (n - 1));
-  const double a = 1.0 / ((sd + 1e-5) * (double)sqrtf((float)Co));
-  for (int i = threadIdx.x; i < n; i += kRedThreads) {
+  standardize_filter(w + (int64_t)c * n, n, Co, sh, [&](int i, float v) {
     const int o = i / (T * T), rs = i - o * T * T;
-    const float v = (float)(((double)f[i] - mu) * a);
     wf[wf_index(c, o, rs, Ci, Co, T)] = v;
     wd[((int64_t)c * T * T + rs) * Co + o] = v;
-  }
+  });
 }
 
 // dw [Ci][Co][T][T] from dwf (the layout of wf), the gradient of the standardised filter
@@ -284,28 +238,8 @@ convt_weight_prep_bwd_kernel(const float* __restrict__ w, const float* __restric
                              float* __restrict__ dw) {
   __shared__ double sh[kRedThreads];
   const int c = blockIdx.x, n = Co * T * T;
-  const float* f = w + (int64_t)c * n;
   auto grad = [&](int i) { const int o = i / (T * T), rs = i - o * T * T; return (double)dwf[wf_index(c, o, rs, Ci, Co, T)]; };
-  double s = 0.0;
-  for (int i = threadIdx.x; i < n; i += kRedThreads) s += (double)f[i];
-  const double mu = block_sum(s, sh) / n;
-  double q = 0.0, g1 = 0.0, g2 = 0.0;
-  for (int i = threadIdx.x; i < n; i += kRedThreads) {
-    const double d = (double)f[i] - mu, gi = grad(i);
-    q += d * d;
-    g1 += gi;
-    g2 += gi * d;
-  }
-  q = block_sum(q, sh);
-  g1 = block_sum(g1, sh);
-  g2 = block_sum(g2, sh);
-  const double sd = sqrt(q / (n - 1)), den = sd + 1e-5;
-  const double a = 1.0 / (den * (double)sqrtf((float)Co));
-  const double k2 = a / den * g2 / ((n - 1) * sd);
-  for (int i = threadIdx.x; i < n; i += kRedThreads) {
-    const double d = (double)f[i] - mu;
-    dw[(int64_t)c * n + i] = (float)(a * (grad(i) - g1 / n) - k2 * d);
-  }
+  standardize_filter_bwd(w + (int64_t)c * n, n, Co, sh, grad, dw + (int64_t)c * n);
 }
 
 __global__ void __launch_bounds__(kRedThreads)
@@ -322,8 +256,6 @@ unary_act_bwd_kernel(const float* __restrict__ dy, const float* __restrict__ z, 
 }
 
 // ---- host-side sizes
-inline int64_t cdiv(int64_t a, int64_t b) { return (a + b - 1) / b; }
-
 inline int check_shape(const char* what, int64_t B, int64_t H, int64_t W, int Ci, int Co, int kind) {
   if (kind != DVA_UNET_UP_2X2 && kind != DVA_UNET_T_3X3) return failf(DVA_EINVAL, "%s: unknown kind", what);
   if (B < 1 || H < 1 || W < 1 || Ci < 1 || Co < 1) return failf(DVA_EINVAL, "%s: bad sizes", what);
@@ -342,11 +274,9 @@ inline WgradPlan wgrad_plan(int64_t B, int64_t H, int64_t W, int Ci, int Co, int
   p.M = B * H * W;
   p.Rw = kind == DVA_UNET_UP_2X2 ? 4 * Co : Co;
   p.Kd = kind == DVA_UNET_UP_2X2 ? Ci : 9 * Ci;
-  const int64_t tiles_mn = cdiv(p.Rw, BM) * cdiv(p.Kd + 1, BN);
-  const int64_t want = std::max<int64_t>(1, cdiv(4 * kNumSMs, tiles_mn));
-  const int64_t splits = std::min<int64_t>(want, cdiv(p.M, 4 * BK));
-  p.rows_per_split = cdiv(cdiv(p.M, splits), BK) * BK;
-  p.splits = (int)cdiv(p.M, p.rows_per_split);
+  const SplitRows s = split_rows(p.M, cdiv(p.Rw, BM) * cdiv(p.Kd + 1, BN));
+  p.rows_per_split = s.rows_per_split;
+  p.splits = s.splits;
   return p;
 }
 
@@ -355,8 +285,6 @@ template <int MODE> int launch_gemm(const ConvTArgs& a, int64_t B, cudaStream_t 
   convt_gemm_kernel<MODE><<<grid, kThreads, 0, st>>>(a);
   return check_launch(what);
 }
-
-inline int elementwise_grid(int64_t n) { return grid_cap(n, kRedThreads, 8); }
 
 }  // namespace dva_unet
 

@@ -49,8 +49,7 @@ template <int MODE>
 __global__ void __launch_bounds__(kThreads) rn_conv_gemm_kernel(ConvArgs a) {
   __shared__ __align__(16) float smem[2 * (BM + BN) * LDS];
   __shared__ double2 colst[2][BN];
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int wm = warp >> 1, g = lane >> 2;
+  const int tid = threadIdx.x;
   const int64_t m0 = (int64_t)blockIdx.x * BM;
   const int n0 = blockIdx.y * BN;
   const int64_t P = (int64_t)a.Ho * a.Wo;
@@ -111,23 +110,8 @@ __global__ void __launch_bounds__(kThreads) rn_conv_gemm_kernel(ConvArgs a) {
         }
       }
   if (MODE == kFwd && a.part) {
-    // column sums over the warp's 32 rows (lanes of equal tq), then over the two row halves
-#pragma unroll
-    for (int n = 0; n < 4; ++n)
-#pragma unroll
-      for (int j = 0; j < 2; ++j)
-#pragma unroll
-        for (int o = 4; o < 32; o <<= 1) {
-          cs[n][j] += __shfl_xor_sync(0xffffffffu, cs[n][j], o);
-          cq[n][j] += __shfl_xor_sync(0xffffffffu, cq[n][j], o);
-        }
-    if (g == 0) {
-#pragma unroll
-      for (int n = 0; n < 4; ++n)
-#pragma unroll
-        for (int j = 0; j < 2; ++j) colst[wm][acc_col(n, j)] = make_double2(cs[n][j], cq[n][j]);
-    }
-    __syncthreads();
+    // column sums over the two row halves
+    column_stats(cs, cq, colst);
     if (tid < BN && n0 + tid < a.N)
       a.part[(int64_t)(n0 + tid) * a.tiles + blockIdx.x] =
           make_double2(colst[0][tid].x + colst[1][tid].x, colst[0][tid].y + colst[1][tid].y);
@@ -154,16 +138,12 @@ rn_bn_stats_kernel(const double2* __restrict__ part, int tiles, int64_t n, int t
     s += d.x;
     q += d.y;
   }
-  s = block_sum(s, sh);
-  q = block_sum(q, sh);
+  const double nn = (double)n;
+  const double2 st = finish_stats(s, q, nn, eps, mean[c], invstd[c], sh);
   if (threadIdx.x == 0) {
-    const double nn = (double)n, mu = s / nn;
-    const double var = fmax(q / nn - mu * mu, 0.0);
-    mean[c] = (float)mu;
-    invstd[c] = (float)(1.0 / sqrt(var + (double)eps));
     const double mo = (double)momentum;
-    running_mean[c] = (float)((1.0 - mo) * (double)running_mean[c] + mo * mu);
-    running_var[c] = (float)((1.0 - mo) * (double)running_var[c] + mo * var * nn / (nn - 1.0));
+    running_mean[c] = (float)((1.0 - mo) * (double)running_mean[c] + mo * st.x);
+    running_var[c] = (float)((1.0 - mo) * (double)running_var[c] + mo * st.y * nn / (nn - 1.0));
   }
 }
 
@@ -195,16 +175,7 @@ __global__ void __launch_bounds__(kThreads) rn_conv_wgrad_kernel(WgradArgs a) {
   };
   float acc[2][4][4];
   gemm_mainloop<true, true>(fa, fb, m_begin, m_end, smem, acc);
-  float* out = a.part + (int64_t)blockIdx.z * a.Co * a.Kd;
-#pragma unroll
-  for (int m = 0; m < 2; ++m)
-#pragma unroll
-    for (int n = 0; n < 4; ++n)
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        const int o = i0 + acc_row(m, q), col = j0 + acc_col(n, q);
-        if (o < a.Co && col < a.Kd) out[(int64_t)o * a.Kd + col] = acc[m][n][q];
-      }
+  store_tile(acc, i0, j0, a.Co, a.Kd, a.Kd, a.part + (int64_t)blockIdx.z * a.Co * a.Kd);
 }
 
 // dw [Co][Ci][T][T]: the split partials [splits][Co][(r * T + s) * Ci + c] summed in fp64, in split order
@@ -252,16 +223,14 @@ rn_bn_apply_kernel(const float* __restrict__ z, int C, const float* __restrict__
   }
 }
 
-constexpr int kBnRows = 8;   // BatchNorm backward CTAs: 32 channels x 8 row lanes
-
 __device__ __forceinline__ float masked(float dy, float y) { return y > 0.f ? dy : 0.f; }
 
 // per (chunk of pixels, channel): sums of g and g * zhat
-__global__ void __launch_bounds__(32 * kBnRows)
+__global__ void __launch_bounds__(32 * kRows)
 rn_bn_bwd_partial_kernel(const float* __restrict__ dy, const float* __restrict__ y, const float* __restrict__ z,
                          int64_t M, int C, const float* __restrict__ mean, const float* __restrict__ invstd,
                          int64_t rows_per_chunk, double2* __restrict__ part) {
-  __shared__ double2 sh[kBnRows][32];
+  __shared__ double2 sh[kRows][32];
   const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
   const int c = blockIdx.y * 32 + tx;
   const int64_t chunk = blockIdx.x;
@@ -269,45 +238,31 @@ rn_bn_bwd_partial_kernel(const float* __restrict__ dy, const float* __restrict__
   if (c < C) {
     const float mu = mean[c], is = invstd[c];
     const int64_t m_end = min(M, (chunk + 1) * rows_per_chunk);
-    for (int64_t m = chunk * rows_per_chunk + ty; m < m_end; m += kBnRows) {
+    for (int64_t m = chunk * rows_per_chunk + ty; m < m_end; m += kRows) {
       const int64_t e = m * C + c;
       const float gv = masked(dy[e], y[e]);
       s1 += (double)gv;
       s2 += (double)gv * (double)((z[e] - mu) * is);
     }
   }
-  sh[ty][tx] = make_double2(s1, s2);
-  __syncthreads();
-  if (ty == 0 && c < C) {
-    for (int r = 1; r < kBnRows; ++r) {
-      s1 += sh[r][tx].x;
-      s2 += sh[r][tx].y;
-    }
-    part[chunk * C + c] = make_double2(s1, s2);
-  }
+  if (fold_rows(sh, tx, ty, c < C, s1, s2)) part[chunk * C + c] = make_double2(s1, s2);
 }
 
 // per channel: the chunk partials in chunk order -> dbeta, dgamma and the means of g and g * zhat (training)
-__global__ void __launch_bounds__(32 * kBnRows)
+__global__ void __launch_bounds__(32 * kRows)
 rn_bn_bwd_reduce_kernel(const double2* __restrict__ part, int64_t chunks, int C, int64_t M, int training,
                         float* __restrict__ dgamma, float* __restrict__ dbeta, double2* __restrict__ coef) {
-  __shared__ double2 sh[kBnRows][32];
+  __shared__ double2 sh[kRows][32];
   const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
   const int c = blockIdx.x * 32 + tx;
   double s1 = 0.0, s2 = 0.0;
   if (c < C)
-    for (int64_t k = ty; k < chunks; k += kBnRows) {
+    for (int64_t k = ty; k < chunks; k += kRows) {
       const double2 d = part[k * C + c];
       s1 += d.x;
       s2 += d.y;
     }
-  sh[ty][tx] = make_double2(s1, s2);
-  __syncthreads();
-  if (ty == 0 && c < C) {
-    for (int r = 1; r < kBnRows; ++r) {
-      s1 += sh[r][tx].x;
-      s2 += sh[r][tx].y;
-    }
+  if (fold_rows(sh, tx, ty, c < C, s1, s2)) {
     dbeta[c] = (float)s1;
     dgamma[c] = (float)s2;
     coef[c] = training ? make_double2(s1 / (double)M, s2 / (double)M) : make_double2(0.0, 0.0);
@@ -471,7 +426,6 @@ rn_resize_bwd_kernel(const float* __restrict__ dy, int64_t ldy, int64_t col0, in
 }
 
 // ---- host-side sizes
-inline int64_t cdiv(int64_t a, int64_t b) { return (a + b - 1) / b; }
 inline int64_t out_size(int64_t n, int stride) { return (n - 1) / stride + 1; }
 inline int pad_of(int T, int dil) { return T == 3 ? dil : 0; }
 
@@ -494,11 +448,9 @@ inline WgradPlan wgrad_plan(int64_t B, int64_t H, int64_t W, int Ci, int Co, int
   WgradPlan p;
   p.M = B * out_size(H, stride) * out_size(W, stride);
   p.Kd = T * T * Ci;
-  const int64_t tiles_mn = cdiv(Co, BM) * cdiv(p.Kd, BN);
-  const int64_t want = std::max<int64_t>(1, cdiv(4 * kNumSMs, tiles_mn));
-  const int64_t splits = std::min<int64_t>(want, cdiv(p.M, 4 * BK));
-  p.rows_per_split = cdiv(cdiv(p.M, splits), BK) * BK;
-  p.splits = (int)cdiv(p.M, p.rows_per_split);
+  const SplitRows s = split_rows(p.M, cdiv(Co, BM) * cdiv(p.Kd, BN));
+  p.rows_per_split = s.rows_per_split;
+  p.splits = s.splits;
   return p;
 }
 
@@ -513,8 +465,6 @@ inline BnPlan bn_plan(int64_t M, int C) {
   p.chunks = cdiv(M, p.rows_per_chunk);
   return p;
 }
-
-inline int elementwise_grid(int64_t n) { return grid_cap(n, kRedThreads, 8); }
 
 }  // namespace dva_resnet
 
@@ -636,11 +586,11 @@ extern "C" int dva_resnet_bn_bwd(const float* dy, const float* y, const float* z
   double2* coef = (double2*)((uint8_t*)ws + round256((size_t)pl.chunks * C * sizeof(double2)));
   cudaStream_t st = (cudaStream_t)stream;
   const int cb = (int)cdiv(C, 32);
-  rn_bn_bwd_partial_kernel<<<dim3((unsigned)pl.chunks, cb), 32 * kBnRows, 0, st>>>(dy, y, z, M, C, mean, invstd,
+  rn_bn_bwd_partial_kernel<<<dim3((unsigned)pl.chunks, cb), 32 * kRows, 0, st>>>(dy, y, z, M, C, mean, invstd,
                                                                                    pl.rows_per_chunk, part);
   int rc = check_launch("resnet_bn_bwd_partial");
   if (rc != DVA_OK) return rc;
-  rn_bn_bwd_reduce_kernel<<<cb, 32 * kBnRows, 0, st>>>(part, pl.chunks, C, M, training, dgamma, dbeta, coef);
+  rn_bn_bwd_reduce_kernel<<<cb, 32 * kRows, 0, st>>>(part, pl.chunks, C, M, training, dgamma, dbeta, coef);
   rc = check_launch("resnet_bn_bwd_reduce");
   if (rc != DVA_OK) return rc;
   const int64_t n = M * C;

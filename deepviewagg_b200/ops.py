@@ -6,6 +6,7 @@ libdva_b200.so: CPU tensors or a missing library raise.  Reference citations are
 reference repository root.
 """
 import contextlib
+import dataclasses
 import math
 import os
 
@@ -1509,11 +1510,11 @@ def _f32(*ts):
     return [None if t is None else t.detach().float().contiguous() for t in ts]
 
 
-def _encoder_input(x, weight):
-    """x as the kernels read it: channels-last rows [B, H, W, C_in], fp32, contiguous (a copy for any other dtype
-    or layout; outside autocast custom_fwd casts nothing)."""
-    if x.dim() != 4 or x.shape[3] != weight.shape[1]:
-        raise ValueError(f"expected channels-last rows [B, H, W, {weight.shape[1]}], got shape {tuple(x.shape)}")
+def _rows_input(x, c_in):
+    """x as the image kernels read it: channels-last rows [B, H, W, c_in], fp32, contiguous (a copy for any other
+    dtype or layout; outside autocast custom_fwd casts nothing)."""
+    if x.dim() != 4 or x.shape[3] != c_in:
+        raise ValueError(f"expected channels-last rows [B, H, W, {c_in}], got shape {tuple(x.shape)}")
     if not x.is_floating_point():
         raise TypeError(f"expected a floating-point feature map, got {x.dtype}")
     return x.float().contiguous()
@@ -1524,21 +1525,43 @@ def _as_dtypes(grads, dtypes):
     return tuple(None if g is None else g.to(d) for g, d in zip(grads, dtypes))
 
 
+@dataclasses.dataclass(frozen=True)
+class _ConvFamily:
+    """The weight-standardised convolutions of one half of the from-scratch image network, as _ConvGNAct and
+    _ResBlock call them: k3 is the kind of its 3x3 convolution; weights(w, kind) -> (wf, wd); fwd(x, wf, bias, C_out,
+    kind, G, eps) -> (z, mean, invstd); wgrad(dz, x, kind) -> (dwf, dbias); dgrad(dz, x_shape, wd, kind, add=None,
+    out=None) -> dx; weight_grad(w, dwf, kind) -> dw; c_in / c_out are the weight dimensions of the input / output
+    channels.  (Not a tuple: custom_fwd would rebuild a tuple argument from a generator.)"""
+    k3: int
+    weights: object
+    fwd: object
+    wgrad: object
+    dgrad: object
+    weight_grad: object
+    c_in: int
+    c_out: int
+
+
+# the encoder's Conv2dWS: reflect padding, w [C_out][C_in][R][S]
+_ENCODER = _ConvFamily(_lib.DVA_CONV_3X3_REFLECT, lambda w, kind: _conv_weights(w, kind, True), _conv_fwd, _wgrad,
+                       _dgrad, lambda w, dwf, kind: _weight_grad(w, dwf, kind, True), 1, 0)
+
+
 class _ConvGNAct(torch.autograd.Function):
-    """ReLUWS(GroupNorm(Conv2dWS(x))), ResNetDown.conv_in (image.py:302-312), as one node.  Saves x, z and the
-    per-(image, group) statistics."""
+    """ReLUWS(GroupNorm(conv(x))) as one node, conv a Conv2dWS (ResNetDown.conv_in, image.py:302-312) or a
+    ConvTranspose2dWS (ResNetUp.conv_in) of family `fam`.  Saves x, z and the per-(image, group) statistics."""
 
     @staticmethod
     @_fwd_f32
-    def forward(ctx, x, weight, bias, gamma, beta, kind, G, eps):
+    def forward(ctx, x, weight, bias, gamma, beta, kind, G, eps, fam):
         require_cuda(x, weight, bias, gamma, beta)
         ctx.dtypes = [t.dtype for t in (x, weight, bias, gamma, beta)]
-        x = _encoder_input(x, weight)
+        x = _rows_input(x, weight.shape[fam.c_in])
         w, b, g, be = _f32(weight, bias, gamma, beta)
-        wf, wd = _conv_weights(w, kind, True)
-        z, mean, invstd = _conv_fwd(x, wf, b, w.shape[0], kind, G, eps)
+        wf, wd = fam.weights(w, kind)
+        z, mean, invstd = fam.fwd(x, wf, b, w.shape[fam.c_out], kind, G, eps)
         ctx.save_for_backward(x, w, wd, g, be, z, mean, invstd)
-        ctx.cfg = (kind, G)
+        ctx.cfg = (kind, G, fam)
         return _gn_apply(z, (G, mean, invstd, g, be), True)
 
     @staticmethod
@@ -1546,32 +1569,34 @@ class _ConvGNAct(torch.autograd.Function):
     @torch.autograd.function.once_differentiable
     def backward(ctx, dy):
         x, w, wd, g, be, z, mean, invstd = ctx.saved_tensors
-        kind, G = ctx.cfg
+        kind, G, fam = ctx.cfg
         dz, dg, dbe = _gn_bwd(dy.float().contiguous(), z, (G, mean, invstd, g, be), True)
-        dwf, db = _wgrad(dz, x, kind)
-        dx = _dgrad(dz, x.shape, wd, kind) if ctx.needs_input_grad[0] else None
-        return (*_as_dtypes((dx, _weight_grad(w, dwf, kind, True), db, dg, dbe), ctx.dtypes), None, None, None)
+        dwf, db = fam.wgrad(dz, x, kind)
+        dx = fam.dgrad(dz, x.shape, wd, kind) if ctx.needs_input_grad[0] else None
+        return (*_as_dtypes((dx, fam.weight_grad(w, dwf, kind), db, dg, dbe), ctx.dtypes), None, None, None, None)
 
 
 class _ResBlock(torch.autograd.Function):
     """ResBlock (image.py:128-189) as one node: h = ReLUWS(GN1(conv1(x))), y = ReLUWS(GN2(conv2(h))) + skip, skip =
-    x or GN_ds(conv1x1(x)), the residual added after the second activation.  Saves x, z1, z2, z_ds and the
+    x or GN_ds(conv1x1(x)), the residual added after the second activation.  conv1 and conv2 are the 3x3
+    convolutions of family `fam` (Conv2dWS, or ConvTranspose2dWS with stride 1 and zero padding 1); the 1x1
+    downsample is a plain nn.Conv2d with bias on libdva_conv2d.so either way.  Saves x, z1, z2, z_ds and the
     statistics; h is recomputed in the backward."""
 
     @staticmethod
     @_fwd_f32
-    def forward(ctx, x, w1, b1, g1, be1, w2, b2, g2, be2, wd, bd, gd, bed, cfg):
+    def forward(ctx, x, w1, b1, g1, be1, w2, b2, g2, be2, wd, bd, gd, bed, cfg, fam):
         require_cuda(x, w1, b1, g1, be1, w2, b2, g2, be2, wd, bd, gd, bed)
         (G1, eps1), (G2, eps2), (Gd, epsd) = cfg
         ctx.dtypes = [None if t is None else t.dtype for t in (x, w1, b1, g1, be1, w2, b2, g2, be2, wd, bd, gd, bed)]
-        x = _encoder_input(x, w1)
+        x = _rows_input(x, w1.shape[fam.c_in])
         w1, b1, g1, be1, w2, b2, g2, be2, wd, bd, gd, bed = _f32(w1, b1, g1, be1, w2, b2, g2, be2, wd, bd, gd, bed)
-        k3 = _lib.DVA_CONV_3X3_REFLECT
-        wf1, wd1 = _conv_weights(w1, k3, True)
-        z1, m1, i1 = _conv_fwd(x, wf1, b1, w1.shape[0], k3, G1, eps1)
+        k3 = fam.k3
+        wf1, wd1 = fam.weights(w1, k3)
+        z1, m1, i1 = fam.fwd(x, wf1, b1, w1.shape[fam.c_out], k3, G1, eps1)
         h = _gn_apply(z1, (G1, m1, i1, g1, be1), True)
-        wf2, wd2 = _conv_weights(w2, k3, True)
-        z2, m2, i2 = _conv_fwd(h, wf2, b2, w2.shape[0], k3, G2, eps2)
+        wf2, wd2 = fam.weights(w2, k3)
+        z2, m2, i2 = fam.fwd(h, wf2, b2, w2.shape[fam.c_out], k3, G2, eps2)
         del h
         ds = None
         wdd = zd = md = idd = None
@@ -1582,7 +1607,7 @@ class _ResBlock(torch.autograd.Function):
         y = _gn_apply(z2, (G2, m2, i2, g2, be2), True, skip=x if ds is None else None, ds=ds)
         ctx.save_for_backward(x, w1, wd1, g1, be1, z1, m1, i1, w2, wd2, g2, be2, z2, m2, i2, wd, wdd, gd, bed, zd,
                               md, idd)
-        ctx.cfg = cfg
+        ctx.cfg = (cfg, fam)
         return y
 
     @staticmethod
@@ -1591,18 +1616,18 @@ class _ResBlock(torch.autograd.Function):
     def backward(ctx, dy):
         (x, w1, wd1, g1, be1, z1, m1, i1, w2, wd2, g2, be2, z2, m2, i2, wd, wdd, gd, bed, zd, md,
          idd) = ctx.saved_tensors
-        (G1, _), (G2, _), (Gd, _) = ctx.cfg
-        k3, k1 = _lib.DVA_CONV_3X3_REFLECT, _lib.DVA_CONV_1X1
+        ((G1, _), (G2, _), (Gd, _)), fam = ctx.cfg
+        k3, k1 = fam.k3, _lib.DVA_CONV_1X1
         dy = dy.float().contiguous()
         gn1, gn2 = (G1, m1, i1, g1, be1), (G2, m2, i2, g2, be2)
         dz2, dg2, dbe2 = _gn_bwd(dy, z2, gn2, True)
         h = _gn_apply(z1, gn1, True)
-        dwf2, db2 = _wgrad(dz2, h, k3)
-        dh = _dgrad(dz2, h.shape, wd2, k3)
+        dwf2, db2 = fam.wgrad(dz2, h, k3)
+        dh = fam.dgrad(dz2, h.shape, wd2, k3)
         del h
         dz1, dg1, dbe1 = _gn_bwd(dh, z1, gn1, True)
         del dh
-        dwf1, db1 = _wgrad(dz1, x, k3)
+        dwf1, db1 = fam.wgrad(dz1, x, k3)
         grads_ds = (None,) * 4
         dx = None
         if wd is not None:
@@ -1612,29 +1637,35 @@ class _ResBlock(torch.autograd.Function):
             if ctx.needs_input_grad[0]:
                 dx = _dgrad(dzd, x.shape, wdd, k1)
         if ctx.needs_input_grad[0]:
-            dx = _dgrad(dz1, x.shape, wd1, k3, add=dy if dx is None else dx, out=dx)
-        grads = (dx, _weight_grad(w1, dwf1, k3, True), db1, dg1, dbe1, _weight_grad(w2, dwf2, k3, True), db2, dg2,
-                 dbe2, *grads_ds)
-        return (*_as_dtypes(grads, ctx.dtypes), None)
+            dx = fam.dgrad(dz1, x.shape, wd1, k3, add=dy if dx is None else dx, out=dx)
+        grads = (dx, fam.weight_grad(w1, dwf1, k3), db1, dg1, dbe1, fam.weight_grad(w2, dwf2, k3), db2, dg2, dbe2,
+                 *grads_ds)
+        return (*_as_dtypes(grads, ctx.dtypes), None, None)
 
 
-def conv_gn_relu_ws(x, conv, norm, kind):
-    """ReLUWS(norm(conv(x))) for channels-last x [B, H, W, C_in] (conv a Conv2dWS, norm an nn.GroupNorm): fp32
-    [B, H', W', C_out], computed from fp32 operands whatever the dtype and layout of x."""
-    return _ConvGNAct.apply(x, conv.weight, conv.bias, norm.weight, norm.bias, kind, norm.num_groups, norm.eps)
-
-
-def res_block(x, block):
-    """A ResBlock on channels-last x [B, H, W, C_in]: fp32 [B, H, W, C_out], computed from fp32 operands whatever the
-    dtype and layout of x."""
+def _res_block_args(block):
+    """The tensors and GroupNorm (num_groups, eps) of a ResBlock, in the order _ResBlock.forward takes them."""
     c1, n1, _, c2, n2, _ = block.block
     ds = block.downsample
     cd, nd = (ds[0], ds[1]) if ds is not None else (None, None)
     cfg = ((n1.num_groups, n1.eps), (n2.num_groups, n2.eps),
            (nd.num_groups, nd.eps) if nd is not None else (1, 1e-5))
-    return _ResBlock.apply(x, c1.weight, c1.bias, n1.weight, n1.bias, c2.weight, c2.bias, n2.weight, n2.bias,
-                           cd.weight if cd is not None else None, cd.bias if cd is not None else None,
-                           nd.weight if nd is not None else None, nd.bias if nd is not None else None, cfg)
+    return (c1.weight, c1.bias, n1.weight, n1.bias, c2.weight, c2.bias, n2.weight, n2.bias,
+            cd.weight if cd is not None else None, cd.bias if cd is not None else None,
+            nd.weight if nd is not None else None, nd.bias if nd is not None else None, cfg)
+
+
+def conv_gn_relu_ws(x, conv, norm, kind):
+    """ReLUWS(norm(conv(x))) for channels-last x [B, H, W, C_in] (conv a Conv2dWS, norm an nn.GroupNorm): fp32
+    [B, H', W', C_out], computed from fp32 operands whatever the dtype and layout of x."""
+    return _ConvGNAct.apply(x, conv.weight, conv.bias, norm.weight, norm.bias, kind, norm.num_groups, norm.eps,
+                            _ENCODER)
+
+
+def res_block(x, block):
+    """A ResBlock on channels-last x [B, H, W, C_in]: fp32 [B, H, W, C_out], computed from fp32 operands whatever the
+    dtype and layout of x."""
+    return _ResBlock.apply(x, *_res_block_args(block), _ENCODER)
 
 
 # --------------------------------------------------------------------------------------------
@@ -1700,107 +1731,9 @@ def _convt_dgrad(dz, x_shape, wd, kind, add=None, out=None):
     return dx
 
 
-def _decoder_input(x, c_in):
-    """x as the kernels read it: channels-last rows [B, H, W, c_in], fp32, contiguous."""
-    if x.dim() != 4 or x.shape[3] != c_in:
-        raise ValueError(f"expected channels-last rows [B, H, W, {c_in}], got shape {tuple(x.shape)}")
-    if not x.is_floating_point():
-        raise TypeError(f"expected a floating-point feature map, got {x.dtype}")
-    return x.float().contiguous()
-
-
-class _ConvTGNAct(torch.autograd.Function):
-    """ReLUWS(GroupNorm(ConvTranspose2dWS(x))), ResNetUp.conv_in, as one node.  Saves x, z and the per-(image,
-    group) statistics."""
-
-    @staticmethod
-    @_fwd_f32
-    def forward(ctx, x, weight, bias, gamma, beta, kind, G, eps):
-        require_cuda(x, weight, bias, gamma, beta)
-        ctx.dtypes = [t.dtype for t in (x, weight, bias, gamma, beta)]
-        x = _decoder_input(x, weight.shape[0])
-        w, b, g, be = _f32(weight, bias, gamma, beta)
-        wf, wd = _convt_weights(w, kind)
-        z, mean, invstd = _convt_fwd(x, wf, b, w.shape[1], kind, G, eps)
-        ctx.save_for_backward(x, w, wd, g, be, z, mean, invstd)
-        ctx.cfg = (kind, G)
-        return _gn_apply(z, (G, mean, invstd, g, be), True)
-
-    @staticmethod
-    @_bwd
-    @torch.autograd.function.once_differentiable
-    def backward(ctx, dy):
-        x, w, wd, g, be, z, mean, invstd = ctx.saved_tensors
-        kind, G = ctx.cfg
-        dz, dg, dbe = _gn_bwd(dy.float().contiguous(), z, (G, mean, invstd, g, be), True)
-        dwf, db = _convt_wgrad(dz, x, kind)
-        dx = _convt_dgrad(dz, x.shape, wd, kind) if ctx.needs_input_grad[0] else None
-        return (*_as_dtypes((dx, _convt_weight_grad(w, dwf, kind), db, dg, dbe), ctx.dtypes), None, None, None)
-
-
-class _ResBlockT(torch.autograd.Function):
-    """A ResBlock of ConvTranspose2dWS (3x3, stride 1, zero padding 1) as one node: h = ReLUWS(GN1(convT1(x))),
-    y = ReLUWS(GN2(convT2(h))) + skip, skip = x or GN_ds(conv1x1(x)) (a plain nn.Conv2d with bias).  Saves x, z1,
-    z2, z_ds and the statistics; h is recomputed in the backward."""
-
-    @staticmethod
-    @_fwd_f32
-    def forward(ctx, x, w1, b1, g1, be1, w2, b2, g2, be2, wd, bd, gd, bed, cfg):
-        require_cuda(x, w1, b1, g1, be1, w2, b2, g2, be2, wd, bd, gd, bed)
-        (G1, eps1), (G2, eps2), (Gd, epsd) = cfg
-        ctx.dtypes = [None if t is None else t.dtype for t in (x, w1, b1, g1, be1, w2, b2, g2, be2, wd, bd, gd, bed)]
-        x = _decoder_input(x, w1.shape[0])
-        w1, b1, g1, be1, w2, b2, g2, be2, wd, bd, gd, bed = _f32(w1, b1, g1, be1, w2, b2, g2, be2, wd, bd, gd, bed)
-        k3 = _lib.DVA_UNET_T_3X3
-        wf1, wd1 = _convt_weights(w1, k3)
-        z1, m1, i1 = _convt_fwd(x, wf1, b1, w1.shape[1], k3, G1, eps1)
-        h = _gn_apply(z1, (G1, m1, i1, g1, be1), True)
-        wf2, wd2 = _convt_weights(w2, k3)
-        z2, m2, i2 = _convt_fwd(h, wf2, b2, w2.shape[1], k3, G2, eps2)
-        del h
-        ds = None
-        wdd = zd = md = idd = None
-        if wd is not None:
-            wfd, wdd = _conv_weights(wd, _lib.DVA_CONV_1X1, False)
-            zd, md, idd = _conv_fwd(x, wfd, bd, wd.shape[0], _lib.DVA_CONV_1X1, Gd, epsd)
-            ds = (zd, Gd, md, idd, gd, bed)
-        y = _gn_apply(z2, (G2, m2, i2, g2, be2), True, skip=x if ds is None else None, ds=ds)
-        ctx.save_for_backward(x, w1, wd1, g1, be1, z1, m1, i1, w2, wd2, g2, be2, z2, m2, i2, wd, wdd, gd, bed, zd,
-                              md, idd)
-        ctx.cfg = cfg
-        return y
-
-    @staticmethod
-    @_bwd
-    @torch.autograd.function.once_differentiable
-    def backward(ctx, dy):
-        (x, w1, wd1, g1, be1, z1, m1, i1, w2, wd2, g2, be2, z2, m2, i2, wd, wdd, gd, bed, zd, md,
-         idd) = ctx.saved_tensors
-        (G1, _), (G2, _), (Gd, _) = ctx.cfg
-        k3, k1 = _lib.DVA_UNET_T_3X3, _lib.DVA_CONV_1X1
-        dy = dy.float().contiguous()
-        gn1, gn2 = (G1, m1, i1, g1, be1), (G2, m2, i2, g2, be2)
-        dz2, dg2, dbe2 = _gn_bwd(dy, z2, gn2, True)
-        h = _gn_apply(z1, gn1, True)
-        dwf2, db2 = _convt_wgrad(dz2, h, k3)
-        dh = _convt_dgrad(dz2, h.shape, wd2, k3)
-        del h
-        dz1, dg1, dbe1 = _gn_bwd(dh, z1, gn1, True)
-        del dh
-        dwf1, db1 = _convt_wgrad(dz1, x, k3)
-        grads_ds = (None,) * 4
-        dx = None
-        if wd is not None:
-            dzd, dgd, dbed = _gn_bwd(dy, zd, (Gd, md, idd, gd, bed), False)
-            dwfd, dbd = _wgrad(dzd, x, k1)
-            grads_ds = (_weight_grad(wd, dwfd, k1, False), dbd, dgd, dbed)
-            if ctx.needs_input_grad[0]:
-                dx = _dgrad(dzd, x.shape, wdd, k1)
-        if ctx.needs_input_grad[0]:
-            dx = _convt_dgrad(dz1, x.shape, wd1, k3, add=dy if dx is None else dx, out=dx)
-        grads = (dx, _convt_weight_grad(w1, dwf1, k3), db1, dg1, dbe1, _convt_weight_grad(w2, dwf2, k3), db2, dg2,
-                 dbe2, *grads_ds)
-        return (*_as_dtypes(grads, ctx.dtypes), None)
+# the decoder's ConvTranspose2dWS: zero padding, transposed weights w [C_in][C_out][R][S]
+_DECODER = _ConvFamily(_lib.DVA_UNET_T_3X3, _convt_weights, _convt_fwd, _convt_wgrad, _convt_dgrad,
+                       _convt_weight_grad, 0, 1)
 
 
 class _UnaryConv(torch.autograd.Function):
@@ -1812,7 +1745,7 @@ class _UnaryConv(torch.autograd.Function):
     def forward(ctx, x, weight, bias, standardize, scale):
         require_cuda(x, weight, bias)
         ctx.dtypes = [t.dtype for t in (x, weight, bias)]
-        x = _encoder_input(x, weight)
+        x = _rows_input(x, weight.shape[1])
         w, b = _f32(weight, bias)
         k1 = _lib.DVA_CONV_1X1
         wf, wd = _conv_weights(w, k1, standardize)
@@ -1845,20 +1778,14 @@ class _UnaryConv(torch.autograd.Function):
 def convt_gn_relu_ws(x, conv, norm, kind):
     """ReLUWS(norm(conv(x))) for channels-last x [B, H, W, C_in] (conv a ConvTranspose2dWS, norm an nn.GroupNorm):
     fp32 [B, H', W', C_out], computed from fp32 operands whatever the dtype and layout of x."""
-    return _ConvTGNAct.apply(x, conv.weight, conv.bias, norm.weight, norm.bias, kind, norm.num_groups, norm.eps)
+    return _ConvGNAct.apply(x, conv.weight, conv.bias, norm.weight, norm.bias, kind, norm.num_groups, norm.eps,
+                            _DECODER)
 
 
 def res_block_t(x, block):
     """A ResBlock of ConvTranspose2dWS on channels-last x [B, H, W, C_in]: fp32 [B, H, W, C_out], computed from fp32
     operands whatever the dtype and layout of x."""
-    c1, n1, _, c2, n2, _ = block.block
-    ds = block.downsample
-    cd, nd = (ds[0], ds[1]) if ds is not None else (None, None)
-    cfg = ((n1.num_groups, n1.eps), (n2.num_groups, n2.eps),
-           (nd.num_groups, nd.eps) if nd is not None else (1, 1e-5))
-    return _ResBlockT.apply(x, c1.weight, c1.bias, n1.weight, n1.bias, c2.weight, c2.bias, n2.weight, n2.bias,
-                            cd.weight if cd is not None else None, cd.bias if cd is not None else None,
-                            nd.weight if nd is not None else None, nd.bias if nd is not None else None, cfg)
+    return _ResBlock.apply(x, *_res_block_args(block), _DECODER)
 
 
 def unary_conv(x, conv, standardize, scale):
@@ -1956,14 +1883,6 @@ def _rn_dgrad(dz, x_shape, wd, geo, add=None, out=None):
     return dx
 
 
-def _rn_input(x, c_in):
-    if x.dim() != 4 or x.shape[3] != c_in:
-        raise ValueError(f"expected channels-last rows [B, H, W, {c_in}], got shape {tuple(x.shape)}")
-    if not x.is_floating_point():
-        raise TypeError(f"expected a floating-point feature map, got {x.dtype}")
-    return x.float().contiguous()
-
-
 def _bn_cfg(bn):
     return (bn.training, bn.momentum, bn.eps)
 
@@ -1977,7 +1896,7 @@ class _RNConvBNReLU(torch.autograd.Function):
     def forward(ctx, x, weight, gamma, beta, running_mean, running_var, geo, bn_cfg):
         require_cuda(x, weight, gamma, beta)
         ctx.dtypes = [t.dtype for t in (x, weight, gamma, beta)]
-        x = _rn_input(x, weight.shape[1])
+        x = _rows_input(x, weight.shape[1])
         w, g, b = _f32(weight, gamma, beta)
         training, momentum, eps = bn_cfg
         wf, wd = _rn_weights(w)
@@ -2009,7 +1928,7 @@ class _RNBasicBlock(torch.autograd.Function):
         require_cuda(x, w1, g1, b1, w2, g2, b2, wd, gd, bd)
         (stride, dil1, dil2), bn1, bn2, bnd = cfg
         ctx.dtypes = [None if t is None else t.dtype for t in (x, w1, g1, b1, w2, g2, b2, wd, gd, bd)]
-        x = _rn_input(x, w1.shape[1])
+        x = _rows_input(x, w1.shape[1])
         w1, g1, b1, w2, g2, b2, wd, gd, bd = _f32(w1, g1, b1, w2, g2, b2, wd, gd, bd)
         geo1, geo2, geod = (3, stride, dil1), (3, 1, dil2), (1, stride, 1)
         wf1, wd1 = _rn_weights(w1)
