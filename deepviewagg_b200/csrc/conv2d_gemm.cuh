@@ -147,7 +147,8 @@ __device__ __forceinline__ void standardize_filter_bwd(const float* f, int n, in
   g2 = block_sum(g2, sh);
   const double sd = sqrt(q / (n - 1)), den = sd + 1e-5;
   const double a = 1.0 / (den * (double)sqrtf((float)fan));
-  const double k2 = a / den * g2 / ((n - 1) * sd);
+  // a filter of equal weights (q = 0, so g2 = 0 and sd = 0) has no std term: torch's std backward masks std == 0
+  const double k2 = q > 0.0 ? a / den * g2 / ((n - 1) * sd) : 0.0;
   for (int i = threadIdx.x; i < n; i += kRedThreads) {
     const double d = (double)f[i] - mu;
     df[i] = (float)(a * (grad(i) - g1 / n) - k2 * d);
