@@ -557,16 +557,28 @@ view_attention_bwd_kernel(const VAParams P) {
   }
 }
 
-// one warp per output (2G <= 64 outputs): lanes stride over the CTA partials in a fixed order
-__global__ void gate_reduce_kernel(const float* __restrict__ partial, float* __restrict__ out,
-                                   int blocks, int twoG) {
-  const int lane = threadIdx.x & 31;
-  for (int j = threadIdx.x >> 5; j < twoG; j += blockDim.x >> 5) {
-    float acc = 0.f;
-    for (int b = lane; b < blocks; b += 32) acc += partial[(int64_t)b * twoG + j];
+// one CTA per output j (2G <= 64 outputs) over the partials b = 0 .. count - 1, partial (b, j) at
+// partial[b * bstride + j * jstride]: thread t sums b = t, t + kGateReduceThreads, ... in order, then a fixed tree
+// over the CTA -- the same sum for the same count, whichever CTA or warp wrote which partial
+constexpr int kGateReduceThreads = 1024;
+__global__ void __launch_bounds__(kGateReduceThreads)
+gate_reduce_kernel(const float* __restrict__ partial, float* __restrict__ out, int64_t count, int64_t bstride,
+                   int64_t jstride) {
+  __shared__ float warp_s[kGateReduceThreads / 32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const float* __restrict__ p = partial + blockIdx.x * jstride;
+  float acc = 0.f;
+#pragma unroll 8
+  for (int64_t b = threadIdx.x; b < count; b += kGateReduceThreads) acc += p[b * bstride];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+  if (lane == 0) warp_s[warp] = acc;
+  __syncthreads();
+  if (warp == 0) {
+    acc = warp_s[lane];
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
-    if (lane == 0) out[j] = acc;
+    if (lane == 0) out[blockIdx.x] = acc;
   }
 }
 
@@ -803,9 +815,16 @@ extern "C" int dva_view_attention_set_path(int path) {
   return DVA_OK;
 }
 
+// Workspace of the backward.  Streaming and ring kernels: one [2G] gate-gradient partial per CTA of the persistent
+// grid (at most kNumSMs x 8 co-resident CTAs) from the start.  Lane kernel: its range queue's counter, then one
+// partial per range, [2G = 8][n_ranges] (view_attention.cuh).
+static size_t cta_partials_bytes(int64_t G) { return (size_t)kNumSMs * 8 * 2 * (size_t)(G > 0 ? G : 1) * sizeof(float); }
+constexpr size_t kLaneQueueBytes = 256;
+
 extern "C" size_t dva_view_attention_bwd_workspace_bytes(int64_t G) {
-  // one [2,G] partial per CTA of the persistent grid (at most kNumSMs x 8 co-resident CTAs)
-  return (size_t)kNumSMs * 8 * 2 * (size_t)(G > 0 ? G : 1) * sizeof(float);
+  const size_t lane = kLaneQueueBytes + round256((size_t)8 * kLaneMaxRanges * sizeof(float));
+  const size_t cta = round256(cta_partials_bytes(G));
+  return lane > cta ? lane : cta;
 }
 
 extern "C" int dva_view_attention_bwd(const void* x, const void* idx, int idx_is_i64,
@@ -830,29 +849,41 @@ extern "C" int dva_view_attention_bwd(const void* x, const void* idx, int idx_is
   }
   if (!x || !compat || !ptr || !grad_out || !seg_max || !seg_den || !seg_arg || !grad_x_rows || !grad_compat)
     return fail(DVA_EINVAL, "view_attention_bwd: null pointer");
-  if (gating && (!grad_gate || !workspace || workspace_bytes < dva_view_attention_bwd_workspace_bytes(G)))
-    return fail(DVA_EINVAL, "view_attention_bwd: gating needs grad_gate and workspace");
+  if (!known_dtype(dtype)) return fail(DVA_EINVAL, "view_attention_bwd: unknown dtype");
+  if (!workspace || workspace_bytes < dva_view_attention_bwd_workspace_bytes(G))
+    return fail(DVA_EINVAL, "view_attention_bwd: workspace too small");
+  if (gating && !grad_gate) return fail(DVA_EINVAL, "view_attention_bwd: gating needs grad_gate");
   VAParams P{};
   P.x = x; P.idx = idx; P.idx64 = idx_is_i64; P.compat = compat; P.ptr = ptr;
   P.gate_w = gate_w; P.gate_b = gate_b; P.gout = grad_out;
   P.s_max = seg_max; P.s_den = seg_den; P.s_arg = seg_arg;
   P.gx = grad_x_rows; P.gcompat = grad_compat; P.scatter = scatter_rows;
-  P.gate_partial = gating ? reinterpret_cast<float*>(workspace) : nullptr;
   P.N = N; P.V = V; P.R = R; P.C = (int)C; P.G = (int)G; P.group_scaling = group_scaling;
-  int grid = 1;
+  uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
+  int64_t partials = 1, bstride = 2 * G, jstride = 1;      // gate partial (b, j) at [b * bstride + j * jstride]
   int rc;
-  if (!known_dtype(dtype)) return fail(DVA_EINVAL, "view_attention_bwd: unknown dtype");
   const bool short_rows = short_bwd_applicable(P, dtype);
   if (use_ring(P, dtype, short_rows, true)) {
+    P.gate_partial = gating ? reinterpret_cast<float*>(ws) : nullptr;
+    int grid = 1;
     rc = va_ring_bwd(P, dtype, &grid, st);
+    partials = grid;
   } else if (use_lane_bwd(P, short_rows)) {
-    rc = va_lane_bwd(P, dtype, &grid, st);
+    P.gate_partial = gating ? reinterpret_cast<float*>(ws + kLaneQueueBytes) : nullptr;
+    const int64_t pr = lane_range_points(N, V);
+    rc = va_lane_bwd(P, dtype, pr, reinterpret_cast<uint32_t*>(ws), st);
+    partials = (N + pr - 1) / pr;
+    bstride = 1;
+    jstride = partials;
   } else {
+    P.gate_partial = gating ? reinterpret_cast<float*>(ws) : nullptr;
+    int grid = 1;
     rc = with_dtype(dtype, [&](auto tag) { return bwd_typed<decltype(tag)>(P, &grid, st); });
+    partials = grid;
   }
   if (rc) return rc;
   if (gating) {
-    gate_reduce_kernel<<<1, 1024, 0, st>>>(P.gate_partial, grad_gate, grid, 2 * (int)G);
+    gate_reduce_kernel<<<2 * (int)G, kGateReduceThreads, 0, st>>>(P.gate_partial, grad_gate, partials, bstride, jstride);
     return check_launch("gate_reduce");
   }
   return DVA_OK;

@@ -141,33 +141,59 @@ __device__ __forceinline__ void store_gate_partial(float* __restrict__ partial, 
 }
 
 // ---- host side
-// Persistent grid of the ring and lane kernels, whose warps stride over ranges of PR points: the co-resident CTAs
-// (kNumSMs x occupancy, at most max_ctas_per_sm), about ranges_per_warp ranges per warp and never fewer than 8
-// points per range, and no more CTAs than there are ranges.
+// Persistent grid of the ring and lane kernels, whose warps take ranges of points: the co-resident CTAs (kNumSMs x
+// occupancy, at most max_ctas_per_sm per SM) ...
 template <typename K>
-int range_geometry(K kern, size_t smem, int warps_per_cta, int max_ctas_per_sm, int ranges_per_warp, int64_t N,
-                   const char* what, int* grid_out, int* pr_out) {
+int resident_ctas(K kern, size_t smem, int warps_per_cta, int max_ctas_per_sm, const char* what, int64_t* ctas_out) {
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return failf((int)e, "%s: %zu bytes of shared memory: %s", what, smem, cudaGetErrorString(e));
   int occ = 0;
   if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, warps_per_cta * 32, smem) != cudaSuccess || occ < 1) occ = 1;
   if (occ > max_ctas_per_sm) occ = max_ctas_per_sm;
-  int64_t grid = (int64_t)kNumSMs * occ;
-  const int64_t slots = grid * warps_per_cta * ranges_per_warp;
+  *ctas_out = (int64_t)kNumSMs * occ;
+  return DVA_OK;
+}
+// ... and no more CTAs than it takes to give every warp one of n_ranges
+inline int range_grid(int64_t ctas, int warps_per_cta, int64_t n_ranges) {
+  const int64_t need = (n_ranges + warps_per_cta - 1) / warps_per_cta;
+  return (int)(ctas > need ? (need < 1 ? 1 : need) : ctas);
+}
+
+// The ring kernels' warps stride over ranges of PR points: about ranges_per_warp ranges per warp of the full grid,
+// and never fewer than 8 points per range.
+template <typename K>
+int range_geometry(K kern, size_t smem, int warps_per_cta, int max_ctas_per_sm, int ranges_per_warp, int64_t N,
+                   const char* what, int* grid_out, int* pr_out) {
+  int64_t ctas = 0;
+  if (int rc = resident_ctas(kern, smem, warps_per_cta, max_ctas_per_sm, what, &ctas)) return rc;
+  const int64_t slots = ctas * warps_per_cta * ranges_per_warp;
   int64_t pr = (N + slots - 1) / slots;
   if (pr < 8) pr = 8;
-  const int64_t n_ranges = (N + pr - 1) / pr;
-  const int64_t need = (n_ranges + warps_per_cta - 1) / warps_per_cta;
-  if (grid > need) grid = need;
-  if (grid < 1) grid = 1;
-  *grid_out = (int)grid; *pr_out = (int)pr;
+  *grid_out = range_grid(ctas, warps_per_cta, (N + pr - 1) / pr); *pr_out = (int)pr;
   return DVA_OK;
+}
+
+// The lane backward's warps take ranges of PR points from a queue (a counter the launcher zeroes on the stream):
+// ranges of about kLaneRangeViews views -- 8 groups of 32 views, a short wait at the end of the kernel -- but never
+// more than kLaneMaxRangePoints points, so that with few views per point the points are still spread over many
+// warps; and at most kLaneMaxRanges ranges, which wins over both.  Its gate-gradient partials are one per range,
+// [2G = 8][n_ranges], so that they do not depend on which warp took which range.
+constexpr int64_t kLaneRangeViews = 256;
+constexpr int64_t kLaneMaxRangePoints = 8192;
+constexpr int64_t kLaneMaxRanges = 1 << 17;
+inline int64_t lane_range_points(int64_t N, int64_t V) {
+  int64_t pr = (kLaneRangeViews * N + V - 1) / (V > 0 ? V : 1);
+  if (pr > kLaneMaxRangePoints) pr = kLaneMaxRangePoints;
+  const int64_t fit = (N + kLaneMaxRanges - 1) / kLaneMaxRanges;   // the workspace holds kLaneMaxRanges partials
+  if (pr < fit) pr = fit;
+  return pr < 1 ? 1 : pr;
 }
 
 // ring kernels (view_attention_ring.cu) and lane-per-view backward (view_attention_lane.cu); the launchers return a
 // DVA_* / cudaError code like every other entry point.  Shape / alignment conditions: view_attention.cu.
 int va_ring_fwd(const VAParams& P, int dtype, cudaStream_t st);
 int va_ring_bwd(const VAParams& P, int dtype, int* grid_out, cudaStream_t st);
-int va_lane_bwd(const VAParams& P, int dtype, int* grid_out, cudaStream_t st);
+// next_range: a counter on the device, zeroed here before the launch
+int va_lane_bwd(const VAParams& P, int dtype, int64_t pr, uint32_t* next_range, cudaStream_t st);
 
 }  // namespace dva

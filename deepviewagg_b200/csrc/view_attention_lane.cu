@@ -24,6 +24,9 @@
 //            coalesced float4 per lane.
 // A point with more than 32 views (never in the short-segment regime this kernel is dispatched for) is
 // walked in chunks of 32 views with its raw s' parked in grad_compat.
+// Warps take ranges of consecutive points (about 256 views each) from a queue, one global counter, so that they all
+// finish within about one range of each other.  The gate-gradient partials are one per range and are summed in
+// range order: no result depends on which warp took which range.
 // Requires G == 4 and the regular channel layout (a row is LPR = 4 * 2^k chunks of 16 bytes, <= 512 bytes).
 // HBM bytes per launch: those of the other two implementations (V (2 C s + 4 + 8 G) + N (C s + 8 + 12 G)).
 #include "view_attention.cuh"
@@ -39,16 +42,20 @@ struct LaneSmem {            // per warp
   float st[32][4];           // raw dot <grad_out, x> per (view, group)
   float Sp[32][4];           // per point: S
   float dq[32][4];           // per point: gate term routed to the arg-max view
-  uint32_t ri[32];           // x row of the view
   uint32_t orow[32];         // dx row of the view
   uint32_t go[32];           // point of the view (grad_out row), relative to the group's first point
   uint64_t bar;              // completion of the group's row copies
   uint64_t pad;
 };
 
+// At 512-byte rows (LPR 32) the 64 KB row buffers of a CTA leave room for two CTAs per SM, and the kernel gets the
+// registers of two: at five it spilled ~160 bytes per thread, and not spilling is 3 % of its time on an H100.
+// Three CTAs per SM (shared memory trimmed to fit) measured 0.8 % slower than two.
+template <int LPR> constexpr int lane_ctas_per_sm() { return LPR == 32 ? 2 : 5; }
+
 template <typename T, int LPR>
-__global__ void __launch_bounds__(kLaneWarps * 32, 5)
-va_lane_bwd_kernel(const VAParams P, const int PR) {
+__global__ void __launch_bounds__(kLaneWarps * 32, lane_ctas_per_sm<LPR>())
+va_lane_bwd_kernel(const VAParams P, const int64_t PR, uint32_t* __restrict__ next_range) {
   constexpr int VEC = Vec16<T>::N, RPI = 32 / LPR, CPE = LPR / 4, U = 4, RS = LPR * 16;
   extern __shared__ __align__(128) unsigned char rows_all[];       // [kLaneWarps][32 rows][RS bytes]
   __shared__ LaneSmem sm_all[kLaneWarps];
@@ -126,9 +133,12 @@ va_lane_bwd_kernel(const VAParams P, const int PR) {
   };
 
   const int64_t n_ranges = (P.N + PR - 1) / PR;
-  const int64_t warps_total = (int64_t)gridDim.x * kLaneWarps;
-  for (int64_t r = (int64_t)blockIdx.x * kLaneWarps + warp; r < n_ranges; r += warps_total) {
-    const int64_t pa = r * PR;
+  for (;;) {
+    uint32_t r = 0;                                                 // the next range of the queue
+    if (lane == 0) r = atomicAdd(next_range, 1u);
+    r = __shfl_sync(kFull, r, 0);
+    if (r >= n_ranges) break;
+    const int64_t pa = (int64_t)r * PR;
     const int64_t pb = (pa + PR < P.N) ? pa + PR : P.N;
     for (int64_t pg = pa; pg < pb;) {
       // ---- group: lane k looks at point pg + k
@@ -171,7 +181,6 @@ va_lane_bwd_kernel(const VAParams P, const int PR) {
             const float4 c = __ldg(reinterpret_cast<const float4*>(P.compat) + v);
             a = make_float4(__expf((c.x - smx.x) * inv_sq) / sdn.x, __expf((c.y - smx.y) * inv_sq) / sdn.y,
                             __expf((c.z - smx.z) * inv_sq) / sdn.z, __expf((c.w - smx.w) * inv_sq) / sdn.w);
-            sm.ri[lane] = rid_l;
             sm.orow[lane] = scatter ? rid_l : (uint32_t)v;
             sm.go[lane] = 0u;
             *reinterpret_cast<float4*>(sm.wt[lane]) = make_float4(a.x * t4.x, a.y * t4.y, a.z * t4.z, a.w * t4.w);
@@ -239,7 +248,6 @@ va_lane_bwd_kernel(const VAParams P, const int PR) {
         a = make_float4(__expf((c.x - smx.x) * inv_sq) / sdn.x, __expf((c.y - smx.y) * inv_sq) / sdn.y,
                         __expf((c.z - smx.z) * inv_sq) / sdn.z, __expf((c.w - smx.w) * inv_sq) / sdn.w);
         if (gating) t4 = gate_t4(gate_z4(gw4, smx, gb4));
-        sm.ri[lane] = rid_m;
         sm.orow[lane] = scatter ? rid_m : (uint32_t)v;
         sm.go[lane] = (uint32_t)mp;
         *reinterpret_cast<float4*>(sm.at[lane]) = a;
@@ -284,22 +292,35 @@ va_lane_bwd_kernel(const VAParams P, const int PR) {
       }
       pg += kfit;
     }
-  }
 
-  if (P.gate_partial != nullptr) store_gate_partial<kLaneWarps>(P.gate_partial, dw4, db4);
+    if (P.gate_partial != nullptr) {                                // the range's gate gradients -> [dw0..3, db0..3][r]
+      float g[8] = {dw4.x, dw4.y, dw4.z, dw4.w, db4.x, db4.y, db4.z, db4.w};
+      float mine = 0.f;
+#pragma unroll
+      for (int q = 0; q < 8; ++q) {
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) g[q] += __shfl_xor_sync(kFull, g[q], o);
+        if (lane == q) mine = g[q];
+      }
+      if (lane < 8) P.gate_partial[lane * n_ranges + r] = mine;
+      dw4 = make_float4(0.f, 0.f, 0.f, 0.f);
+      db4 = dw4;
+    }
+  }
 }
 
-int va_lane_bwd(const VAParams& P, int dtype, int* grid_out, cudaStream_t st) {
+int va_lane_bwd(const VAParams& P, int dtype, int64_t pr, uint32_t* next_range, cudaStream_t st) {
   return with_dtype(dtype, [&](auto tag) {
     using T = decltype(tag);
     return with_lpr(P.C / Vec16<T>::N, [&](auto lpr) {
       constexpr int LPR = decltype(lpr)::value;
       auto kern = va_lane_bwd_kernel<T, LPR>;
       const size_t smem = (size_t)kLaneWarps * 32 * LPR * 16;    // row buffers: 32 rows per warp
-      int grid, pr;   // at most 8 CTAs per SM (gate partials); ~4 ranges per warp balance ragged counts
-      if (int rc = range_geometry(kern, smem, kLaneWarps, 8, 4, P.N, "va_lane_bwd", &grid, &pr)) return rc;
-      kern<<<grid, kLaneWarps * 32, smem, st>>>(P, pr);
-      *grid_out = grid;
+      int64_t ctas = 0;
+      if (int rc = resident_ctas(kern, smem, kLaneWarps, lane_ctas_per_sm<LPR>(), "va_lane_bwd", &ctas)) return rc;
+      cudaError_t e = cudaMemsetAsync(next_range, 0, sizeof(uint32_t), st);
+      if (e != cudaSuccess) return failf((int)e, "va_lane_bwd: %s", cudaGetErrorString(e));
+      kern<<<range_grid(ctas, kLaneWarps, (P.N + pr - 1) / pr), kLaneWarps * 32, smem, st>>>(P, pr, next_range);
       return check_launch("va_lane_bwd");
     });
   });

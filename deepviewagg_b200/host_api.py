@@ -38,8 +38,8 @@ class ViewAttentionHostPlan:
         self.gx = e((V, C), dtype)
         self.gcompat = e((V, G), torch.float32)
         self.ggate = e((2, G), torch.float32) if gating else None
-        # the workspace holds the gate-gradient partials; without gating the kernel does not read it
-        self.ws = _lib.workspace(_lib.load().dva_view_attention_bwd_workspace_bytes(G) if gating else 0, d)
+        # gate-gradient partials and the lane kernel's range queue
+        self.ws = _lib.workspace(_lib.load().dva_view_attention_bwd_workspace_bytes(G), d)
         self.dcode = _lib.DTYPE_CODES[dtype]
 
     # -- device-resident pieces (bench.py's `value` times exactly these two calls) ---------------

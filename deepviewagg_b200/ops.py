@@ -278,13 +278,12 @@ class _ViewAttention(torch.autograd.Function):
         scatter = int(idx is not None and is_perm and R == V)
         gx_rows = torch.empty((V, C), dtype=x.dtype, device=x.device)
         gcompat = torch.empty((V, G), dtype=torch.float32, device=x.device)
-        ggate, ws = None, None                      # the workspace holds the gate-gradient partials only
-        if gw is not None:
-            ggate = torch.empty((2, G), dtype=torch.float32, device=x.device)
-            ws = _lib.workspace(_lib.load().dva_view_attention_bwd_workspace_bytes(G), x.device)
+        ggate = torch.empty((2, G), dtype=torch.float32, device=x.device) if gw is not None else None
+        # gate-gradient partials and the lane kernel's range queue
+        ws = _lib.workspace(_lib.load().dva_view_attention_bwd_workspace_bytes(G), x.device)
         launch("dva_view_attention_bwd", x.device, x, idx, idx64, compat, csr_idx, gw, gb, grad_out, seg_max,
                seg_den, seg_arg, gx_rows, gcompat, ggate, scatter, N, V, R, C, G, int(scaling), dtype_code(x), ws,
-               0 if ws is None else ws.numel())
+               ws.numel())
         if idx is None or scatter:
             gx = gx_rows
         else:  # general (non-injective) gather: accumulate duplicated rows (red.global.add.v4.f32 kernel)

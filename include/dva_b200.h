@@ -117,7 +117,8 @@ int dva_view_attention_set_path(int path);
  *   requires idx to be injective, as view_cat_sorting is, image.py:1549-1574),
  *   grad_compat [V,G] fp32 (softmax path + gating arg-max path),
  *   grad_gate [2,G] fp32 (d gate_w ; d gate_b), nullable when no gating.
- *   workspace: dva_view_attention_bwd_workspace_bytes(G) bytes (per-block partials). */
+ *   workspace: dva_view_attention_bwd_workspace_bytes(G) bytes, with or without gating (gate-gradient
+ *   partials and the lane kernel's range queue; one call at a time per workspace). */
 size_t dva_view_attention_bwd_workspace_bytes(int64_t G);
 int dva_view_attention_bwd(const void* x, const void* idx, int idx_is_i64, const float* compat,
                            const int64_t* ptr, const float* gate_w, const float* gate_b,
