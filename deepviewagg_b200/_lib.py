@@ -1,13 +1,16 @@
-"""ctypes binding of libdva_b200.so (the C ABI declared in include/dva_b200.h), of libdva_eval.so, the
-evaluation kernels (include/dva_eval.h), of libdva_conv2d.so, the image encoder's convolutions
-(include/dva_conv2d.h), of libdva_unet.so, the image decoder's transposed convolutions (include/dva_unet.h), and of
-libdva_resnet.so, the ADE20K ResNet-18 encoder (include/dva_resnet.h); the last four link against the first and share
-its error string and launch counter.
+"""ctypes binding of the package's native libraries, one `Library` record each in `LIBRARIES`: its file, the ctypes
+signatures of its entry points (a dict that mirrors its header under include/ one to one), that header, the namespace
+of its kernels, and whether it links against libdva_b200.so.  The linked libraries find libdva_b200.so next to them
+through rpath $ORIGIN and share its error string and launch counter, so last_error() and launch_count() cover them
+all; entry(name) finds an entry point in whichever library declares it.  Adding a library means adding a record, a
+header and a signatures dict here, and the library's sources to the list of linked libraries in csrc/Makefile.
 
-There is NO fallback: if the shared library is missing or a call fails, a RuntimeError is
+There is NO fallback: if a shared library is missing or a call fails, a RuntimeError is
 raised.  PyTorch is used above this layer only for device memory and streams.
 """
 import ctypes
+import dataclasses
+import functools
 import os
 import subprocess
 
@@ -17,11 +20,6 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # DVA_B200_LIB: developer knob to load a tuning variant of the same library (bench sweeps)
 LIB_PATH = os.environ.get("DVA_B200_LIB") or os.path.join(_HERE, "libdva_b200.so")
 CSRC_DIR = os.path.join(_HERE, "csrc")
-# libdva_eval.so loads the libdva_b200.so next to it (rpath $ORIGIN), whatever DVA_B200_LIB names
-EVAL_LIB_PATH = os.path.join(_HERE, "libdva_eval.so")
-CONV_LIB_PATH = os.path.join(_HERE, "libdva_conv2d.so")
-UNET_LIB_PATH = os.path.join(_HERE, "libdva_unet.so")
-RESNET_LIB_PATH = os.path.join(_HERE, "libdva_resnet.so")
 
 DVA_OK, DVA_EINVAL, DVA_EALIGN, DVA_EUNSUPPORTED = 0, -1, -2, -3
 DVA_F32, DVA_BF16, DVA_F16 = 0, 1, 2
@@ -196,15 +194,39 @@ RESNET_SIGNATURES = {
     "dva_resnet_resize_bwd": (_i32, [_vp, _i64, _i64, _i64, _i64, _i64, _i32, _i64, _i64, _f32, _f32, _vp, _vp]),
 }
 
-_lib = None
-_eval_lib = None
-_conv_lib = None
-_unet_lib = None
-_resnet_lib = None
+
+@dataclasses.dataclass(frozen=True, eq=False)
+class Library:
+    """One shared library of the package (see the module docstring)."""
+    file: str
+    signatures: dict
+    header: str
+    namespace: str
+    linked: bool = True
+
+    @property
+    def path(self):
+        """The package's copy of a linked library; LIB_PATH (DVA_B200_LIB if set) for libdva_b200.so."""
+        return os.path.join(_HERE, self.file) if self.linked else LIB_PATH
+
+
+B200 = Library("libdva_b200.so", SIGNATURES, "dva_b200.h", "dva::", linked=False)
+EVAL = Library("libdva_eval.so", EVAL_SIGNATURES, "dva_eval.h", "dva_eval::")
+CONV = Library("libdva_conv2d.so", CONV_SIGNATURES, "dva_conv2d.h", "dva_conv2d::")
+UNET = Library("libdva_unet.so", UNET_SIGNATURES, "dva_unet.h", "dva_unet::")
+RESNET = Library("libdva_resnet.so", RESNET_SIGNATURES, "dva_resnet.h", "dva_resnet::")
+LIBRARIES = (B200, EVAL, CONV, UNET, RESNET)
+
+EVAL_LIB_PATH, CONV_LIB_PATH, UNET_LIB_PATH, RESNET_LIB_PATH = EVAL.path, CONV.path, UNET.path, RESNET.path
+
+_LIBRARY_OF_ENTRY = {name: rec for rec in LIBRARIES for name in rec.signatures}
+if len(_LIBRARY_OF_ENTRY) != sum(len(rec.signatures) for rec in LIBRARIES):
+    raise RuntimeError("an entry point is declared by two libraries")
+_loaded = {}      # file -> ctypes.CDLL, each library loaded once per process
 
 
 def build(verbose=False):
-    """Compile libdva_b200.so for sm_90a (nvcc cross-compiles without a GPU)."""
+    """Compile the libraries for sm_90a (nvcc cross-compiles without a GPU)."""
     out = subprocess.run(["make", "-C", CSRC_DIR, "-j8"], capture_output=True, text=True)
     if verbose or out.returncode != 0:
         print(out.stdout[-4000:])
@@ -214,91 +236,46 @@ def build(verbose=False):
     return LIB_PATH
 
 
-def load():
-    """Load the shared library (once). Raises if it has not been built -- no CPU fallback."""
-    global _lib
-    if _lib is not None:
-        return _lib
-    if not os.path.exists(LIB_PATH):
+def load_library(rec):
+    """Load `rec` (once) and declare its entry points' signatures; a linked library loads libdva_b200.so first.
+    Raises if it has not been built -- no CPU fallback."""
+    lib = _loaded.get(rec.file)
+    if lib is not None:
+        return lib
+    if rec.linked:
+        in_tree = os.path.join(_HERE, B200.file)
+        if os.path.realpath(LIB_PATH) != os.path.realpath(in_tree):
+            # the library would load a second libdva_b200.so, whose error string and launch counter last_error()
+            # and launch_count() do not read
+            raise RuntimeError(f"{rec.file} links against {in_tree}; it cannot run beside the variant "
+                               f"DVA_B200_LIB={LIB_PATH}")
+        load_library(B200)
+    if not os.path.exists(rec.path):
         raise RuntimeError(
-            f"{LIB_PATH} not found: build it with `python -c 'import __graft_entry__ as g; "
+            f"{rec.path} not found: build it with `python -c 'import __graft_entry__ as g; "
             f"g.build()'` (or `make -C deepviewagg_b200/csrc`). deepviewagg_b200 has no CPU "
             f"fallback.")
-    lib = ctypes.CDLL(LIB_PATH)
-    for name, (res, args) in SIGNATURES.items():
+    lib = ctypes.CDLL(rec.path)
+    for name, (res, args) in rec.signatures.items():
         fn = getattr(lib, name)  # AttributeError if the symbol is not exported
         fn.restype = res
         fn.argtypes = args
-    if lib.dva_abi_version() != 1:
+    if not rec.linked and lib.dva_abi_version() != 1:
         raise RuntimeError("libdva_b200.so ABI version mismatch")
-    _lib = lib
+    _loaded[rec.file] = lib
     return lib
 
 
-def _load_linked(path, signatures):
-    """Load a library that links against libdva_b200.so (rpath $ORIGIN), after it.  Raises if it has not been
-    built."""
-    name = os.path.basename(path)
-    if os.path.realpath(LIB_PATH) != os.path.realpath(os.path.join(_HERE, "libdva_b200.so")):
-        # the library would load a second libdva_b200.so, whose error string and launch counter last_error()
-        # and launch_count() do not read
-        raise RuntimeError(f"{name} links against {os.path.join(_HERE, 'libdva_b200.so')}; it cannot run "
-                           f"beside the variant DVA_B200_LIB={LIB_PATH}")
-    load()
-    if not os.path.exists(path):
-        raise RuntimeError(f"{path} not found: build it with `make -C deepviewagg_b200/csrc` "
-                           f"(the same build as libdva_b200.so). deepviewagg_b200 has no CPU fallback.")
-    lib = ctypes.CDLL(path)
-    for fname, (res, args) in signatures.items():
-        fn = getattr(lib, fname)
-        fn.restype = res
-        fn.argtypes = args
-    return lib
-
-
-def load_eval():
-    """Load libdva_eval.so (once), after libdva_b200.so.  Raises if it has not been built."""
-    global _eval_lib
-    if _eval_lib is None:
-        _eval_lib = _load_linked(EVAL_LIB_PATH, EVAL_SIGNATURES)
-    return _eval_lib
-
-
-def load_conv():
-    """Load libdva_conv2d.so (once), after libdva_b200.so.  Raises if it has not been built."""
-    global _conv_lib
-    if _conv_lib is None:
-        _conv_lib = _load_linked(CONV_LIB_PATH, CONV_SIGNATURES)
-    return _conv_lib
-
-
-def load_unet():
-    """Load libdva_unet.so (once), after libdva_b200.so.  Raises if it has not been built."""
-    global _unet_lib
-    if _unet_lib is None:
-        _unet_lib = _load_linked(UNET_LIB_PATH, UNET_SIGNATURES)
-    return _unet_lib
-
-
-def load_resnet():
-    """Load libdva_resnet.so (once), after libdva_b200.so.  Raises if it has not been built."""
-    global _resnet_lib
-    if _resnet_lib is None:
-        _resnet_lib = _load_linked(RESNET_LIB_PATH, RESNET_SIGNATURES)
-    return _resnet_lib
+load = functools.partial(load_library, B200)
+load_eval = functools.partial(load_library, EVAL)
+load_conv = functools.partial(load_library, CONV)
+load_unet = functools.partial(load_library, UNET)
+load_resnet = functools.partial(load_library, RESNET)
 
 
 def entry(name):
     """The entry point `name`, from whichever library declares it."""
-    if name in RESNET_SIGNATURES:
-        return getattr(load_resnet(), name)
-    if name in UNET_SIGNATURES:
-        return getattr(load_unet(), name)
-    if name in EVAL_SIGNATURES:
-        return getattr(load_eval(), name)
-    if name in CONV_SIGNATURES:
-        return getattr(load_conv(), name)
-    return getattr(load(), name)
+    return getattr(load_library(_LIBRARY_OF_ENTRY.get(name, B200)), name)
 
 
 def last_error():

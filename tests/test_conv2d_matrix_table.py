@@ -1,25 +1,15 @@
 """Kernel table of libdva_conv2d.so, the image encoder's convolutions and GroupNorm (namespace dva_conv2d::,
 csrc/conv2d.cu).
 
-tests/test_gpu_conv2d_matrix.py runs every instantiation on the GPU under the kernel recorder and asserts, by name,
-that it ran.  This file checks, without a GPU, that
-  * the table holds exactly the kernels compiled into libdva_conv2d.so, all of them in dva_conv2d::;
-  * no kernel name of libdva_conv2d.so appears in libdva_b200.so or libdva_eval.so;
-  * include/dva_conv2d.h, _lib.CONV_SIGNATURES and the exported symbols agree, and are disjoint from the other
-    two tables of signatures;
-  * an argument error of the new library is reported through _lib.last_error() (the libraries share the error
-    string).
+tests/test_gpu_library_matrix.py runs every instantiation on the GPU under the kernel recorder and asserts, by name,
+that it ran; tests/test_library_tables.py checks the table against the library without a GPU.  This file checks
+that an argument error of the library is reported through _lib.last_error() (the libraries share the error
+string).
 conv_gemm_kernel<MODE>: 0/1/2 = forward 3x3 reflect / 2x2 stride 2 / 1x1, 3/4/5 = data gradient of the same;
 conv_wgrad_kernel<KIND>: KIND = DVA_CONV_3X3_REFLECT (0), DVA_CONV_2X2_S2 (1), DVA_CONV_1X1 (2)."""
-import os
-import re
-
-import pytest
-
-from conftest import ROOT
 from deepviewagg_b200 import _lib
-from test_kernel_matrix_table import kname, parse_kernel
-from test_loss_matrix_table import demangled_kernels
+import test_kernel_matrix_table as KM
+from test_kernel_matrix_table import kname
 
 NAMESPACE = "dva_conv2d::"
 FAMILIES = ("conv_gemm_kernel", "conv_wgrad_kernel", "gn_stats_kernel", "wgrad_reduce_kernel", "weight_prep_kernel",
@@ -28,72 +18,15 @@ FAMILIES = ("conv_gemm_kernel", "conv_wgrad_kernel", "gn_stats_kernel", "wgrad_r
 
 
 def canonical(name):
-    """Demangled dva_conv2d:: kernel name -> 'family<args>'; None for anything else."""
-    s = name.strip()
-    if s.startswith("void "):
-        s = s[5:]
-    if not s.startswith(NAMESPACE):
-        return None
-    p = parse_kernel("dva::" + s[len(NAMESPACE):])
-    if p is None or p[0] not in FAMILIES:
-        return None
-    return kname(p[0], *p[1])
+    return KM.canonical(name, FAMILIES, NAMESPACE)
 
 
-# every kernel runs in the one scenario of tests/test_gpu_conv2d_matrix.py: forward + backward of a two-stage
+# every kernel runs in the one scenario of tests/test_gpu_library_matrix.py: forward + backward of a two-stage
 # encoder (3x3 conv_in, then a 2x2 conv_in and two ResBlocks, the first with a 1x1 downsample) with the input's
 # gradient
 TABLE = {kname("conv_gemm_kernel", m): "encoder" for m in range(6)}
 TABLE.update({kname("conv_wgrad_kernel", k): "encoder" for k in range(3)})
 TABLE.update({f: "encoder" for f in FAMILIES[2:]})
-
-
-def _built():
-    for p in (_lib.LIB_PATH, _lib.CONV_LIB_PATH):
-        if not os.path.exists(p):
-            pytest.fail(f"{p} is not built")
-    return _lib.CONV_LIB_PATH
-
-
-def test_table_matches_library():
-    names = demangled_kernels(_built())
-    names = [n for n in names if "__internal" not in n]
-    outside = sorted(n for n in names if not n.replace("void ", "", 1).startswith(NAMESPACE))
-    assert not outside, outside
-    built = {canonical(n) for n in names}
-    assert None not in built, names
-    assert built == set(TABLE), {"compiled without a case": sorted(built - set(TABLE)),
-                                 "case without a kernel": sorted(set(TABLE) - built)}
-    assert len(TABLE) == 18
-
-
-def test_no_kernel_name_shared_with_the_other_libraries():
-    _built()
-    ours = {canonical(n).split("<")[0] for n in demangled_kernels(_lib.CONV_LIB_PATH) if canonical(n)}
-    for other in (_lib.LIB_PATH, _lib.EVAL_LIB_PATH):
-        names = {n.replace("void ", "", 1).split("(")[0] for n in demangled_kernels(other)}
-        assert not any(n.startswith(NAMESPACE) for n in names)
-        assert not {n for n in names if n.split("::")[-1].split("<")[0] in ours}
-
-
-def _declared(header):
-    text = open(os.path.join(ROOT, "include", header)).read()
-    text = re.sub(r"/\*.*?\*/", "", text, flags=re.S)
-    return set(re.findall(r"\b(dva_[a-z0-9_]+)\s*\(", text))
-
-
-def test_header_signatures_and_exports_agree():
-    _built()
-    names = _declared("dva_conv2d.h")
-    assert names == set(_lib.CONV_SIGNATURES)
-    assert all(n.startswith("dva_conv2d_") for n in names)
-    assert not names & set(_lib.SIGNATURES) and not names & set(_lib.EVAL_SIGNATURES)
-    lib = _lib.load_conv()
-    for n in names:
-        assert hasattr(lib, n), n
-        assert _lib.entry(n) is getattr(lib, n)
-    assert _lib.entry("dva_knn_query") is getattr(_lib.load(), "dva_knn_query")
-    assert _lib.entry("dva_eval_vote") is getattr(_lib.load_eval(), "dva_eval_vote")
 
 
 def test_errors_reach_the_shared_error_string():

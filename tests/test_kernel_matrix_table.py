@@ -56,16 +56,16 @@ SEG_LENGTHS = (0, 1, 31, 32, 33, 127, 128, 129, 255, 256, 257)   # a warp of vie
 # ------------------------------------------------------------------------------------------------
 # kernel names
 # ------------------------------------------------------------------------------------------------
-def parse_kernel(name):
+def parse_kernel(name, namespace="dva::"):
     """Demangled kernel name -> (family, template args), e.g.
     'void dva::view_attention_bwd_kernel<__nv_bfloat16, 1, 32, 4, 2, true>(dva::VAParams)'
-    -> ('view_attention_bwd_kernel', ('__nv_bfloat16', '1', '32', '4', '2', 'true')); None outside dva::."""
+    -> ('view_attention_bwd_kernel', ('__nv_bfloat16', '1', '32', '4', '2', 'true')); None outside `namespace`."""
     s = name.strip()
     if s.startswith("void "):
         s = s[5:]
-    if not s.startswith("dva::"):
+    if not s.startswith(namespace):
         return None
-    s = s[5:]
+    s = s[len(namespace):]
     cut = len(s)
     for ch in "<(":
         if ch in s:
@@ -82,8 +82,8 @@ def kname(family, *args):
         else family
 
 
-def canonical(name, families=FAMILIES):
-    p = parse_kernel(name)
+def canonical(name, families=FAMILIES, namespace="dva::"):
+    p = parse_kernel(name, namespace)
     if p is None or p[0] not in families:
         return None
     return kname(p[0], *p[1])

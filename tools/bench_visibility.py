@@ -147,13 +147,13 @@ def main():
     res = {name: [] for name, _ in libs}
     for rnd in range(3):                                     # alternate the libraries
         for name, lib in libs:
-            saved = _lib._lib
-            _lib._lib = lib
+            saved = _lib._loaded[_lib.B200.file]
+            _lib._loaded[_lib.B200.file] = lib
             try:
                 nb = knn_grid(pos, 20)
                 r = timed(lambda: knn_grid(pos, 20), args.iters, args.warmup)
             finally:
-                _lib._lib = saved
+                _lib._loaded[_lib.B200.file] = saved
             res[name].append((r, nb))
     ref_nb = res["this"][0][1]
     for name, runs in res.items():
