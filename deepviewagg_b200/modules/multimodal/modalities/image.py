@@ -697,6 +697,45 @@ def load_mit_semseg_encoder(module, state_dict):
     return module
 
 
+def _check_bn_values(bn, training, B, H, W):
+    """torch's error for a training BatchNorm that would see one value per channel, raised before any launch."""
+    if training and B * H * W <= 1:
+        raise ValueError(f"Expected more than 1 value per channel when training, got input size "
+                         f"{[B, bn.num_features, H, W]}")
+
+
+# A trunk as _run_trunk walks it: a list of layers, each the stem -- a list of three (conv, BatchNorm) units, then the
+# max pool -- or a Sequential of BasicBlocks.
+def _trunk_bn_sizes(trunk, H, W):
+    """Yields (BatchNorm, H, W of the map it normalises) along the trunk for an H x W input."""
+    for layer in trunk:
+        if isinstance(layer, list):
+            for conv, bn in layer:
+                H, W = ops.rn_out(H, conv.stride[0]), ops.rn_out(W, conv.stride[0])
+                yield bn, H, W
+            H, W = ops.rn_out(H, 2), ops.rn_out(W, 2)
+        else:
+            for block in layer:
+                H, W = ops.rn_out(H, block.conv1.stride[0]), ops.rn_out(W, block.conv1.stride[0])
+                yield block.bn1, H, W
+                yield block.bn2, H, W
+                if block.downsample is not None:
+                    yield block.downsample[1], H, W
+
+
+def _run_trunk(trunk, h):
+    """Yields the channels-last output of each layer of the trunk for channels-last rows h."""
+    for layer in trunk:
+        if isinstance(layer, list):
+            for conv, bn in layer:
+                h = ops.rn_conv_bn_relu(h, conv, bn)
+            h = ops.rn_maxpool(h)
+        else:
+            for block in layer:
+                h = ops.rn_basic_block(h, block)
+        yield h
+
+
 class ADE20KResNet18TruncatedLayer4(nn.Module):
     """ResNet-18 encoder pretrained on ADE20K (mit_semseg's resnet18dilated), truncated after `_LAYERS`
     (image.py:793-898), on the sm_90a kernels of libdva_resnet.so.
@@ -738,37 +777,19 @@ class ADE20KResNet18TruncatedLayer4(nn.Module):
                              f"{tuple(x.shape)}")
         B, _, H, W = x.shape
         for bn, H, W in self._bn_sizes(H, W):
-            if bn.training and B * H * W <= 1:
-                raise ValueError(f"Expected more than 1 value per channel when training, got input size "
-                                 f"{[B, bn.num_features, H, W]}")
+            _check_bn_values(bn, bn.training, B, H, W)
+
+    def _trunk(self):
+        return [layer if isinstance(layer[0], BasicBlock) else [(layer[i], layer[i + 1]) for i in (0, 3, 6)]
+                for layer in self.conv]
 
     def _bn_sizes(self, H, W):
         """Yields (BatchNorm, H, W of the map it normalises) along the trunk for an H x W input."""
-        for layer in self.conv:
-            if isinstance(layer[0], BasicBlock):
-                for block in layer:
-                    H, W = ops.rn_out(H, block.conv1.stride[0]), ops.rn_out(W, block.conv1.stride[0])
-                    yield block.bn1, H, W
-                    yield block.bn2, H, W
-                    if block.downsample is not None:
-                        yield block.downsample[1], H, W
-            else:
-                for i in (0, 3, 6):
-                    H, W = ops.rn_out(H, layer[i].stride[0]), ops.rn_out(W, layer[i].stride[0])
-                    yield layer[i + 1], H, W
-                H, W = ops.rn_out(H, 2), ops.rn_out(W, 2)
+        return _trunk_bn_sizes(self._trunk(), H, W)
 
     def _layers(self, h):
         """Yields the channels-last output of each layer of self.conv for channels-last rows h."""
-        for layer in self.conv:
-            if isinstance(layer[0], BasicBlock):
-                for block in layer:
-                    h = ops.rn_basic_block(h, block)
-            else:
-                for i in (0, 3, 6):
-                    h = ops.rn_conv_bn_relu(h, layer[i], layer[i + 1])
-                h = ops.rn_maxpool(h)
-            yield h
+        return _run_trunk(self._trunk(), h)
 
     def forward(self, x, *args, **kwargs):
         self._check_input(x)
@@ -858,3 +879,189 @@ class ADE20KResNet18Pyramid(ADE20KResNet18TruncatedLayer4):
         size = [int(s * self.scale_factor / self.conv_scale_factor) for s in x.shape[2:4]]
         h = ops.rn_resize(list(self._layers(_rows(x))), size)
         return h.to(_out_dtype(x)).permute(0, 3, 1, 2)
+
+
+# --------------------------------------------------------------------------------------------------------------------
+# ResNet-18 + pyramid pooling pretrained on ADE20K (mit_semseg's resnet18dilated-ppm_deepsup) behind the reference's
+# ADE20KResNet18PPM (image.py:634-790): the trunk above under mit_semseg's flat names, and PPMFeatMap, the PPMDeepsup
+# decoder without its classifiers, run as one node (ops.rn_ppm_head).
+# --------------------------------------------------------------------------------------------------------------------
+class FusedAdaptiveAvgPool2d(nn.AdaptiveAvgPool2d):
+    """AdaptiveAvgPool2d of a pyramid branch; run by the PPMFeatMap that holds it."""
+
+    def forward(self, input):
+        raise NotImplementedError("FusedAdaptiveAvgPool2d is run by the PPMFeatMap that holds it")
+
+
+class PrudentSynchronizedBatchNorm2d(SynchronizedBatchNorm2d):
+    """SynchronizedBatchNorm2d that runs in eval mode for a (1, C, 1, 1) input (image.py:634-656): in a pyramid
+    branch, the scale-1 branch at batch size 1 normalises with the running stats and leaves them unchanged."""
+
+    def forward(self, input):
+        raise NotImplementedError("PrudentSynchronizedBatchNorm2d runs fused with its convolution: call the "
+                                  "PPMFeatMap that holds it")
+
+
+class ResnetDilated(nn.Module):
+    """mit_semseg's ResnetDilated(resnet18, dilate_scale=8) under its flat names (conv1, bn1, relu1, ..., maxpool,
+    layer1..layer4), so that encoder_epoch_20.pth loads into it as it is."""
+
+    def __init__(self):
+        super().__init__()
+        stem = _make_trunk_layer('layer0')
+        for name, i in (('conv1', 0), ('bn1', 1), ('relu1', 2), ('conv2', 3), ('bn2', 4), ('relu2', 5),
+                        ('conv3', 6), ('bn3', 7), ('relu3', 8), ('maxpool', 9)):
+            setattr(self, name, stem[i])
+        for name in _TRUNK_LAYERS[1:]:
+            setattr(self, name, _make_trunk_layer(name))
+        _mit_semseg_init(self)
+
+    def _trunk(self):
+        return [[(self.conv1, self.bn1), (self.conv2, self.bn2), (self.conv3, self.bn3)], self.layer1, self.layer2,
+                self.layer3, self.layer4]
+
+    def forward(self, x, return_feature_maps=False):
+        """mit_semseg's forward: [conv5], or the outputs of layer1..layer4 when return_feature_maps; fp32 maps with
+        channels-last strides."""
+        outs = [h.permute(0, 3, 1, 2) for h in _run_trunk(self._trunk(), _rows(x))][1:]
+        return outs if return_feature_maps else [outs[-1]]
+
+
+class PPMFeatMap(nn.Module):
+    """Pyramid Pooling Module for feature extraction (image.py:659-716): mit_semseg's PPMDeepsup without the deep
+    supervision and the classifier.  forward(conv_out, out_size=None) runs on conv_out[-1] ([B, fc_dim, h, w] CUDA)
+    as one node (ops.rn_ppm_head) and returns [B, 512, h, w] fp32 with channels-last strides, resized to out_size
+    when given."""
+
+    def __init__(self, fc_dim=4096, pool_scales=(1, 2, 3, 6)):
+        super().__init__()
+        self.ppm = nn.ModuleList([nn.Sequential(FusedAdaptiveAvgPool2d(scale),
+                                                FusedConv2d(fc_dim, 512, kernel_size=1, bias=False),
+                                                PrudentSynchronizedBatchNorm2d(512), FusedReLU(inplace=True))
+                                  for scale in pool_scales])
+        self.conv_last = nn.Sequential(FusedConv2d(fc_dim + len(pool_scales) * 512, 512, kernel_size=3, padding=1,
+                                                   bias=False),
+                                       SynchronizedBatchNorm2d(512), FusedReLU(inplace=True))
+
+    def _check(self, B, h, w, out_size):
+        """ValueError, before any launch, where the reference's torch would raise; returns out_size as two ints."""
+        for m in self.ppm:
+            s = m[0].output_size
+            _check_bn_values(m[2], ops.ppm_branch_training(m[2], B, s), B, s, s)
+        _check_bn_values(self.conv_last[1], self.conv_last[1].training, B, h, w)
+        if out_size is None:
+            return None
+        if (not isinstance(out_size, (tuple, list, torch.Size)) or len(out_size) != 2
+                or not all(isinstance(v, int) and not isinstance(v, bool) and v > 0 for v in out_size)):
+            raise ValueError(f"out_size must be two positive ints, got {out_size!r}")
+        return tuple(out_size)
+
+    def forward(self, conv_out, *args, out_size=None, **kwargs):
+        conv5 = conv_out[-1]
+        require_cuda(conv5)
+        if conv5.dim() != 4 or conv5.shape[1] != self.ppm[0][1].in_channels:
+            raise ValueError(f"PPMFeatMap expects [B, {self.ppm[0][1].in_channels}, h, w] maps, got shape "
+                             f"{tuple(conv5.shape)}")
+        B, _, h, w = conv5.shape
+        out_size = self._check(B, h, w, out_size)
+        return ops.rn_ppm_head(_rows(conv5), self, out_size).permute(0, 3, 1, 2)
+
+
+def _mit_semseg_decoder_init(module):
+    """mit_semseg's ModelBuilder.weights_init: conv weights kaiming_normal_, BN weight 1 and bias 1e-4."""
+    for m in module.modules():
+        if isinstance(m, nn.Conv2d):
+            nn.init.kaiming_normal_(m.weight.data)
+        elif isinstance(m, nn.BatchNorm2d):
+            m.weight.data.fill_(1.)
+            m.bias.data.fill_(1e-4)
+
+
+def _mit_semseg_decoder_keys(fc_dim=512, num_class=150):
+    """Every key of mit_semseg's PPMDeepsup decoder_epoch_20.pth -> its shape; PPMFeatMap keeps ppm.* and
+    conv_last.0/1.*."""
+    keys = {k: tuple(v.shape) for k, v in PPMFeatMap(fc_dim).state_dict().items()}
+    keys['cbr_deepsup.0.weight'] = (fc_dim // 4, fc_dim // 2, 3, 3)
+    keys.update({f"cbr_deepsup.1.{k}": tuple(v.shape)
+                 for k, v in SynchronizedBatchNorm2d(fc_dim // 4).state_dict().items()})
+    keys.update({'conv_last.4.weight': (num_class, 512, 1, 1), 'conv_last.4.bias': (num_class,),
+                 'conv_last_deepsup.weight': (num_class, fc_dim // 4, 1, 1), 'conv_last_deepsup.bias': (num_class,)})
+    return keys
+
+
+def load_mit_semseg_decoder(module, state_dict):
+    """Load mit_semseg's PPMDeepsup decoder state dict (decoder_epoch_20.pth: ppm.*, cbr_deepsup.*, conv_last.*,
+    conv_last_deepsup.*) into a PPMFeatMap, or into the decoder of an ADE20KResNet18PPM, keeping what
+    PPMFeatMap.from_pretrained keeps: ppm and conv_last[:3].  The state dict must have exactly the checkpoint's keys;
+    a missing or extra key raises KeyError."""
+    decoder = getattr(module, 'decoder', module)
+    mapping = _mit_semseg_decoder_keys()
+    missing = sorted(set(mapping) - set(state_dict))
+    extra = sorted(set(state_dict) - set(mapping))
+    if missing or extra:
+        raise KeyError(f"not a mit_semseg ppm_deepsup decoder state dict: missing {missing[:5]}"
+                       f"{' ...' if len(missing) > 5 else ''}, unexpected {extra[:5]}"
+                       f"{' ...' if len(extra) > 5 else ''}")
+    keep = decoder.state_dict()
+    decoder.load_state_dict({k: v for k, v in state_dict.items() if k in keep}, strict=True)
+    return module
+
+
+class ADE20KResNet18PPM(nn.Module):
+    """ResNet-18 encoder with the PPM decoder pretrained on ADE20K (mit_semseg's resnet18dilated-ppm_deepsup,
+    image.py:719-790), on the sm_90a kernels of libdva_resnet.so and the gather pool of libdva_b200.so.
+
+    weights: None (mit_semseg's random initialisation of both halves) or (encoder, decoder), each a path to or the
+    state dict of encoder_epoch_20.pth (loaded into .encoder as it is) and decoder_epoch_20.pth
+    (load_mit_semseg_decoder).  `pretrained`, like any other unused config key, is swallowed: the reference always
+    loads the checkpoints from its own tree.
+    forward(x, out_size=None): x [B, 3, H, W] on CUDA, NCHW or channels-last; output [B, 512, h, w] with h =
+    ceil(ceil(ceil(H / 2) / 2) / 2) (the same for w), or [B, 512, *out_size], in the input's dtype (fp32 under
+    autocast) with channels-last strides.  Each BatchNorm runs in its own mode, except the Prudent rule of the
+    scale-1 branch at batch size 1."""
+
+    def __init__(self, *args, frozen=False, weights=None, **kwargs):
+        super().__init__()
+        self.encoder = ResnetDilated()
+        self.decoder = PPMFeatMap(fc_dim=512)
+        _mit_semseg_decoder_init(self.decoder)
+        if weights is not None:
+            enc, dec = [w if isinstance(w, dict) else torch.load(w, map_location='cpu') for w in weights]
+            self.encoder.load_state_dict(enc, strict=True)
+            load_mit_semseg_decoder(self, dec)
+
+        # If the model is frozen, it will always remain in eval mode and the parameters will have requires_grad=False
+        self.frozen = frozen
+        if self.frozen:
+            self.training = False
+
+    input_nc = 3
+    output_nc = 512
+
+    def forward(self, x, *args, out_size=None, **kwargs):
+        require_cuda(x)
+        if x.dim() != 4 or x.shape[1] != self.input_nc:
+            raise ValueError(f"ADE20KResNet18PPM expects [B, 3, H, W] images, got shape {tuple(x.shape)}")
+        B, _, H, W = x.shape
+        trunk = self.encoder._trunk()
+        for bn, h, w in _trunk_bn_sizes(trunk, H, W):
+            _check_bn_values(bn, bn.training, B, h, w)
+        out_size = self.decoder._check(B, h, w, out_size)
+        for conv5 in _run_trunk(trunk, _rows(x)):
+            pass
+        y = ops.rn_ppm_head(conv5, self.decoder, out_size)
+        return y.to(_out_dtype(x)).permute(0, 3, 1, 2)
+
+    @property
+    def frozen(self):
+        return self._frozen
+
+    @frozen.setter
+    def frozen(self, frozen):
+        if isinstance(frozen, bool):
+            self._frozen = frozen
+        for p in self.parameters():
+            p.requires_grad = not self.frozen
+
+    def train(self, mode=True):
+        return super().train(mode and not self.frozen)

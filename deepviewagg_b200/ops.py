@@ -2078,6 +2078,186 @@ def rn_maxpool(x):
     return _RNMaxPool.apply(x)
 
 
+# --------------------------------------------------------------------------------------------
+# The pyramid-pooling head of ADE20KResNet18PPM (modalities/image.py:658-716, PPMFeatMap): for each pool scale s,
+# adaptive average pool to s x s -> 1x1 conv -> BatchNorm -> ReLU -> bilinear resize back to h x w; the map and the
+# resized branches concatenated, then conv_last (3x3 conv -> BatchNorm -> ReLU).  All on existing kernels: the pool is
+# the mean gather pool of libdva_b200.so over an index of torch's bins, the rest libdva_resnet.so.
+# --------------------------------------------------------------------------------------------
+_PPM_INDEX = {}
+
+
+def _ppm_index(B, h, w, scales, device):
+    """The gather-pool index of the adaptive average pools at `scales` of a [B, h, w, C] map, built on the device and
+    cached per shape: one atom per (scale, image, bin), scale-major, so that the pooled rows of scale s are one
+    [B, s, s, C] block; an atom's pixels (x, y) are torch's bin [floor(i h / s), ceil((i + 1) h / s)) x
+    [floor(j w / s), ceil((j + 1) w / s)), row-major (bins overlap and repeat where s does not divide the side).
+    Returns (img [B * sum s^2] int64, pix [P, 2] int32, aptr int64, row offset of each scale)."""
+    key = (B, h, w, tuple(scales), str(device))
+    if key in _PPM_INDEX:
+        return _PPM_INDEX[key]
+    imgs, pixs, counts, offsets, off = [], [], [], [], 0
+    for s in scales:
+        i = torch.arange(s, device=device)
+        y0, y1 = (i * h) // s, ((i + 1) * h + s - 1) // s
+        x0, x1 = (i * w) // s, ((i + 1) * w + s - 1) // s
+        dy = torch.arange(int((y1 - y0).max()), device=device)
+        dx = torch.arange(int((x1 - x0).max()), device=device)
+        # [bin row, bin col, dy, dx] -> the pixels of each bin, row-major
+        y = (y0[:, None, None, None] + dy[None, None, :, None]).expand(s, s, dy.numel(), dx.numel())
+        x = (x0[None, :, None, None] + dx[None, None, None, :]).expand(s, s, dy.numel(), dx.numel())
+        keep = ((dy[None, None, :, None] < (y1 - y0)[:, None, None, None])
+                & (dx[None, None, None, :] < (x1 - x0)[None, :, None, None]))
+        pix = torch.stack([x[keep], y[keep]], dim=1).int()
+        n = ((y1 - y0)[:, None] * (x1 - x0)[None, :]).reshape(-1)
+        pixs.append(pix.repeat(B, 1))
+        counts.append(n.repeat(B))
+        imgs.append(torch.arange(B, device=device).repeat_interleave(s * s))
+        offsets.append(off)
+        off += B * s * s
+    counts = torch.cat(counts)
+    aptr = torch.zeros(counts.numel() + 1, dtype=torch.int64, device=device)
+    torch.cumsum(counts, 0, out=aptr[1:])
+    idx = (torch.cat(imgs).long().contiguous(), torch.cat(pixs).contiguous(), aptr, offsets)
+    _PPM_INDEX[key] = idx
+    return idx
+
+
+def ppm_branch_training(bn, B, s):
+    """Whether a pyramid branch's BatchNorm uses batch statistics: PrudentSynchronizedBatchNorm2d runs in eval mode
+    for a (1, C, 1, 1) input, so the scale-1 branch at batch size 1 never does."""
+    return bool(bn.training) and not (B == 1 and s == 1)
+
+
+class _RNPPMHead(torch.autograd.Function):
+    """PPMFeatMap on channels-last conv5 [B, h, w, C] as one node, with the final resize to out_size.  The concat
+    [B, h, w, C + 512 n] is one buffer: conv5 is copied into its first C columns and each branch is resized into its
+    own column slice.  Saves the concat, the pooled maps, the pre-activations, statistics and outputs of the five
+    BatchNorms and the data-gradient filters.  The pool's backward is the deterministic gather-pool backward, whatever
+    torch.use_deterministic_algorithms says: no sum of the head uses atomics."""
+
+    @staticmethod
+    @_fwd_f32
+    def forward(ctx, x, out_size, scales, branch_cfg, last_cfg, *params):
+        require_cuda(x, *params)
+        ctx.dtypes = [x.dtype] + [p.dtype for p in params]
+        B, h, w, C = x.shape
+        x = _rows_input(x, C)
+        n = len(scales)
+        ws_, gs, bs = _f32(*params[0:3 * n:3]), _f32(*params[1:3 * n:3]), _f32(*params[2:3 * n:3])
+        w_last, g_last, b_last = _f32(*params[3 * n:3 * n + 3])
+        running = params[3 * n + 3:]
+        dev = x.device
+        img, pix, aptr, offsets = _ppm_index(B, h, w, scales, dev)
+        Vw, P = img.numel(), pix.shape[0]
+        pooled = torch.empty(Vw, C, dtype=torch.float32, device=dev)
+        launch("dva_gather_pool_fwd", dev, x, 1, img, pix, 0, aptr, pooled, None, B, C, h, w, Vw, P,
+               REDUCE_CODES["mean"], dtype_code(x))
+        ld = C + sum(wk.shape[0] for wk in ws_)
+        cat = torch.empty(B, h, w, ld, dtype=torch.float32, device=dev)
+        cat[..., :C].copy_(x)
+        saved, col = [], C
+        for k, s in enumerate(scales):
+            training, momentum, eps = branch_cfg[k]
+            xs = pooled[offsets[k]:offsets[k] + B * s * s].view(B, s, s, C)
+            wf, wd = _rn_weights(ws_[k])
+            Co = ws_[k].shape[0]
+            z, mean, invstd = _rn_conv_bn(xs, wf, Co, (1, 1, 1), (running[2 * k], running[2 * k + 1], training,
+                                                                 momentum, eps))
+            y = _rn_apply(z, mean, invstd, gs[k], bs[k])
+            sh, sw = resize_scale(s, h), resize_scale(s, w)
+            launch("dva_resnet_resize", dev, y, B, s, s, Co, h, w, sh, sw, cat, ld, col)
+            saved += [wd, z, mean, invstd, y]
+            col += Co
+        wf, wd = _rn_weights(w_last)
+        training, momentum, eps = last_cfg
+        z, mean, invstd = _rn_conv_bn(cat, wf, w_last.shape[0], (3, 1, 1), (running[2 * n], running[2 * n + 1],
+                                                                           training, momentum, eps))
+        y = _rn_apply(z, mean, invstd, g_last, b_last)
+        out = y
+        if out_size is not None:
+            out = torch.empty(B, *out_size, y.shape[3], dtype=torch.float32, device=dev)
+            launch("dva_resnet_resize", dev, y, B, h, w, y.shape[3], out_size[0], out_size[1],
+                   resize_scale(h, out_size[0]), resize_scale(w, out_size[1]), out, y.shape[3], 0)
+        ctx.save_for_backward(pooled, cat, *gs, g_last, wd, z, mean, invstd, y, *saved)
+        ctx.cfg = (B, h, w, C, tuple(scales), offsets, [c[0] for c in branch_cfg], last_cfg[0], out_size)
+        return out
+
+    @staticmethod
+    @_bwd
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, dy):
+        B, h, w, C, scales, offsets, branch_training, last_training, out_size = ctx.cfg
+        n = len(scales)
+        pooled, cat, *rest = ctx.saved_tensors
+        gs, g_last, rest = rest[:n], rest[n], rest[n + 1:]
+        wd, z, mean, invstd, y = rest[:5]
+        branches = [rest[5 + 5 * k:10 + 5 * k] for k in range(n)]
+        need = ctx.needs_input_grad[5:]
+        dev = dy.device
+        dy = dy.float().contiguous()
+        Co = y.shape[3]
+        if out_size is not None:
+            dyh = torch.empty_like(y)
+            launch("dva_resnet_resize_bwd", dev, dy, Co, 0, B, h, w, Co, out_size[0], out_size[1],
+                   resize_scale(h, out_size[0]), resize_scale(w, out_size[1]), dyh)
+            dy = dyh
+        dz, _, dg_last, db_last = _rn_bn_bwd(dy, y, z, mean, invstd, g_last, last_training)
+        dw_last = _rn_wgrad(dz, cat, Co, (3, 1, 1)) if need[3 * n] else None
+        dcat = _rn_dgrad(dz, cat.shape, wd, (3, 1, 1))
+        del dz
+        ld = cat.shape[3]
+        dpooled = torch.empty_like(pooled) if ctx.needs_input_grad[0] else None
+        grads, col = [], C
+        for k, s in enumerate(scales):
+            wdk, zk, mk, ik, yk = branches[k]
+            Ck = yk.shape[3]
+            dyk = torch.empty_like(yk)
+            launch("dva_resnet_resize_bwd", dev, dcat, ld, col, B, s, s, Ck, h, w, resize_scale(s, h),
+                   resize_scale(s, w), dyk)
+            dzk, _, dgk, dbk = _rn_bn_bwd(dyk, yk, zk, mk, ik, gs[k], branch_training[k])
+            xs = pooled[offsets[k]:offsets[k] + B * s * s].view(B, s, s, C)
+            dwk = _rn_wgrad(dzk, xs, Ck, (1, 1, 1)) if need[3 * k] else None
+            if dpooled is not None:
+                dxs = dpooled[offsets[k]:offsets[k] + B * s * s].view(B, s, s, C)
+                _rn_dgrad(dzk, xs.shape, wdk, (1, 1, 1), out=dxs)
+            grads += [dwk, dgk, dbk]
+            col += Ck
+        dx = None
+        if dpooled is not None:
+            img, pix, aptr, _ = _ppm_index(B, h, w, scales, dev)
+            Vw, P = img.numel(), pix.shape[0]
+            dx = torch.empty(B, h, w, C, dtype=torch.float32, device=dev)
+            ws = _lib.workspace(_lib.load().dva_gather_pool_bwd_det_workspace_bytes(B, h, w, P), dev)
+            launch("dva_gather_pool_bwd_det", dev, dpooled, 1, img, pix, 0, aptr, None, dx, B, C, h, w, Vw, P,
+                   REDUCE_CODES["mean"], dtype_code(dpooled), ws, ws.numel())
+            dx += dcat[..., :C]
+        grads += [dw_last, dg_last, db_last]
+        dx, *grads = _as_dtypes([dx] + grads, ctx.dtypes)
+        n_running = len(ctx.needs_input_grad) - 5 - len(grads)
+        return (dx, None, None, None, None, *grads, *([None] * n_running))
+
+
+def rn_ppm_head(x, decoder, out_size=None):
+    """PPMFeatMap (`decoder`: .ppm[i] = (adaptive pool, 1x1 conv, Prudent BatchNorm, ReLU), .conv_last = (3x3 conv,
+    BatchNorm, ReLU)) on channels-last conv5 x [B, h, w, C]: fp32 [B, h, w, 512], or [B, *out_size, 512] after a
+    size-based bilinear resize.  Training-mode BatchNorms update their running stats; the scale-1 branch at batch
+    size 1 runs in eval mode (ppm_branch_training)."""
+    B = x.shape[0]
+    scales = [int(m[0].output_size if isinstance(m[0].output_size, int) else m[0].output_size[0])
+              for m in decoder.ppm]
+    conv, bn = decoder.conv_last[0], decoder.conv_last[1]
+    params, running, branch_cfg = [], [], []
+    for m, s in zip(decoder.ppm, scales):
+        params += [m[1].weight, m[2].weight, m[2].bias]
+        running += [m[2].running_mean, m[2].running_var]
+        branch_cfg.append((ppm_branch_training(m[2], B, s), m[2].momentum, m[2].eps))
+    params += [conv.weight, bn.weight, bn.bias]
+    running += [bn.running_mean, bn.running_var]
+    size = None if out_size is None else (int(out_size[0]), int(out_size[1]))
+    return _RNPPMHead.apply(x, size, scales, branch_cfg, _bn_cfg(bn), *params, *running)
+
+
 def rn_resize(xs, size, scale_factor=None):
     """Bilinear resizes (align_corners=False) of the channels-last maps xs to size (Ho, Wo), concatenated along the
     channels; scale_factor, when given, sets torch's source scale 1 / scale_factor (F.interpolate(scale_factor=))."""
