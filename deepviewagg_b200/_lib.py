@@ -190,6 +190,8 @@ RESNET_SIGNATURES = {
     "dva_resnet_bn_bwd": (_i32, [_vp, _vp, _vp, _i64, _i32, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "dva_resnet_maxpool": (_i32, [_vp, _i64, _i64, _i64, _i32, _vp, _vp, _vp]),
     "dva_resnet_maxpool_bwd": (_i32, [_vp, _vp, _i64, _i64, _i64, _i32, _vp, _vp]),
+    "dva_resnet_maxpool_pad": (_i32, [_vp, _i64, _i64, _i64, _i32, _i32, _vp, _vp, _vp]),
+    "dva_resnet_maxpool_pad_bwd": (_i32, [_vp, _vp, _i64, _i64, _i64, _i32, _i32, _vp, _vp]),
     "dva_resnet_resize": (_i32, [_vp, _i64, _i64, _i64, _i32, _i64, _i64, _f32, _f32, _vp, _i64, _i64, _vp]),
     "dva_resnet_resize_bwd": (_i32, [_vp, _i64, _i64, _i64, _i64, _i64, _i32, _i64, _i64, _f32, _f32, _vp, _vp]),
 }

@@ -1,6 +1,7 @@
-// The dilated ResNet-18 image encoder pretrained on ADE20K (libdva_resnet.so, C ABI include/dva_resnet.h):
-// zero-padded, strided and dilated convolutions with train-mode BatchNorm statistics in their epilogue, BatchNorm
-// apply / backward, the stem's max pool and the wrappers' bilinear resize.
+// The ResNet-18 image encoders (libdva_resnet.so, C ABI include/dva_resnet.h): the dilated ResNet-18 pretrained on
+// ADE20K, torchvision's ImageNet ResNet-18 (7x7 stem) and the Cityscapes one (unpadded max pool).  Zero-padded,
+// strided and dilated convolutions with train-mode BatchNorm statistics in their epilogue, BatchNorm apply /
+// backward, the stems' max pools and the wrappers' bilinear resize.
 //
 //   rn_weight_prep_kernel  w [Co][Ci][T][T] -> the forward's K-major filter and the data gradient's.
 //   rn_conv_gemm_kernel<MODE>  the main loop of conv2d_gemm.cuh (64 x 64 tiles, mma.sync in 3xTF32); the A operand
@@ -15,8 +16,9 @@
 //   rn_bn_apply_kernel  y = relu(BN(z) [+ skip] [+ BN_s(zs)]) in one pass.
 //   rn_bn_bwd_partial_kernel -> rn_bn_bwd_reduce_kernel -> rn_bn_bwd_dz_kernel  per-channel sums of g and g * zhat
 //        over pixel chunks (g = dy masked by the saved output), reduced in chunk order; dgamma, dbeta, dz.
-//   rn_maxpool_kernel / rn_maxpool_bwd_kernel  3x3 / 2 / 1 with the window position of the max; the backward is a
-//        gather over the <= 4 windows covering a pixel.
+//   rn_maxpool_kernel / rn_maxpool_bwd_kernel  3x3 / 2 with padding 1 or 0 and the window position of the max; the
+//        backward is a gather over the <= 4 windows covering a pixel (none for the last row / column that padding 0
+//        can leave out).
 //   rn_resize_kernel / rn_resize_bwd_kernel  bilinear, align_corners=False, torch's source index; the forward writes a
 //        column slice of a wider row, the backward gathers over the output pixels that read each input pixel.
 // Nothing that is summed uses atomics: every result is bitwise reproducible run to run.
@@ -286,14 +288,14 @@ rn_bn_bwd_dz_kernel(const float* __restrict__ dy, const float* __restrict__ y, c
 
 // one thread per output element; the window's first valid tap starts as the max (as torch's max_pool2d)
 __global__ void __launch_bounds__(kRedThreads)
-rn_maxpool_kernel(const float* __restrict__ x, int H, int W, int Ho, int Wo, int C, float* __restrict__ y,
+rn_maxpool_kernel(const float* __restrict__ x, int H, int W, int Ho, int Wo, int C, int pad, float* __restrict__ y,
                   uint8_t* __restrict__ arg, int64_t n) {
   for (int64_t e = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; e < n; e += (int64_t)gridDim.x * blockDim.x) {
     const int64_t pix = e / C;
     const int c = (int)(e - pix * C);
     const int64_t b = pix / ((int64_t)Ho * Wo);
     const int p = (int)(pix - b * Ho * Wo), oh = p / Wo, ow = p - oh * Wo;
-    const int h0 = 2 * oh - 1, w0 = 2 * ow - 1;
+    const int h0 = 2 * oh - pad, w0 = 2 * ow - pad;
     const float* xb = x + b * H * W * (int64_t)C + c;
     float mx = -INFINITY;
     int best = (h0 < 0 ? 3 : 0) + (w0 < 0 ? 1 : 0);
@@ -317,7 +319,7 @@ rn_maxpool_kernel(const float* __restrict__ x, int H, int W, int Ho, int Wo, int
 // one thread per input element: the windows (oh, ow) covering (ih, iw) in row-major order
 __global__ void __launch_bounds__(kRedThreads)
 rn_maxpool_bwd_kernel(const float* __restrict__ dy, const uint8_t* __restrict__ arg, int H, int W, int Ho, int Wo,
-                      int C, float* __restrict__ dx, int64_t n) {
+                      int C, int pad, float* __restrict__ dx, int64_t n) {
   for (int64_t e = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; e < n; e += (int64_t)gridDim.x * blockDim.x) {
     const int64_t pix = e / C;
     const int c = (int)(e - pix * C);
@@ -326,11 +328,11 @@ rn_maxpool_bwd_kernel(const float* __restrict__ dy, const uint8_t* __restrict__ 
     float v = 0.f;
 #pragma unroll
     for (int r = 2; r >= 0; --r) {
-      const int th = ih + 1 - r;
+      const int th = ih + pad - r;
       if (th < 0 || (th & 1) || th / 2 >= Ho) continue;
 #pragma unroll
       for (int s = 2; s >= 0; --s) {
-        const int tw = iw + 1 - s;
+        const int tw = iw + pad - s;
         if (tw < 0 || (tw & 1) || tw / 2 >= Wo) continue;
         const int64_t o = ((b * Ho + th / 2) * Wo + tw / 2) * C + c;
         if (arg[o] == r * 3 + s) v += dy[o];
@@ -427,11 +429,14 @@ rn_resize_bwd_kernel(const float* __restrict__ dy, int64_t ldy, int64_t col0, in
 
 // ---- host-side sizes
 inline int64_t out_size(int64_t n, int stride) { return (n - 1) / stride + 1; }
-inline int pad_of(int T, int dil) { return T == 3 ? dil : 0; }
+inline int pad_of(int T, int dil) { return dil * (T - 1) / 2; }
+// MaxPool2d(3, 2, pad): floor((n + 2 pad - 3) / 2) + 1, for n + 2 pad >= 3
+inline int64_t pool_out(int64_t n, int pad) { return (n + 2 * pad - 3) / 2 + 1; }
 
 inline int check_conv(const char* what, int64_t B, int64_t H, int64_t W, int Ci, int Co, int T, int stride, int dil) {
   const bool ok = (T == 3 && stride == 1 && (dil == 1 || dil == 2 || dil == 4)) ||
-                  (T == 3 && stride == 2 && dil == 1) || (T == 1 && (stride == 1 || stride == 2) && dil == 1);
+                  (T == 3 && stride == 2 && dil == 1) || (T == 1 && (stride == 1 || stride == 2) && dil == 1) ||
+                  (T == 7 && stride == 2 && dil == 1);
   if (!ok) return failf(DVA_EINVAL, "%s: unsupported shape (T %d, stride %d, dilation %d)", what, T, stride, dil);
   if (B < 1 || H < 1 || W < 1 || Ci < 1 || Co < 1) return failf(DVA_EINVAL, "%s: bad sizes", what);
   if ((int64_t)Co * T * T * Ci > (int64_t)INT32_MAX / 4 || H > INT32_MAX / 8 || W > INT32_MAX / 8)
@@ -472,7 +477,7 @@ using namespace dva;
 using namespace dva_resnet;
 
 extern "C" int dva_resnet_weight_prep(const float* w, int Co, int Ci, int T, float* wf, float* wd, void* stream) {
-  if (T != 1 && T != 3) return fail(DVA_EINVAL, "resnet_weight_prep: T must be 1 or 3");
+  if (T != 1 && T != 3 && T != 7) return fail(DVA_EINVAL, "resnet_weight_prep: T must be 1, 3 or 7");
   if (Co < 1 || Ci < 1) return fail(DVA_EINVAL, "resnet_weight_prep: bad sizes");
   if (!w || !wf || !wd) return fail(DVA_EINVAL, "resnet_weight_prep: null pointer");
   const int64_t n = (int64_t)Co * Ci * T * T;
@@ -528,7 +533,7 @@ extern "C" int dva_resnet_conv_dgrad(const float* dz, int64_t B, int64_t H, int6
 
 extern "C" size_t dva_resnet_wgrad_workspace_bytes(int64_t B, int64_t H, int64_t W, int Ci, int Co, int T, int stride,
                                                    int dil) {
-  if (B < 1 || H < 1 || W < 1 || Ci < 1 || Co < 1 || (T != 1 && T != 3) || stride < 1 || dil < 1) return 0;
+  if (B < 1 || H < 1 || W < 1 || Ci < 1 || Co < 1 || (T != 1 && T != 3 && T != 7) || stride < 1 || dil < 1) return 0;
   const WgradPlan p = wgrad_plan(B, H, W, Ci, Co, T, stride);
   return (size_t)p.splits * Co * p.Kd * sizeof(float);
 }
@@ -599,28 +604,45 @@ extern "C" int dva_resnet_bn_bwd(const float* dy, const float* y, const float* z
   return check_launch("resnet_bn_bwd_dz");
 }
 
+static int check_maxpool(const char* what, int64_t B, int64_t H, int64_t W, int C, int pad) {
+  if (pad != 0 && pad != 1) return failf(DVA_EINVAL, "%s: padding must be 0 or 1", what);
+  if (B < 1 || H < 1 || W < 1 || C < 1) return failf(DVA_EINVAL, "%s: bad sizes", what);
+  if (H + 2 * pad < 3 || W + 2 * pad < 3) return failf(DVA_EINVAL, "%s: input smaller than one window", what);
+  if (H > INT32_MAX / 4 || W > INT32_MAX / 4 || H * W > INT32_MAX)
+    return failf(DVA_EUNSUPPORTED, "%s: sizes beyond the 32-bit index range", what);
+  return DVA_OK;
+}
+
+extern "C" int dva_resnet_maxpool_pad(const float* x, int64_t B, int64_t H, int64_t W, int C, int pad, float* y,
+                                      uint8_t* arg, void* stream) {
+  const int rc = check_maxpool("resnet_maxpool", B, H, W, C, pad);
+  if (rc != DVA_OK) return rc;
+  if (!x || !y || !arg) return fail(DVA_EINVAL, "resnet_maxpool: null pointer");
+  const int64_t Ho = pool_out(H, pad), Wo = pool_out(W, pad), n = B * Ho * Wo * C;
+  rn_maxpool_kernel<<<elementwise_grid(n), kRedThreads, 0, (cudaStream_t)stream>>>(x, (int)H, (int)W, (int)Ho,
+                                                                                   (int)Wo, C, pad, y, arg, n);
+  return check_launch("resnet_maxpool");
+}
+
+extern "C" int dva_resnet_maxpool_pad_bwd(const float* dy, const uint8_t* arg, int64_t B, int64_t H, int64_t W, int C,
+                                          int pad, float* dx, void* stream) {
+  const int rc = check_maxpool("resnet_maxpool_bwd", B, H, W, C, pad);
+  if (rc != DVA_OK) return rc;
+  if (!dy || !arg || !dx) return fail(DVA_EINVAL, "resnet_maxpool_bwd: null pointer");
+  const int64_t n = B * H * W * C;
+  rn_maxpool_bwd_kernel<<<elementwise_grid(n), kRedThreads, 0, (cudaStream_t)stream>>>(
+      dy, arg, (int)H, (int)W, (int)pool_out(H, pad), (int)pool_out(W, pad), C, pad, dx, n);
+  return check_launch("resnet_maxpool_bwd");
+}
+
 extern "C" int dva_resnet_maxpool(const float* x, int64_t B, int64_t H, int64_t W, int C, float* y, uint8_t* arg,
                                   void* stream) {
-  if (B < 1 || H < 1 || W < 1 || C < 1) return fail(DVA_EINVAL, "resnet_maxpool: bad sizes");
-  if (H > INT32_MAX / 4 || W > INT32_MAX / 4 || H * W > INT32_MAX)
-    return fail(DVA_EUNSUPPORTED, "resnet_maxpool: sizes beyond the 32-bit index range");
-  if (!x || !y || !arg) return fail(DVA_EINVAL, "resnet_maxpool: null pointer");
-  const int64_t Ho = out_size(H, 2), Wo = out_size(W, 2), n = B * Ho * Wo * C;
-  rn_maxpool_kernel<<<elementwise_grid(n), kRedThreads, 0, (cudaStream_t)stream>>>(x, (int)H, (int)W, (int)Ho,
-                                                                                   (int)Wo, C, y, arg, n);
-  return check_launch("resnet_maxpool");
+  return dva_resnet_maxpool_pad(x, B, H, W, C, 1, y, arg, stream);
 }
 
 extern "C" int dva_resnet_maxpool_bwd(const float* dy, const uint8_t* arg, int64_t B, int64_t H, int64_t W, int C,
                                       float* dx, void* stream) {
-  if (B < 1 || H < 1 || W < 1 || C < 1) return fail(DVA_EINVAL, "resnet_maxpool_bwd: bad sizes");
-  if (H > INT32_MAX / 4 || W > INT32_MAX / 4 || H * W > INT32_MAX)
-    return fail(DVA_EUNSUPPORTED, "resnet_maxpool_bwd: sizes beyond the 32-bit index range");
-  if (!dy || !arg || !dx) return fail(DVA_EINVAL, "resnet_maxpool_bwd: null pointer");
-  const int64_t n = B * H * W * C;
-  rn_maxpool_bwd_kernel<<<elementwise_grid(n), kRedThreads, 0, (cudaStream_t)stream>>>(
-      dy, arg, (int)H, (int)W, (int)out_size(H, 2), (int)out_size(W, 2), C, dx, n);
-  return check_launch("resnet_maxpool_bwd");
+  return dva_resnet_maxpool_pad_bwd(dy, arg, B, H, W, C, 1, dx, stream);
 }
 
 static int check_resize(const char* what, int64_t B, int64_t H, int64_t W, int C, int64_t Ho, int64_t Wo,

@@ -571,6 +571,8 @@ class SynchronizedBatchNorm2d(nn.BatchNorm2d):
     F.batch_norm(x, running_mean, running_var, weight, bias, training, momentum, eps): num_batches_tracked never moves
     and the momentum is 0.001.  The three extra buffers are in the state dict and never touched on one device."""
 
+    steps_counter = False   # ops._bn_cfg: num_batches_tracked stays where it is
+
     def __init__(self, num_features, eps=1e-5, momentum=0.001, affine=True):
         super().__init__(num_features, eps=eps, momentum=momentum, affine=affine)
         self.register_buffer('_tmp_running_mean', torch.zeros(num_features))
@@ -580,6 +582,15 @@ class SynchronizedBatchNorm2d(nn.BatchNorm2d):
     def forward(self, input):
         raise NotImplementedError("SynchronizedBatchNorm2d runs fused with its convolution: call the "
                                   "ADE20KResNet18* module that holds it")
+
+
+class FusedBatchNorm2d(nn.BatchNorm2d):
+    """Parameters and buffers of a plain nn.BatchNorm2d of the ImageNet and Cityscapes trunks (momentum 0.1 or None,
+    num_batches_tracked += 1 per training forward, as torch's); it runs fused with its convolution."""
+
+    def forward(self, input):
+        raise NotImplementedError("FusedBatchNorm2d runs fused with its convolution: call the ResNet18* or "
+                                  "CityscapesResNet18* module that holds it")
 
 
 class FusedConv2d(nn.Conv2d):
@@ -599,13 +610,13 @@ class FusedReLU(nn.ReLU):
 
 
 class FusedMaxPool2d(nn.MaxPool2d):
-    """MaxPool2d(3, stride 2, padding 1) of the stem; run by the ADE20KResNet18* module that holds it."""
+    """MaxPool2d(3, stride 2, padding 1 or 0) of a stem; run by the ResNet-18 module that holds it."""
 
-    def __init__(self):
-        super().__init__(kernel_size=3, stride=2, padding=1)
+    def __init__(self, padding=1):
+        super().__init__(kernel_size=3, stride=2, padding=padding)
 
     def forward(self, input):
-        raise NotImplementedError("FusedMaxPool2d is run by the ADE20KResNet18* module that holds it")
+        raise NotImplementedError("FusedMaxPool2d is run by the ResNet-18 module that holds it")
 
 
 def _conv3x3(c_in, c_out, stride=1, dilation=1):
@@ -613,16 +624,17 @@ def _conv3x3(c_in, c_out, stride=1, dilation=1):
 
 
 class BasicBlock(nn.Module):
-    """mit_semseg's BasicBlock: relu(bn2(conv2(relu(bn1(conv1 x)))) + residual), the residual x or
-    downsample = (1x1 conv, BN).  Runs as one node (ops.rn_basic_block)."""
+    """mit_semseg's, torchvision's and the Cityscapes BasicBlock: relu(bn2(conv2(relu(bn1(conv1 x)))) + residual),
+    the residual x or downsample = (1x1 conv, BN); `norm` is the BatchNorm class.  Runs as one node
+    (ops.rn_basic_block)."""
 
-    def __init__(self, inplanes, planes, stride=1, dilation=(1, 1), downsample=None):
+    def __init__(self, inplanes, planes, stride=1, dilation=(1, 1), downsample=None, norm=SynchronizedBatchNorm2d):
         super().__init__()
         self.conv1 = _conv3x3(inplanes, planes, stride, dilation[0])
-        self.bn1 = SynchronizedBatchNorm2d(planes)
+        self.bn1 = norm(planes)
         self.relu = FusedReLU(inplace=True)
         self.conv2 = _conv3x3(planes, planes, 1, dilation[1])
-        self.bn2 = SynchronizedBatchNorm2d(planes)
+        self.bn2 = norm(planes)
         self.downsample = downsample
         self.stride = stride
 
@@ -630,15 +642,15 @@ class BasicBlock(nn.Module):
         return ops.rn_basic_block(x, self)
 
 
-def _make_layer(inplanes, planes, stride, dilations):
+def _make_layer(inplanes, planes, stride, dilations=(1, 1), norm=SynchronizedBatchNorm2d):
     """Two BasicBlocks as resnet18dilated has them after _nostride_dilate: dilations of (block 0 conv1, every other
     3x3); the downsample 1x1 has the block's stride."""
     ds = None
     if stride != 1 or inplanes != planes:
-        ds = nn.Sequential(FusedConv2d(inplanes, planes, kernel_size=1, stride=stride, bias=False),
-                           SynchronizedBatchNorm2d(planes))
+        ds = nn.Sequential(FusedConv2d(inplanes, planes, kernel_size=1, stride=stride, bias=False), norm(planes))
     d0, d = dilations
-    return nn.Sequential(BasicBlock(inplanes, planes, stride, (d0, d), ds), BasicBlock(planes, planes, 1, (d, d)))
+    return nn.Sequential(BasicBlock(inplanes, planes, stride, (d0, d), ds, norm),
+                         BasicBlock(planes, planes, 1, (d, d), norm=norm))
 
 
 def _make_trunk_layer(name):
@@ -704,16 +716,38 @@ def _check_bn_values(bn, training, B, H, W):
                          f"{[B, bn.num_features, H, W]}")
 
 
-# A trunk as _run_trunk walks it: a list of layers, each the stem -- a list of three (conv, BatchNorm) units, then the
-# max pool -- or a Sequential of BasicBlocks.
+# A trunk as _run_trunk walks it: a list of layers, each the stem -- a list of (conv, BatchNorm) units, then the
+# max pool, of padding `pool_padding` (1 when the list does not say) -- or a Sequential of BasicBlocks.
+class _Stem(list):
+    """A stem's (conv, BatchNorm) units in order, and the padding of the max pool after them."""
+
+    def __init__(self, units, pool_padding):
+        super().__init__(units)
+        self.pool_padding = pool_padding
+
+
+def _stem_of(layer):
+    """The stem Sequential of a wrapper (nested Sequentials flattened: convs, BatchNorms, ReLUs, then the max pool) as
+    _run_trunk walks it."""
+    mods = [m for m in layer.modules() if not isinstance(m, nn.Sequential)]
+    convs = [m for m in mods if isinstance(m, nn.Conv2d)]
+    bns = [m for m in mods if isinstance(m, nn.BatchNorm2d)]
+    return _Stem(list(zip(convs, bns)), mods[-1].padding)
+
+
+def _pool_padding(stem):
+    return getattr(stem, 'pool_padding', 1)
+
+
 def _trunk_bn_sizes(trunk, H, W):
-    """Yields (BatchNorm, H, W of the map it normalises) along the trunk for an H x W input."""
+    """Yields (BatchNorm, H, W of the map it normalises) along the trunk for an H x W input; ValueError when a max
+    pool would get a map smaller than its window."""
     for layer in trunk:
         if isinstance(layer, list):
             for conv, bn in layer:
                 H, W = ops.rn_out(H, conv.stride[0]), ops.rn_out(W, conv.stride[0])
                 yield bn, H, W
-            H, W = ops.rn_out(H, 2), ops.rn_out(W, 2)
+            H, W = ops.rn_pool_out(H, _pool_padding(layer)), ops.rn_pool_out(W, _pool_padding(layer))
         else:
             for block in layer:
                 H, W = ops.rn_out(H, block.conv1.stride[0]), ops.rn_out(W, block.conv1.stride[0])
@@ -729,37 +763,25 @@ def _run_trunk(trunk, h):
         if isinstance(layer, list):
             for conv, bn in layer:
                 h = ops.rn_conv_bn_relu(h, conv, bn)
-            h = ops.rn_maxpool(h)
+            h = ops.rn_maxpool(h, _pool_padding(layer))
         else:
             for block in layer:
                 h = ops.rn_basic_block(h, block)
         yield h
 
 
-class ADE20KResNet18TruncatedLayer4(nn.Module):
-    """ResNet-18 encoder pretrained on ADE20K (mit_semseg's resnet18dilated), truncated after `_LAYERS`
-    (image.py:793-898), on the sm_90a kernels of libdva_resnet.so.
+def _load_weights(weights):
+    """A state dict, or the file at `weights` loaded on the CPU."""
+    return weights if isinstance(weights, dict) else torch.load(weights, map_location='cpu')
 
-    weights: None (mit_semseg's random initialisation), a path to mit_semseg's encoder_epoch_20.pth or its state
-    dict (load_mit_semseg_encoder).  The reference always loads that checkpoint from its own tree.
-    Input [B, 3, H, W] on CUDA (input_nc channels), NCHW or channels-last; output [B, output_nc, H', W'] in the
-    input's dtype (fp32 under autocast) with channels-last strides.  Each BatchNorm runs in its own mode (its
-    .training): batch statistics and a running-stat update (momentum 0.001) in training mode, the running stats in
-    eval mode."""
-    _LAYERS = ['layer0', 'layer1', 'layer2', 'layer3', 'layer4']
-    _LAYERS_IN = {k: v for k, v in zip(_TRUNK_LAYERS, [3, 128, 64, 128, 256])}
-    _LAYERS_OUT = {k: v for k, v in zip(_TRUNK_LAYERS, [128, 64, 128, 256, 512])}
-    _LAYERS_SCALE = {k: v for k, v in zip(_TRUNK_LAYERS, [4, 1, 2, 1, 1])}
 
-    def __init__(self, frozen=False, scale_factor=None, weights=None, **kwargs):
-        super().__init__()
-        self.conv = nn.Sequential(*[_make_trunk_layer(layer) for layer in self._LAYERS])
-        _mit_semseg_init(self.conv)
-        if weights is not None:
-            if not isinstance(weights, dict):
-                weights = torch.load(weights, map_location='cpu')
-            load_mit_semseg_encoder(self, weights)
+class _ResNet18Wrapper(nn.Module):
+    """What the reference's ResNet-18 wrappers share (ADE20KResNet18*, ResNet18*, CityscapesResNet18*): `frozen` and
+    train(), scale_factor (< 0: conv_scale_factor), input_nc / output_nc / conv_scale_factor, the input checks and
+    the trunk walk over self.conv.  A subclass builds self.conv (its _LAYERS) and calls _setup."""
+    _LAYERS = _TRUNK_LAYERS
 
+    def _setup(self, frozen, scale_factor):
         # If the model is frozen, it will always remain in eval mode and the parameters will have requires_grad=False
         self.frozen = frozen
         if self.frozen:
@@ -779,16 +801,18 @@ class ADE20KResNet18TruncatedLayer4(nn.Module):
         for bn, H, W in self._bn_sizes(H, W):
             _check_bn_values(bn, bn.training, B, H, W)
 
+    def _trunk_modules(self):
+        return self.conv
+
     def _trunk(self):
-        return [layer if isinstance(layer[0], BasicBlock) else [(layer[i], layer[i + 1]) for i in (0, 3, 6)]
-                for layer in self.conv]
+        return [layer if isinstance(layer[0], BasicBlock) else _stem_of(layer) for layer in self._trunk_modules()]
 
     def _bn_sizes(self, H, W):
         """Yields (BatchNorm, H, W of the map it normalises) along the trunk for an H x W input."""
         return _trunk_bn_sizes(self._trunk(), H, W)
 
     def _layers(self, h):
-        """Yields the channels-last output of each layer of self.conv for channels-last rows h."""
+        """Yields the channels-last output of each layer of the trunk for channels-last rows h."""
         return _run_trunk(self._trunk(), h)
 
     def forward(self, x, *args, **kwargs):
@@ -830,6 +854,46 @@ class ADE20KResNet18TruncatedLayer4(nn.Module):
         return f"scale_factor={self.scale_factor}" if self.scale_factor is not None else ""
 
 
+class _Pyramid:
+    """The Pyramid forward of the wrappers: every layer's output resized to int(side * scale_factor /
+    conv_scale_factor) of the input sides (a size-based bilinear resize) and concatenated along the channels,
+    written into one buffer."""
+
+    def __init__(self, frozen=False, scale_factor=-1, **kwargs):
+        assert scale_factor is not None, f'scale_factor cannot be None for feature pyramid.'
+        super().__init__(frozen=frozen, scale_factor=scale_factor, **kwargs)
+
+    def forward(self, x, *args, **kwargs):
+        self._check_input(x)
+        size = [int(s * self.scale_factor / self.conv_scale_factor) for s in x.shape[2:4]]
+        h = ops.rn_resize(list(self._layers(_rows(x))), size)
+        return h.to(_out_dtype(x)).permute(0, 3, 1, 2)
+
+
+class ADE20KResNet18TruncatedLayer4(_ResNet18Wrapper):
+    """ResNet-18 encoder pretrained on ADE20K (mit_semseg's resnet18dilated), truncated after `_LAYERS`
+    (image.py:793-898), on the sm_90a kernels of libdva_resnet.so.
+
+    weights: None (mit_semseg's random initialisation), a path to mit_semseg's encoder_epoch_20.pth or its state
+    dict (load_mit_semseg_encoder).  The reference always loads that checkpoint from its own tree.
+    Input [B, 3, H, W] on CUDA (input_nc channels), NCHW or channels-last; output [B, output_nc, H', W'] in the
+    input's dtype (fp32 under autocast) with channels-last strides.  Each BatchNorm runs in its own mode (its
+    .training): batch statistics and a running-stat update (momentum 0.001) in training mode, the running stats in
+    eval mode."""
+    _LAYERS = ['layer0', 'layer1', 'layer2', 'layer3', 'layer4']
+    _LAYERS_IN = {k: v for k, v in zip(_TRUNK_LAYERS, [3, 128, 64, 128, 256])}
+    _LAYERS_OUT = {k: v for k, v in zip(_TRUNK_LAYERS, [128, 64, 128, 256, 512])}
+    _LAYERS_SCALE = {k: v for k, v in zip(_TRUNK_LAYERS, [4, 1, 2, 1, 1])}
+
+    def __init__(self, frozen=False, scale_factor=None, weights=None, **kwargs):
+        super().__init__()
+        self.conv = nn.Sequential(*[_make_trunk_layer(layer) for layer in self._LAYERS])
+        _mit_semseg_init(self.conv)
+        if weights is not None:
+            load_mit_semseg_encoder(self, _load_weights(weights))
+        self._setup(frozen, scale_factor)
+
+
 class ADE20KResNet18TruncatedLayer0(ADE20KResNet18TruncatedLayer4):
     _LAYERS = ['layer0']
 
@@ -866,19 +930,247 @@ class ADE20KResNet18Layer4(ADE20KResNet18TruncatedLayer4):
     _LAYERS = ['layer4']
 
 
-class ADE20KResNet18Pyramid(ADE20KResNet18TruncatedLayer4):
-    """Every layer's output resized to int(side * scale_factor / conv_scale_factor) of the input sides (a size-based
-    bilinear resize) and concatenated: 128 + 64 + 128 + 256 + 512 = 1088 channels, written into one buffer."""
+class ADE20KResNet18Pyramid(_Pyramid, ADE20KResNet18TruncatedLayer4):
+    """Every layer's output resized to int(side * scale_factor / conv_scale_factor) of the input sides and
+    concatenated: 128 + 64 + 128 + 256 + 512 = 1088 channels, written into one buffer."""
 
-    def __init__(self, frozen=False, scale_factor=-1, **kwargs):
-        assert scale_factor is not None, f'scale_factor cannot be None for feature pyramid.'
-        super().__init__(frozen=frozen, scale_factor=scale_factor, **kwargs)
 
-    def forward(self, x, *args, **kwargs):
-        self._check_input(x)
-        size = [int(s * self.scale_factor / self.conv_scale_factor) for s in x.shape[2:4]]
-        h = ops.rn_resize(list(self._layers(_rows(x))), size)
-        return h.to(_out_dtype(x)).permute(0, 3, 1, 2)
+# --------------------------------------------------------------------------------------------------------------------
+# torchvision's ImageNet ResNet-18 (ResNet18*, image.py:959-1126) and the Cityscapes ResNet-18 of SFSegNets
+# (CityscapesResNet18*, image.py:1129-1399) on the same kernels and trunk walk.  Both use plain nn.BatchNorm2d
+# (momentum 0.1, num_batches_tracked += 1 per training forward) and no dilation.  ImageNet layer0 is (7x7/2 conv, BN,
+# ReLU, MaxPool2d(3, 2, 1)); Cityscapes layer0 is (Sequential(3x3/2 conv, BN, ReLU, 3x3 conv, BN, ReLU, 3x3 conv),
+# BN, ReLU, MaxPool2d(3, 2, 0)), whose last row and column can belong to no window.
+# --------------------------------------------------------------------------------------------------------------------
+def _make_imagenet_layer(name):
+    if name == 'layer0':
+        return nn.Sequential(FusedConv2d(3, 64, kernel_size=7, stride=2, padding=3, bias=False), FusedBatchNorm2d(64),
+                             FusedReLU(inplace=True), FusedMaxPool2d(padding=1))
+    inplanes, planes, stride = {'layer1': (64, 64, 1), 'layer2': (64, 128, 2), 'layer3': (128, 256, 2),
+                                'layer4': (256, 512, 2)}[name]
+    return _make_layer(inplanes, planes, stride, norm=FusedBatchNorm2d)
+
+
+def _make_cityscapes_layer(name):
+    if name == 'layer0':
+        stem = nn.Sequential(_conv3x3(3, 64, stride=2), FusedBatchNorm2d(64), FusedReLU(inplace=True),
+                             _conv3x3(64, 64), FusedBatchNorm2d(64), FusedReLU(inplace=True), _conv3x3(64, 128))
+        return nn.Sequential(stem, FusedBatchNorm2d(128), FusedReLU(inplace=True), FusedMaxPool2d(padding=0))
+    inplanes, planes, stride = {'layer1': (128, 64, 1), 'layer2': (64, 128, 2), 'layer3': (128, 256, 2),
+                                'layer4': (256, 512, 2)}[name]
+    return _make_layer(inplanes, planes, stride, norm=FusedBatchNorm2d)
+
+
+def _kaiming_init(module):
+    """torchvision's and SFSegNets' initialisation: conv weights kaiming_normal_ (fan_out, relu), BN weight 1 and
+    bias 0."""
+    for m in module.modules():
+        if isinstance(m, nn.Conv2d):
+            nn.init.kaiming_normal_(m.weight, mode='fan_out', nonlinearity='relu')
+        elif isinstance(m, nn.BatchNorm2d):
+            nn.init.constant_(m.weight, 1)
+            nn.init.constant_(m.bias, 0)
+
+
+def _check_keys(what, expected, state_dict, optional=()):
+    """KeyError unless state_dict has every key of `expected` and nothing outside expected | optional."""
+    missing = sorted(set(expected) - set(state_dict))
+    extra = sorted(set(state_dict) - set(expected) - set(optional))
+    if missing or extra:
+        raise KeyError(f"not a {what} state dict: missing {missing[:5]}{' ...' if len(missing) > 5 else ''}, "
+                       f"unexpected {extra[:5]}{' ...' if len(extra) > 5 else ''}")
+
+
+def _load_layers(module, state_dict):
+    """Load {layer name: {key inside the layer: tensor}} into the layers `module` holds (conv.<i>.* of a wrapper,
+    layer<i>.* of CityscapesResNet18) with strict=True."""
+    position = {name: i for i, name in enumerate(module._LAYERS)}
+    prefix = (lambda name: f"conv.{position[name]}.") if hasattr(module, 'conv') else (lambda name: f"{name}.")
+    module.load_state_dict({prefix(layer) + k: v for (layer, k), v in state_dict.items() if layer in position},
+                           strict=True)
+    return module
+
+
+def _torchvision_resnet18_keys():
+    """Every key of torchvision's resnet18 state dict -> (layer, key inside that layer of the wrapper); fc -> None."""
+    keys = {'fc.weight': None, 'fc.bias': None}
+    for name in _TRUNK_LAYERS:
+        for k in _make_imagenet_layer(name).state_dict():
+            if name == 'layer0':
+                head, rest = k.split('.', 1)
+                keys[f"{ {'0': 'conv1', '1': 'bn1'}[head]}.{rest}"] = (name, k)
+            else:
+                keys[f"{name}.{k}"] = (name, k)
+    return keys
+
+
+def load_torchvision_resnet18(module, state_dict):
+    """Load torchvision's ImageNet resnet18 state dict (conv1, bn1, layer1..layer4, fc) into the layers a ResNet18*
+    module holds; fc is dropped.  The state dict must have exactly torchvision's keys, except that
+    num_batches_tracked may be missing, as in checkpoints saved before torch 0.4.1: those counters are left as they
+    are, as torch's BatchNorm loads such a checkpoint.  A missing or extra key raises KeyError."""
+    mapping = _torchvision_resnet18_keys()
+    counters = [k for k in mapping if k.endswith('.num_batches_tracked')]
+    _check_keys("torchvision resnet18", [k for k in mapping if k not in counters], state_dict, counters)
+    own = module.state_dict()
+    position = {name: i for i, name in enumerate(module._LAYERS)}
+    return _load_layers(module, {target: state_dict[key] if key in state_dict else
+                                 own[f"conv.{position[target[0]]}.{target[1]}"]
+                                 for key, target in mapping.items() if target is not None and target[0] in position})
+
+
+def _cityscapes_resnet18_keys():
+    """Every key of SFSegNets' resnet18_SFSegNets.pth (CityscapesResNet18's state dict) -> (layer, key inside it)."""
+    return {f"{name}.{k}": (name, k) for name in _TRUNK_LAYERS for k in _make_cityscapes_layer(name).state_dict()}
+
+
+def load_cityscapes_resnet18(module, state_dict):
+    """Load SFSegNets' Cityscapes ResNet-18 state dict (resnet18_SFSegNets.pth: layer0.0.0.weight, ...,
+    layer4.1.bn2.*, 138 keys) into CityscapesResNet18 or the layers a CityscapesResNet18* module holds.  The state
+    dict must have exactly those keys; a missing or extra key raises KeyError."""
+    mapping = _cityscapes_resnet18_keys()
+    _check_keys("Cityscapes ResNet-18 (resnet18_SFSegNets.pth)", mapping, state_dict)
+    return _load_layers(module, {target: state_dict[key] for key, target in mapping.items()})
+
+
+class ResNet18TruncatedLayer4(_ResNet18Wrapper):
+    """torchvision's ImageNet ResNet-18, truncated after `_LAYERS` (image.py:992-1066), on the sm_90a kernels of
+    libdva_resnet.so; layer0 is (conv1 7x7/2, bn1, relu, maxpool 3/2/1).
+
+    weights: None (torchvision's random initialisation), a path to torchvision's resnet18 state dict or the dict
+    (load_torchvision_resnet18).  `pretrained`, like any other unused config key, is swallowed: the reference loads
+    the checkpoint from its own tree.  Input [B, 3, H, W] on CUDA (input_nc channels), NCHW or channels-last; output
+    [B, output_nc, H', W'] in the input's dtype (fp32 under autocast) with channels-last strides.  Each BatchNorm
+    runs in its own mode: batch statistics, a running-stat update with its momentum (None: the cumulative average)
+    and num_batches_tracked += 1 in training mode, the running stats in eval mode."""
+    _LAYERS_IN = {k: v for k, v in zip(_TRUNK_LAYERS, [3, 64, 64, 128, 256])}
+    _LAYERS_OUT = {k: v for k, v in zip(_TRUNK_LAYERS, [64, 64, 128, 256, 512])}
+    _LAYERS_SCALE = {k: v for k, v in zip(_TRUNK_LAYERS, [4, 1, 2, 2, 2])}
+    _make = staticmethod(_make_imagenet_layer)
+    _load = staticmethod(load_torchvision_resnet18)
+
+    def __init__(self, frozen=False, scale_factor=None, weights=None, **kwargs):
+        super().__init__()
+        self.conv = nn.Sequential(*[self._make(layer) for layer in self._LAYERS])
+        _kaiming_init(self.conv)
+        if weights is not None:
+            self._load(self, _load_weights(weights))
+        self._setup(frozen, scale_factor)
+
+
+class ResNet18TruncatedLayer0(ResNet18TruncatedLayer4):
+    _LAYERS = ['layer0']
+
+
+class ResNet18TruncatedLayer1(ResNet18TruncatedLayer4):
+    _LAYERS = ['layer0', 'layer1']
+
+
+class ResNet18TruncatedLayer2(ResNet18TruncatedLayer4):
+    _LAYERS = ['layer0', 'layer1', 'layer2']
+
+
+class ResNet18TruncatedLayer3(ResNet18TruncatedLayer4):
+    _LAYERS = ['layer0', 'layer1', 'layer2', 'layer3']
+
+
+class ResNet18Layer0(ResNet18TruncatedLayer4):
+    _LAYERS = ['layer0']
+
+
+class ResNet18Layer1(ResNet18TruncatedLayer4):
+    _LAYERS = ['layer1']
+
+
+class ResNet18Layer2(ResNet18TruncatedLayer4):
+    _LAYERS = ['layer2']
+
+
+class ResNet18Layer3(ResNet18TruncatedLayer4):
+    _LAYERS = ['layer3']
+
+
+class ResNet18Layer4(ResNet18TruncatedLayer4):
+    _LAYERS = ['layer4']
+
+
+class ResNet18Pyramid(_Pyramid, ResNet18TruncatedLayer4):
+    """Every layer's output resized to the input size (scale_factor -1) and concatenated: 64 + 64 + 128 + 256 + 512 =
+    1024 channels, written into one buffer."""
+
+
+class CityscapesResNet18TruncatedLayer4(ResNet18TruncatedLayer4):
+    """The Cityscapes ResNet-18 of SFSegNets, truncated after `_LAYERS` (image.py:1268-1339); layer0 is
+    (Sequential(conv 3x3/2, bn, relu, conv, bn, relu, conv), bn, relu, maxpool 3/2/0).  The maxpool keeps
+    floor((side - 3) / 2) + 1 of each side, so an image whose stem output is smaller than 3 raises ValueError.
+
+    weights: None (SFSegNets' random initialisation), a path to resnet18_SFSegNets.pth or its state dict
+    (load_cityscapes_resnet18).  Otherwise as ResNet18TruncatedLayer4."""
+    _LAYERS_IN = {k: v for k, v in zip(_TRUNK_LAYERS, [3, 128, 64, 128, 256])}
+    _LAYERS_OUT = {k: v for k, v in zip(_TRUNK_LAYERS, [128, 64, 128, 256, 512])}
+    _make = staticmethod(_make_cityscapes_layer)
+    _load = staticmethod(load_cityscapes_resnet18)
+
+
+class CityscapesResNet18TruncatedLayer0(CityscapesResNet18TruncatedLayer4):
+    _LAYERS = ['layer0']
+
+
+class CityscapesResNet18TruncatedLayer1(CityscapesResNet18TruncatedLayer4):
+    _LAYERS = ['layer0', 'layer1']
+
+
+class CityscapesResNet18TruncatedLayer2(CityscapesResNet18TruncatedLayer4):
+    _LAYERS = ['layer0', 'layer1', 'layer2']
+
+
+class CityscapesResNet18TruncatedLayer3(CityscapesResNet18TruncatedLayer4):
+    _LAYERS = ['layer0', 'layer1', 'layer2', 'layer3']
+
+
+class CityscapesResNet18Layer0(CityscapesResNet18TruncatedLayer4):
+    _LAYERS = ['layer0']
+
+
+class CityscapesResNet18Layer1(CityscapesResNet18TruncatedLayer4):
+    _LAYERS = ['layer1']
+
+
+class CityscapesResNet18Layer2(CityscapesResNet18TruncatedLayer4):
+    _LAYERS = ['layer2']
+
+
+class CityscapesResNet18Layer3(CityscapesResNet18TruncatedLayer4):
+    _LAYERS = ['layer3']
+
+
+class CityscapesResNet18Layer4(CityscapesResNet18TruncatedLayer4):
+    _LAYERS = ['layer4']
+
+
+class CityscapesResNet18Pyramid(_Pyramid, CityscapesResNet18TruncatedLayer4):
+    """Every layer's output resized to the input size (scale_factor -1) and concatenated: 128 + 64 + 128 + 256 + 512
+    = 1088 channels, written into one buffer."""
+
+
+class CityscapesResNet18(CityscapesResNet18TruncatedLayer4):
+    """The whole Cityscapes ResNet-18 under SFSegNets' names (image.py:1175-1265): layer0..layer4 attributes, so
+    resnet18_SFSegNets.pth loads into it as it is; forward returns layer4's output (/32), without resize."""
+
+    def __init__(self, *args, frozen=False, weights=None, **kwargs):
+        nn.Module.__init__(self)
+        for name in _TRUNK_LAYERS:
+            setattr(self, name, _make_cityscapes_layer(name))
+        _kaiming_init(self)
+        if weights is not None:
+            load_cityscapes_resnet18(self, _load_weights(weights))
+        self._setup(frozen, None)
+
+    def _trunk_modules(self):
+        return [getattr(self, name) for name in _TRUNK_LAYERS]
+
+    def extra_repr(self) -> str:
+        return ""
 
 
 # --------------------------------------------------------------------------------------------------------------------

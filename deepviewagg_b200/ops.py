@@ -1883,7 +1883,13 @@ def _rn_dgrad(dz, x_shape, wd, geo, add=None, out=None):
 
 
 def _bn_cfg(bn):
-    return (bn.training, bn.momentum, bn.eps)
+    """(training, momentum, eps) of bn for one forward.  A plain nn.BatchNorm2d (the ImageNet and Cityscapes trunks)
+    gets torch's bookkeeping here, in the module's forward, as _bn_step does it: num_batches_tracked += 1 in training
+    (so a reentrant checkpoint's recompute counts twice, as torch's module does) and momentum None as the cumulative
+    average.  mit_semseg's SynchronizedBatchNorm2d (steps_counter False) never moves its counter."""
+    if not getattr(bn, "steps_counter", True):
+        return (bn.training, bn.momentum, bn.eps)
+    return (bn.training, _bn_step(bn)[2], bn.eps)
 
 
 class _RNConvBNReLU(torch.autograd.Function):
@@ -1975,21 +1981,31 @@ class _RNBasicBlock(torch.autograd.Function):
         return (*_as_dtypes(grads, ctx.dtypes), *([None] * 7))
 
 
+def rn_pool_out(n, padding=1):
+    """Output side of the stems' MaxPool2d(3, 2, padding), padding 1 (ceil(n / 2)) or 0 (floor((n - 3) / 2) + 1);
+    ValueError when n + 2 padding < 3 leaves no window."""
+    if padding not in (0, 1):
+        raise ValueError(f"max pool padding must be 0 or 1, got {padding!r}")
+    if n + 2 * padding < 3:
+        raise ValueError(f"MaxPool2d(3, 2, {padding}): input side {n} is smaller than one window")
+    return (n + 2 * padding - 3) // 2 + 1
+
+
 class _RNMaxPool(torch.autograd.Function):
-    """MaxPool2d(3, stride 2, padding 1) with the window position of the max saved for the backward."""
+    """MaxPool2d(3, stride 2, padding 1 or 0) with the window position of the max saved for the backward."""
 
     @staticmethod
     @_fwd_f32
-    def forward(ctx, x):
+    def forward(ctx, x, padding):
         require_cuda(x)
         ctx.dtype = x.dtype
         x = x.float().contiguous()
         B, H, W, C = x.shape
-        y = torch.empty(B, rn_out(H, 2), rn_out(W, 2), C, dtype=torch.float32, device=x.device)
+        y = torch.empty(B, rn_pool_out(H, padding), rn_pool_out(W, padding), C, dtype=torch.float32, device=x.device)
         arg = torch.empty(y.shape, dtype=torch.uint8, device=x.device)
-        launch("dva_resnet_maxpool", x.device, x, B, H, W, C, y, arg)
+        launch("dva_resnet_maxpool_pad", x.device, x, B, H, W, C, padding, y, arg)
         ctx.save_for_backward(arg)
-        ctx.shape = (B, H, W, C)
+        ctx.cfg = (B, H, W, C, padding)
         ctx.mark_non_differentiable(arg)
         return y
 
@@ -1998,10 +2014,10 @@ class _RNMaxPool(torch.autograd.Function):
     @torch.autograd.function.once_differentiable
     def backward(ctx, dy):
         (arg,) = ctx.saved_tensors
-        B, H, W, C = ctx.shape
+        B, H, W, C, padding = ctx.cfg
         dx = torch.empty(B, H, W, C, dtype=torch.float32, device=dy.device)
-        launch("dva_resnet_maxpool_bwd", dy.device, dy.float().contiguous(), arg, B, H, W, C, dx)
-        return dx.to(ctx.dtype)
+        launch("dva_resnet_maxpool_pad_bwd", dy.device, dy.float().contiguous(), arg, B, H, W, C, padding, dx)
+        return dx.to(ctx.dtype), None
 
 
 def resize_scale(n_in, n_out, scale_factor=None):
@@ -2073,9 +2089,10 @@ def rn_basic_block(x, block):
                                nd.running_var if nd is not None else None, cfg)
 
 
-def rn_maxpool(x):
-    """MaxPool2d(3, 2, 1) of channels-last x [B, H, W, C]: fp32 [B, ceil(H/2), ceil(W/2), C]."""
-    return _RNMaxPool.apply(x)
+def rn_maxpool(x, padding=1):
+    """MaxPool2d(3, 2, padding) of channels-last x [B, H, W, C], padding 1 (the ADE20K and ImageNet stems) or 0 (the
+    Cityscapes stem): fp32 [B, rn_pool_out(H, padding), rn_pool_out(W, padding), C]."""
+    return _RNMaxPool.apply(x, padding)
 
 
 # --------------------------------------------------------------------------------------------

@@ -1,7 +1,8 @@
 /*
- * dva_resnet.h -- C ABI of libdva_resnet.so: the dilated ResNet-18 image encoder pretrained on ADE20K (mit_semseg's
- * resnet18dilated behind the reference's ADE20KResNet18* wrappers) on the H100 (sm_90a): zero-padded convolutions
- * with the BatchNorm statistics in their epilogue, train- and eval-mode BatchNorm, the 3x3 stride-2 max pool and the
+ * dva_resnet.h -- C ABI of libdva_resnet.so: the ResNet-18 image encoders on the H100 (sm_90a) -- the dilated one
+ * pretrained on ADE20K (mit_semseg's resnet18dilated behind the reference's ADE20KResNet18* wrappers), torchvision's
+ * ImageNet one (ResNet18*) and the Cityscapes one (CityscapesResNet18*): zero-padded convolutions with the BatchNorm
+ * statistics in their epilogue, train- and eval-mode BatchNorm, the 3x3 stride-2 max pools (padding 1 or 0) and the
  * bilinear resize of the wrappers (align_corners=False).
  *
  * libdva_resnet.so links against libdva_b200.so (rpath $ORIGIN): it reports its errors through dva_last_error() and
@@ -10,8 +11,8 @@
  * Conventions: fp32 channels-last rows [B * H * W, C]; products in 3xTF32 on tensor cores (the main loop of
  * libdva_conv2d.so); no atomics: every result is bitwise reproducible run to run; the stream last; DVA_E* return
  * codes.  A convolution is (T, stride, dilation) with zero padding = dilation * (T - 1) / 2 and no bias; the shapes
- * are those of the trunk: 3x3 stride 1 with dilation 1, 2 or 4, 3x3 stride 2 with dilation 1, and 1x1 with stride 1
- * or 2.  Its output is H' = (H - 1) / stride + 1 (ceil(H / stride)).
+ * are those of the trunks: 3x3 stride 1 with dilation 1, 2 or 4, 3x3 stride 2 with dilation 1, 1x1 with stride 1
+ * or 2, and the ImageNet stem's 7x7 stride 2 (padding 3).  Its output is H' = (H - 1) / stride + 1 (ceil(H / stride)).
  */
 #ifndef DVA_RESNET_H_
 #define DVA_RESNET_H_
@@ -63,9 +64,16 @@ int dva_resnet_bn_bwd(const float* dy, const float* y, const float* z, int64_t M
                       const float* invstd, const float* gamma, int training, float* dz, float* gout, float* dgamma,
                       float* dbeta, void* ws, size_t ws_bytes, void* stream);
 
-/* MaxPool2d(3, stride 2, padding 1): y [B*H'*W', C], H' = (H - 1) / 2 + 1, and the window position (r * 3 + s) of
- * the max: the first in row-major order, padding never, a NaN as torch takes it.  The backward sums, for each input
- * pixel, the at most 4 windows that chose it. */
+/* MaxPool2d(3, stride 2, padding pad), pad 0 or 1: y [B*H'*W', C], H' = (H + 2 pad - 3) / 2 + 1, and the window
+ * position (r * 3 + s) of the max: the first valid tap starts as the max and a later one replaces it when greater or
+ * NaN (torch's rule), so padding never wins.  H + 2 pad < 3 (no window) is DVA_EINVAL.  The backward sums, for each
+ * input pixel, the at most 4 windows that chose it; a pixel no window covers (the last row or column at pad 0) gets
+ * 0. */
+int dva_resnet_maxpool_pad(const float* x, int64_t B, int64_t H, int64_t W, int C, int pad, float* y, uint8_t* arg,
+                           void* stream);
+int dva_resnet_maxpool_pad_bwd(const float* dy, const uint8_t* arg, int64_t B, int64_t H, int64_t W, int C, int pad,
+                               float* dx, void* stream);
+/* The same with padding 1, H' = (H - 1) / 2 + 1. */
 int dva_resnet_maxpool(const float* x, int64_t B, int64_t H, int64_t W, int C, float* y, uint8_t* arg, void* stream);
 int dva_resnet_maxpool_bwd(const float* dy, const uint8_t* arg, int64_t B, int64_t H, int64_t W, int C, float* dx,
                            void* stream);
