@@ -188,6 +188,11 @@ RESNET_SIGNATURES = {
     "dva_resnet_bn_apply": (_i32, [_vp, _i64, _i32] + [_vp] * 11 + [_vp]),
     "dva_resnet_bn_bwd_workspace_bytes": (_sz, [_i64, _i32]),
     "dva_resnet_bn_bwd": (_i32, [_vp, _vp, _vp, _i64, _i32, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "dva_resnet_conv_bn_fwd_sums": (_i32, [_vp, _i64, _i64, _i64, _i32, _vp, _i32, _i32, _i32, _i32, _vp, _vp, _vp,
+                                           _sz, _vp]),
+    "dva_resnet_bn_sync_stats": (_i32, [_vp, _i32, _i64, _f32, _f32, _vp, _vp, _vp, _vp, _vp]),
+    "dva_resnet_bn_bwd_sums": (_i32, [_vp, _vp, _vp, _i64, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "dva_resnet_bn_sync_bwd": (_i32, [_vp, _vp, _vp, _i64, _i32, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _sz, _vp]),
     "dva_resnet_maxpool": (_i32, [_vp, _i64, _i64, _i64, _i32, _vp, _vp, _vp]),
     "dva_resnet_maxpool_bwd": (_i32, [_vp, _vp, _i64, _i64, _i64, _i32, _vp, _vp]),
     "dva_resnet_maxpool_pad": (_i32, [_vp, _i64, _i64, _i64, _i32, _i32, _vp, _vp, _vp]),

@@ -35,10 +35,18 @@ class FastBatchNorm1d(nn.Module):
 class MLPLayer(nn.Sequential):
     """One `Linear -> FastBatchNorm1d -> activation` layer.  An nn.Sequential (children '0', '1',
     '2': reference parameter names), whose forward fuses BatchNorm + LeakyReLU into two streaming
-    passes (ops.batch_norm_act) when the input is a CUDA [rows, C] matrix."""
+    passes (ops.batch_norm_act) when the input is a CUDA [rows, C] matrix.  When
+    nn.SyncBatchNorm.convert_sync_batchnorm has replaced the inner BatchNorm1d, the projection
+    still runs on ops.linear and the nn.SyncBatchNorm module itself normalises, synchronised over
+    its process group as torch does it, before the activation."""
 
     def forward(self, x):
         lin, bn, act = self[0], self[1], self[2]
+        if (isinstance(bn, FastBatchNorm1d) and isinstance(bn.batch_norm, nn.SyncBatchNorm)
+                and x.dim() == 2 and x.is_cuda and x.shape[0] > 0):
+            from .. import ops
+            z = ops.linear(x, lin.weight)
+            return act(bn(z if lin.bias is None else z + lin.bias))
         fusable = (x.dim() == 2 and x.is_cuda and isinstance(bn, FastBatchNorm1d)
                    and isinstance(act, (nn.LeakyReLU, nn.ReLU, nn.Identity, Identity)) and x.shape[0] > 0)
         if not fusable:

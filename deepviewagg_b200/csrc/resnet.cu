@@ -10,12 +10,15 @@
 //          kDgrad  taps of dz reaching input pixel ih: (ih + pad - r * dil) / stride where it divides
 //        The forward epilogue takes per-(tile, channel) fp64 sums of z and z^2 (training only).
 //   rn_bn_stats_kernel  one CTA per channel: the tile partials in a fixed order -> mean, invstd, and the running
-//        stats updated as F.batch_norm does; in eval mode mean / invstd from the running stats.
+//        stats updated as F.batch_norm does; in eval mode mean / invstd from the running stats.  For a BatchNorm
+//        synchronised over ranks (nn.SyncBatchNorm) the same kernel runs twice: once to this rank's per-channel sums,
+//        and once over the all-reduced sums as a single tile with the global count.
 //   rn_conv_wgrad_kernel + rn_wgrad_reduce_kernel  dW = dz^T . im2col(x) split over the output pixels, one fp32
 //        partial per split, summed in fp64 in split order into the torch layout.
 //   rn_bn_apply_kernel  y = relu(BN(z) [+ skip] [+ BN_s(zs)]) in one pass.
 //   rn_bn_bwd_partial_kernel -> rn_bn_bwd_reduce_kernel -> rn_bn_bwd_dz_kernel  per-channel sums of g and g * zhat
-//        over pixel chunks (g = dy masked by the saved output), reduced in chunk order; dgamma, dbeta, dz.
+//        over pixel chunks (g = dy masked by the saved output), reduced in chunk order; dgamma, dbeta, dz.  Synchronised:
+//        the reduce writes this rank's sums, then runs again over the all-reduced sums as a single chunk.
 //   rn_maxpool_kernel / rn_maxpool_bwd_kernel  3x3 / 2 with padding 1 or 0 and the window position of the max; the
 //        backward is a gather over the <= 4 windows covering a pixel (none for the last row / column that padding 0
 //        can leave out).
@@ -34,6 +37,8 @@ using namespace dva;
 using namespace dva_convgemm;
 
 enum { kFwd = 0, kDgrad = 1 };
+// BatchNorm statistics modes of rn_bn_stats_kernel and rn_bn_bwd_reduce_kernel
+enum { kEval = 0, kTrain = 1, kSums = 2 };
 
 struct ConvArgs {
   const float* src;   // the gathered operand: x (forward) or dz (data gradient)
@@ -120,14 +125,15 @@ __global__ void __launch_bounds__(kThreads) rn_conv_gemm_kernel(ConvArgs a) {
   }
 }
 
-// one CTA per channel: the tile partials in a fixed order (training) or the running stats (eval)
+// one CTA per channel: the tile partials in a fixed order -> mean, invstd and the running stats (kTrain), or their
+// sums to sums[c] and the count n after the C channels (kSums); kEval: mean / invstd from the running stats
 __global__ void __launch_bounds__(kRedThreads)
-rn_bn_stats_kernel(const double2* __restrict__ part, int tiles, int64_t n, int training, float momentum, float eps,
+rn_bn_stats_kernel(const double2* __restrict__ part, int tiles, int64_t n, int mode, float momentum, float eps,
                    float* __restrict__ running_mean, float* __restrict__ running_var, float* __restrict__ mean,
-                   float* __restrict__ invstd) {
+                   float* __restrict__ invstd, double2* __restrict__ sums) {
   __shared__ double sh[kRedThreads];
   const int c = blockIdx.x;
-  if (!training) {
+  if (mode == kEval) {
     if (threadIdx.x == 0) {
       mean[c] = running_mean[c];
       invstd[c] = (float)(1.0 / sqrt((double)running_var[c] + (double)eps));
@@ -139,6 +145,15 @@ rn_bn_stats_kernel(const double2* __restrict__ part, int tiles, int64_t n, int t
     const double2 d = part[(int64_t)c * tiles + t];
     s += d.x;
     q += d.y;
+  }
+  if (mode == kSums) {
+    s = block_sum(s, sh);
+    q = block_sum(q, sh);
+    if (threadIdx.x == 0) {
+      sums[c] = make_double2(s, q);
+      if (c == 0) reinterpret_cast<double*>(sums + gridDim.x)[0] = (double)n;
+    }
+    return;
   }
   const double nn = (double)n;
   const double2 st = finish_stats(s, q, nn, eps, mean[c], invstd[c], sh);
@@ -250,9 +265,10 @@ rn_bn_bwd_partial_kernel(const float* __restrict__ dy, const float* __restrict__
   if (fold_rows(sh, tx, ty, c < C, s1, s2)) part[chunk * C + c] = make_double2(s1, s2);
 }
 
-// per channel: the chunk partials in chunk order -> dbeta, dgamma and the means of g and g * zhat (training)
+// per channel: the chunk partials in chunk order -> dbeta, dgamma (when not NULL) and coef: the means of g and
+// g * zhat over M (kTrain), 0 (kEval), or the sums themselves followed by the count M after the C channels (kSums)
 __global__ void __launch_bounds__(32 * kRows)
-rn_bn_bwd_reduce_kernel(const double2* __restrict__ part, int64_t chunks, int C, int64_t M, int training,
+rn_bn_bwd_reduce_kernel(const double2* __restrict__ part, int64_t chunks, int C, int64_t M, int mode,
                         float* __restrict__ dgamma, float* __restrict__ dbeta, double2* __restrict__ coef) {
   __shared__ double2 sh[kRows][32];
   const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
@@ -265,9 +281,16 @@ rn_bn_bwd_reduce_kernel(const double2* __restrict__ part, int64_t chunks, int C,
       s2 += d.y;
     }
   if (fold_rows(sh, tx, ty, c < C, s1, s2)) {
-    dbeta[c] = (float)s1;
-    dgamma[c] = (float)s2;
-    coef[c] = training ? make_double2(s1 / (double)M, s2 / (double)M) : make_double2(0.0, 0.0);
+    if (dbeta) {
+      dbeta[c] = (float)s1;
+      dgamma[c] = (float)s2;
+    }
+    if (mode == kSums) {
+      coef[c] = make_double2(s1, s2);
+      if (c == 0) reinterpret_cast<double*>(coef + C)[0] = (double)M;
+    } else {
+      coef[c] = mode == kTrain ? make_double2(s1 / (double)M, s2 / (double)M) : make_double2(0.0, 0.0);
+    }
   }
 }
 
@@ -511,9 +534,44 @@ extern "C" int dva_resnet_conv_bn_fwd(const float* x, int64_t B, int64_t H, int6
   rn_conv_gemm_kernel<kFwd><<<dim3((unsigned)a.tiles, (unsigned)cdiv(Co, BN)), kThreads, 0, st>>>(a);
   const int r2 = check_launch("resnet_conv_bn_fwd");
   if (r2 != DVA_OK) return r2;
-  rn_bn_stats_kernel<<<Co, kRedThreads, 0, st>>>(a.part, a.tiles, M, training, momentum, eps, running_mean,
-                                                 running_var, mean, invstd);
+  rn_bn_stats_kernel<<<Co, kRedThreads, 0, st>>>(a.part, a.tiles, M, training ? kTrain : kEval, momentum, eps,
+                                                 running_mean, running_var, mean, invstd, nullptr);
   return check_launch("resnet_conv_bn_fwd_stats");
+}
+
+extern "C" int dva_resnet_conv_bn_fwd_sums(const float* x, int64_t B, int64_t H, int64_t W, int Ci, const float* wf,
+                                           int Co, int T, int stride, int dil, float* z, double* sums, void* ws,
+                                           size_t ws_bytes, void* stream) {
+  const int rc = check_conv("resnet_conv_bn_fwd_sums", B, H, W, Ci, Co, T, stride, dil);
+  if (rc != DVA_OK) return rc;
+  if (!x || !wf || !z || !sums || !ws) return fail(DVA_EINVAL, "resnet_conv_bn_fwd_sums: null pointer");
+  const int64_t Ho = out_size(H, stride), Wo = out_size(W, stride), M = B * Ho * Wo;
+  if (ws_bytes < dva_resnet_fwd_workspace_bytes(B, Ho, Wo, Co))
+    return fail(DVA_EINVAL, "resnet_conv_bn_fwd_sums: workspace too small");
+  ConvArgs a{};
+  a.src = x; a.wt = wf; a.out = z; a.part = (double2*)ws;
+  a.M = M; a.H = (int)H; a.W = (int)W; a.Ho = (int)Ho; a.Wo = (int)Wo;
+  a.Cs = Ci; a.N = Co; a.K = T * T * Ci; a.T = T; a.stride = stride; a.dil = dil; a.pad = pad_of(T, dil);
+  a.tiles = (int)cdiv(M, BM);
+  cudaStream_t st = (cudaStream_t)stream;
+  rn_conv_gemm_kernel<kFwd><<<dim3((unsigned)a.tiles, (unsigned)cdiv(Co, BN)), kThreads, 0, st>>>(a);
+  const int r2 = check_launch("resnet_conv_bn_fwd_sums");
+  if (r2 != DVA_OK) return r2;
+  rn_bn_stats_kernel<<<Co, kRedThreads, 0, st>>>(a.part, a.tiles, M, kSums, 0.f, 0.f, nullptr, nullptr, nullptr,
+                                                 nullptr, (double2*)sums);
+  return check_launch("resnet_conv_bn_fwd_sums_stats");
+}
+
+extern "C" int dva_resnet_bn_sync_stats(const double* sums, int C, int64_t n, float momentum, float eps,
+                                        float* running_mean, float* running_var, float* mean, float* invstd,
+                                        void* stream) {
+  if (C < 1) return fail(DVA_EINVAL, "resnet_bn_sync_stats: bad sizes");
+  if (n < 2) return fail(DVA_EINVAL, "resnet_bn_sync_stats: training needs more than 1 value per channel");
+  if (!sums || !running_mean || !running_var || !mean || !invstd)
+    return fail(DVA_EINVAL, "resnet_bn_sync_stats: null pointer");
+  rn_bn_stats_kernel<<<C, kRedThreads, 0, (cudaStream_t)stream>>>((const double2*)sums, 1, n, kTrain, momentum, eps,
+                                                                  running_mean, running_var, mean, invstd, nullptr);
+  return check_launch("resnet_bn_sync_stats");
 }
 
 extern "C" int dva_resnet_conv_dgrad(const float* dz, int64_t B, int64_t H, int64_t W, int Ci, int Co,
@@ -595,13 +653,54 @@ extern "C" int dva_resnet_bn_bwd(const float* dy, const float* y, const float* z
                                                                                    pl.rows_per_chunk, part);
   int rc = check_launch("resnet_bn_bwd_partial");
   if (rc != DVA_OK) return rc;
-  rn_bn_bwd_reduce_kernel<<<cb, 32 * kRows, 0, st>>>(part, pl.chunks, C, M, training, dgamma, dbeta, coef);
+  rn_bn_bwd_reduce_kernel<<<cb, 32 * kRows, 0, st>>>(part, pl.chunks, C, M, training ? kTrain : kEval, dgamma,
+                                                     dbeta, coef);
   rc = check_launch("resnet_bn_bwd_reduce");
   if (rc != DVA_OK) return rc;
   const int64_t n = M * C;
   rn_bn_bwd_dz_kernel<<<elementwise_grid(n), kRedThreads, 0, st>>>(dy, y, z, C, mean, invstd, gamma, coef, dz, gout,
                                                                    n);
   return check_launch("resnet_bn_bwd_dz");
+}
+
+extern "C" int dva_resnet_bn_bwd_sums(const float* dy, const float* y, const float* z, int64_t M, int C,
+                                      const float* mean, const float* invstd, float* dgamma, float* dbeta,
+                                      double* sums, void* ws, size_t ws_bytes, void* stream) {
+  if (M < 1 || C < 1) return fail(DVA_EINVAL, "resnet_bn_bwd_sums: bad sizes");
+  if (!dy || !y || !z || !mean || !invstd || !dgamma || !dbeta || !sums || !ws)
+    return fail(DVA_EINVAL, "resnet_bn_bwd_sums: null pointer");
+  if (ws_bytes < dva_resnet_bn_bwd_workspace_bytes(M, C))
+    return fail(DVA_EINVAL, "resnet_bn_bwd_sums: workspace too small");
+  const BnPlan pl = bn_plan(M, C);
+  double2* part = (double2*)ws;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int cb = (int)cdiv(C, 32);
+  rn_bn_bwd_partial_kernel<<<dim3((unsigned)pl.chunks, cb), 32 * kRows, 0, st>>>(dy, y, z, M, C, mean, invstd,
+                                                                                   pl.rows_per_chunk, part);
+  const int rc = check_launch("resnet_bn_bwd_sums_partial");
+  if (rc != DVA_OK) return rc;
+  rn_bn_bwd_reduce_kernel<<<cb, 32 * kRows, 0, st>>>(part, pl.chunks, C, M, kSums, dgamma, dbeta, (double2*)sums);
+  return check_launch("resnet_bn_bwd_sums_reduce");
+}
+
+extern "C" int dva_resnet_bn_sync_bwd(const float* dy, const float* y, const float* z, int64_t M, int C,
+                                      const float* mean, const float* invstd, const float* gamma, const double* sums,
+                                      int64_t n, float* dz, float* gout, void* ws, size_t ws_bytes, void* stream) {
+  if (M < 1 || C < 1) return fail(DVA_EINVAL, "resnet_bn_sync_bwd: bad sizes");
+  if (n < 2 || n < M) return fail(DVA_EINVAL, "resnet_bn_sync_bwd: bad global count");
+  if (!dy || !y || !z || !mean || !invstd || !gamma || !sums || !dz || !ws)
+    return fail(DVA_EINVAL, "resnet_bn_sync_bwd: null pointer");
+  if (ws_bytes < (size_t)C * sizeof(double2)) return fail(DVA_EINVAL, "resnet_bn_sync_bwd: workspace too small");
+  double2* coef = (double2*)ws;
+  cudaStream_t st = (cudaStream_t)stream;
+  rn_bn_bwd_reduce_kernel<<<(int)cdiv(C, 32), 32 * kRows, 0, st>>>((const double2*)sums, 1, C, n, kTrain, nullptr,
+                                                                   nullptr, coef);
+  const int rc = check_launch("resnet_bn_sync_bwd_reduce");
+  if (rc != DVA_OK) return rc;
+  const int64_t e = M * C;
+  rn_bn_bwd_dz_kernel<<<elementwise_grid(e), kRedThreads, 0, st>>>(dy, y, z, C, mean, invstd, gamma, coef, dz, gout,
+                                                                   e);
+  return check_launch("resnet_bn_sync_bwd_dz");
 }
 
 static int check_maxpool(const char* what, int64_t B, int64_t H, int64_t W, int C, int pad) {

@@ -696,7 +696,8 @@ def _mit_semseg_keys():
 def load_mit_semseg_encoder(module, state_dict):
     """Load mit_semseg's resnet18dilated encoder state dict (encoder_epoch_20.pth: conv1, bn1, ..., layer4.1.bn2.*)
     into the layers an ADE20KResNet18* module holds (its conv.<i>.*).  The state dict must have exactly the
-    checkpoint's keys; a missing or extra key raises KeyError."""
+    checkpoint's keys; a missing or extra key raises KeyError.
+    Load before nn.SyncBatchNorm.convert_sync_batchnorm: the loader expects the unconverted BatchNorm classes."""
     mapping = _mit_semseg_keys()
     missing = sorted(set(mapping) - set(state_dict))
     extra = sorted(set(state_dict) - set(mapping))
@@ -710,10 +711,19 @@ def load_mit_semseg_encoder(module, state_dict):
 
 
 def _check_bn_values(bn, training, B, H, W):
-    """torch's error for a training BatchNorm that would see one value per channel, raised before any launch."""
+    """torch's error for a training BatchNorm that would see one value per channel, raised before any launch.  A
+    BatchNorm synchronised over ranks (ops.bn_sync_group) counts the values of every rank: ops raises it after its
+    all-reduce, on every rank at once."""
+    if ops.bn_sync_group(bn) is not None:
+        return
     if training and B * H * W <= 1:
         raise ValueError(f"Expected more than 1 value per channel when training, got input size "
                          f"{[B, bn.num_features, H, W]}")
+
+
+# The BatchNorms a trunk or a pyramid head holds: SynchronizedBatchNorm2d, PrudentSynchronizedBatchNorm2d and
+# FusedBatchNorm2d, or the nn.SyncBatchNorm that nn.SyncBatchNorm.convert_sync_batchnorm makes of any of them.
+_BATCHNORMS = (nn.BatchNorm2d, nn.SyncBatchNorm)
 
 
 # A trunk as _run_trunk walks it: a list of layers, each the stem -- a list of (conv, BatchNorm) units, then the
@@ -731,7 +741,7 @@ def _stem_of(layer):
     _run_trunk walks it."""
     mods = [m for m in layer.modules() if not isinstance(m, nn.Sequential)]
     convs = [m for m in mods if isinstance(m, nn.Conv2d)]
-    bns = [m for m in mods if isinstance(m, nn.BatchNorm2d)]
+    bns = [m for m in mods if isinstance(m, _BATCHNORMS)]
     return _Stem(list(zip(convs, bns)), mods[-1].padding)
 
 
@@ -1008,7 +1018,8 @@ def load_torchvision_resnet18(module, state_dict):
     """Load torchvision's ImageNet resnet18 state dict (conv1, bn1, layer1..layer4, fc) into the layers a ResNet18*
     module holds; fc is dropped.  The state dict must have exactly torchvision's keys, except that
     num_batches_tracked may be missing, as in checkpoints saved before torch 0.4.1: those counters are left as they
-    are, as torch's BatchNorm loads such a checkpoint.  A missing or extra key raises KeyError."""
+    are, as torch's BatchNorm loads such a checkpoint.  A missing or extra key raises KeyError.
+    Load before nn.SyncBatchNorm.convert_sync_batchnorm: the loader expects the unconverted BatchNorm classes."""
     mapping = _torchvision_resnet18_keys()
     counters = [k for k in mapping if k.endswith('.num_batches_tracked')]
     _check_keys("torchvision resnet18", [k for k in mapping if k not in counters], state_dict, counters)
@@ -1027,7 +1038,8 @@ def _cityscapes_resnet18_keys():
 def load_cityscapes_resnet18(module, state_dict):
     """Load SFSegNets' Cityscapes ResNet-18 state dict (resnet18_SFSegNets.pth: layer0.0.0.weight, ...,
     layer4.1.bn2.*, 138 keys) into CityscapesResNet18 or the layers a CityscapesResNet18* module holds.  The state
-    dict must have exactly those keys; a missing or extra key raises KeyError."""
+    dict must have exactly those keys; a missing or extra key raises KeyError.
+    Load before nn.SyncBatchNorm.convert_sync_batchnorm: the loader expects the unconverted BatchNorm classes."""
     mapping = _cityscapes_resnet18_keys()
     _check_keys("Cityscapes ResNet-18 (resnet18_SFSegNets.pth)", mapping, state_dict)
     return _load_layers(module, {target: state_dict[key] for key, target in mapping.items()})
@@ -1285,7 +1297,8 @@ def load_mit_semseg_decoder(module, state_dict):
     """Load mit_semseg's PPMDeepsup decoder state dict (decoder_epoch_20.pth: ppm.*, cbr_deepsup.*, conv_last.*,
     conv_last_deepsup.*) into a PPMFeatMap, or into the decoder of an ADE20KResNet18PPM, keeping what
     PPMFeatMap.from_pretrained keeps: ppm and conv_last[:3].  The state dict must have exactly the checkpoint's keys;
-    a missing or extra key raises KeyError."""
+    a missing or extra key raises KeyError.
+    Load before nn.SyncBatchNorm.convert_sync_batchnorm: the loader expects the unconverted BatchNorm classes."""
     decoder = getattr(module, 'decoder', module)
     mapping = _mit_semseg_decoder_keys()
     missing = sorted(set(mapping) - set(state_dict))

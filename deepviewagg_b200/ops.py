@@ -1821,8 +1821,9 @@ def _rn_running(t):
     return t if t.dtype == torch.float32 and t.is_contiguous() else t.detach().float().contiguous()
 
 
-def _rn_conv_bn(x, wf, Co, geo, bn):
-    """z = conv(x) and the BatchNorm statistics of z; bn = (running_mean, running_var, training, momentum, eps)."""
+def _rn_conv_bn(x, wf, Co, geo, bn, sync=None):
+    """z = conv(x) and the BatchNorm statistics of z; bn = (running_mean, running_var, training, momentum, eps); sync
+    a _BNSync when the statistics are taken over the ranks of a process group."""
     T, stride, dil = geo
     rm, rv, training, momentum, eps = bn
     B, H, W, Ci = x.shape
@@ -1830,10 +1831,21 @@ def _rn_conv_bn(x, wf, Co, geo, bn):
     z = torch.empty(B, Ho, Wo, Co, dtype=torch.float32, device=x.device)
     mean = torch.empty(Co, dtype=torch.float32, device=x.device)
     invstd = torch.empty_like(mean)
-    ws = _lib.workspace(_lib.load_resnet().dva_resnet_fwd_workspace_bytes(B, Ho, Wo, Co) if training else 0, x.device)
     rm32, rv32 = _rn_running(rm), _rn_running(rv)
-    launch("dva_resnet_conv_bn_fwd", x.device, x, B, H, W, Ci, wf, Co, T, stride, dil, int(training), float(momentum),
-           float(eps), rm32, rv32, z, mean, invstd, ws, ws.numel())
+    if sync is not None:
+        sums = torch.zeros(2 * Co + 1, dtype=torch.float64, device=x.device)
+        if B > 0:
+            ws = _lib.workspace(_lib.load_resnet().dva_resnet_fwd_workspace_bytes(B, Ho, Wo, Co), x.device)
+            launch("dva_resnet_conv_bn_fwd_sums", x.device, x, B, H, W, Ci, wf, Co, T, stride, dil, z, sums, ws,
+                   ws.numel())
+        sync.count = sync.all_reduce(sums)
+        launch("dva_resnet_bn_sync_stats", x.device, sums, Co, sync.count, float(momentum), float(eps), rm32, rv32,
+               mean, invstd)
+    else:
+        ws = _lib.workspace(_lib.load_resnet().dva_resnet_fwd_workspace_bytes(B, Ho, Wo, Co) if training else 0,
+                            x.device)
+        launch("dva_resnet_conv_bn_fwd", x.device, x, B, H, W, Ci, wf, Co, T, stride, dil, int(training),
+               float(momentum), float(eps), rm32, rv32, z, mean, invstd, ws, ws.numel())
     if training:
         for buf, b32 in ((rm, rm32), (rv, rv32)):
             if b32 is not buf:
@@ -1846,18 +1858,36 @@ def _rn_apply(z, mean, invstd, gamma, beta, skip=None, ds=None):
     B, H, W, C = z.shape
     zs, ms, iss, gs, bs = ds if ds is not None else (None,) * 5
     y = torch.empty_like(z)
+    if B == 0:      # a rank without images in a synchronised BatchNorm
+        return y
     launch("dva_resnet_bn_apply", z.device, z, B * H * W, C, mean, invstd, gamma, beta, skip, zs, ms, iss, gs, bs, y)
     return y
 
 
-def _rn_bn_bwd(dy, y, z, mean, invstd, gamma, training, want_g=False):
-    """(dz, g, dgamma, dbeta) of y = relu(BN(z) + r); g, the gradient reaching r, only when want_g."""
+def _rn_bn_bwd(dy, y, z, mean, invstd, gamma, training, want_g=False, sync=None):
+    """(dz, g, dgamma, dbeta) of y = relu(BN(z) + r); g, the gradient reaching r, only when want_g.  sync: the
+    forward's _BNSync (the sums of g and g * zhat all-reduced over its group; dgamma and dbeta stay this rank's)."""
     B, H, W, C = z.shape
     M = B * H * W
     dz = torch.empty_like(z)
     g = torch.empty_like(z) if want_g else None
     dgamma = torch.empty(C, dtype=torch.float32, device=z.device)
     dbeta = torch.empty_like(dgamma)
+    if sync is not None:
+        sums = torch.zeros(2 * C + 1, dtype=torch.float64, device=z.device)
+        if M > 0:
+            ws = _lib.workspace(_lib.load_resnet().dva_resnet_bn_bwd_workspace_bytes(M, C), z.device)
+            launch("dva_resnet_bn_bwd_sums", z.device, dy, y, z, M, C, mean, invstd, dgamma, dbeta, sums, ws,
+                   ws.numel())
+        else:
+            dgamma.zero_()
+            dbeta.zero_()
+        sync.all_reduce(sums)
+        if M > 0:
+            ws = _lib.workspace(C * 16, z.device)
+            launch("dva_resnet_bn_sync_bwd", z.device, dy, y, z, M, C, mean, invstd, gamma, sums, sync.count, dz, g,
+                   ws, ws.numel())
+        return dz, g, dgamma, dbeta
     ws = _lib.workspace(_lib.load_resnet().dva_resnet_bn_bwd_workspace_bytes(M, C), z.device)
     launch("dva_resnet_bn_bwd", z.device, dy, y, z, M, C, mean, invstd, gamma, int(training), dz, g, dgamma, dbeta,
            ws, ws.numel())
@@ -1867,6 +1897,8 @@ def _rn_bn_bwd(dy, y, z, mean, invstd, gamma, training, want_g=False):
 def _rn_wgrad(dz, x, Co, geo):
     T, stride, dil = geo
     B, H, W, Ci = x.shape
+    if B == 0:
+        return torch.zeros(Co, Ci, T, T, dtype=torch.float32, device=x.device)
     dw = torch.empty(Co, Ci, T, T, dtype=torch.float32, device=x.device)
     ws = _lib.workspace(_lib.load_resnet().dva_resnet_wgrad_workspace_bytes(B, H, W, Ci, Co, T, stride, dil), x.device)
     launch("dva_resnet_conv_wgrad", x.device, dz, x, B, H, W, Ci, Co, T, stride, dil, dw, ws, ws.numel())
@@ -1878,18 +1910,79 @@ def _rn_dgrad(dz, x_shape, wd, geo, add=None, out=None):
     T, stride, dil = geo
     B, H, W, Ci = x_shape
     dx = out if out is not None else torch.empty(B, H, W, Ci, dtype=torch.float32, device=dz.device)
+    if B == 0:
+        return dx
     launch("dva_resnet_conv_dgrad", dz.device, dz, B, H, W, Ci, dz.shape[-1], wd, T, stride, dil, add, dx)
     return dx
 
 
+class _BNSync:
+    """The process group of a training nn.SyncBatchNorm for one forward, and the global count (values per channel
+    over the group's ranks) its forward found; the backward reuses the count."""
+
+    def __init__(self, group):
+        self.group = group
+        self.count = None
+
+    def all_reduce(self, sums):
+        """Sums the packed fp64 [2 C + 1] (per-channel sums, then the count) over the group, in place on the current
+        stream; returns the global count.  In the forward a count of at most 1 raises ValueError on every rank, as
+        each rank decides it from the same all-reduced value."""
+        torch.distributed.all_reduce(sums, group=self.group)
+        n = int(sums[-1].item()) if self.count is None else self.count
+        if n <= 1:
+            raise ValueError(f"Expected more than 1 value per channel when training, got {n} over the "
+                             f"{torch.distributed.get_world_size(self.group)} ranks of the process group")
+        return n
+
+
+_SYNC_BN = {"split_at_one_rank": False}
+
+
+@contextlib.contextmanager
+def sync_batchnorm_split_at_one_rank():
+    """Inside this context a training nn.SyncBatchNorm takes the split (all-reduce) path also in a process group of
+    one rank, where it otherwise takes the fused one; both give the same bits.  For tests and measurements."""
+    prev = _SYNC_BN["split_at_one_rank"]
+    _SYNC_BN["split_at_one_rank"] = True
+    try:
+        yield
+    finally:
+        _SYNC_BN["split_at_one_rank"] = prev
+
+
+def bn_sync_group(bn):
+    """The process group whose union batch a BatchNorm normalises over: for a training nn.SyncBatchNorm when
+    torch.distributed is initialised and its group (bn.process_group, default the world) has more than one rank;
+    None otherwise (eval mode, no process group, one rank, or any other BatchNorm), as torch's SyncBatchNorm
+    decides it."""
+    if not (isinstance(bn, torch.nn.SyncBatchNorm) and bn.training):
+        return None
+    dist = torch.distributed
+    if not (dist.is_available() and dist.is_initialized()):
+        return None
+    group = bn.process_group if bn.process_group else dist.group.WORLD
+    if dist.get_world_size(group) > 1 or _SYNC_BN["split_at_one_rank"]:
+        return group
+    return None
+
+
 def _bn_cfg(bn):
     """(training, momentum, eps) of bn for one forward.  A plain nn.BatchNorm2d (the ImageNet and Cityscapes trunks)
-    gets torch's bookkeeping here, in the module's forward, as _bn_step does it: num_batches_tracked += 1 in training
-    (so a reentrant checkpoint's recompute counts twice, as torch's module does) and momentum None as the cumulative
-    average.  mit_semseg's SynchronizedBatchNorm2d (steps_counter False) never moves its counter."""
+    and an nn.SyncBatchNorm get torch's bookkeeping here, in the module's forward, as _bn_step does it:
+    num_batches_tracked += 1 in training (so a reentrant checkpoint's recompute counts twice, as torch's module does)
+    and momentum None as the cumulative average.  mit_semseg's SynchronizedBatchNorm2d (steps_counter False) never
+    moves its counter."""
     if not getattr(bn, "steps_counter", True):
         return (bn.training, bn.momentum, bn.eps)
     return (bn.training, _bn_step(bn)[2], bn.eps)
+
+
+def _rn_bn_cfg(bn):
+    """(training, momentum, eps, sync) of bn for one forward: _bn_cfg, and a _BNSync when its statistics are
+    synchronised over a process group (bn_sync_group), else None."""
+    group = bn_sync_group(bn)
+    return (*_bn_cfg(bn), _BNSync(group) if group is not None else None)
 
 
 class _RNConvBNReLU(torch.autograd.Function):
@@ -1903,12 +1996,13 @@ class _RNConvBNReLU(torch.autograd.Function):
         ctx.dtypes = [t.dtype for t in (x, weight, gamma, beta)]
         x = _rows_input(x, weight.shape[1])
         w, g, b = _f32(weight, gamma, beta)
-        training, momentum, eps = bn_cfg
+        training, momentum, eps, sync = bn_cfg
         wf, wd = _rn_weights(w)
-        z, mean, invstd = _rn_conv_bn(x, wf, w.shape[0], geo, (running_mean, running_var, training, momentum, eps))
+        z, mean, invstd = _rn_conv_bn(x, wf, w.shape[0], geo, (running_mean, running_var, training, momentum, eps),
+                                      sync)
         y = _rn_apply(z, mean, invstd, g, b)
         ctx.save_for_backward(x, wd, g, z, mean, invstd, y)
-        ctx.cfg = (geo, training, w.shape[0])
+        ctx.cfg = (geo, training, sync, w.shape[0])
         return y
 
     @staticmethod
@@ -1916,8 +2010,8 @@ class _RNConvBNReLU(torch.autograd.Function):
     @torch.autograd.function.once_differentiable
     def backward(ctx, dy):
         x, wd, g, z, mean, invstd, y = ctx.saved_tensors
-        geo, training, Co = ctx.cfg
-        dz, _, dg, db = _rn_bn_bwd(dy.float().contiguous(), y, z, mean, invstd, g, training)
+        geo, training, sync, Co = ctx.cfg
+        dz, _, dg, db = _rn_bn_bwd(dy.float().contiguous(), y, z, mean, invstd, g, training, sync=sync)
         dw = _rn_wgrad(dz, x, Co, geo) if ctx.needs_input_grad[1] else None
         dx = _rn_dgrad(dz, x.shape, wd, geo) if ctx.needs_input_grad[0] else None
         return (*_as_dtypes((dx, dw, dg, db), ctx.dtypes), None, None, None, None)
@@ -1937,20 +2031,20 @@ class _RNBasicBlock(torch.autograd.Function):
         w1, g1, b1, w2, g2, b2, wd, gd, bd = _f32(w1, g1, b1, w2, g2, b2, wd, gd, bd)
         geo1, geo2, geod = (3, stride, dil1), (3, 1, dil2), (1, stride, 1)
         wf1, wd1 = _rn_weights(w1)
-        z1, m1, i1 = _rn_conv_bn(x, wf1, w1.shape[0], geo1, (rm1, rv1, *bn1))
+        z1, m1, i1 = _rn_conv_bn(x, wf1, w1.shape[0], geo1, (rm1, rv1, *bn1[:3]), bn1[3])
         h = _rn_apply(z1, m1, i1, g1, b1)
         wf2, wd2 = _rn_weights(w2)
-        z2, m2, i2 = _rn_conv_bn(h, wf2, w2.shape[0], geo2, (rm2, rv2, *bn2))
+        z2, m2, i2 = _rn_conv_bn(h, wf2, w2.shape[0], geo2, (rm2, rv2, *bn2[:3]), bn2[3])
         del h
         wdd = zd = md = idd = None
         if wd is not None:
             wfd, wdd = _rn_weights(wd)
-            zd, md, idd = _rn_conv_bn(x, wfd, wd.shape[0], geod, (rmd, rvd, *bnd))
+            zd, md, idd = _rn_conv_bn(x, wfd, wd.shape[0], geod, (rmd, rvd, *bnd[:3]), bnd[3])
             y = _rn_apply(z2, m2, i2, g2, b2, ds=(zd, md, idd, gd, bd))
         else:
             y = _rn_apply(z2, m2, i2, g2, b2, skip=x)
         ctx.save_for_backward(x, wd1, g1, b1, z1, m1, i1, wd2, g2, z2, m2, i2, wdd, gd, zd, md, idd, y)
-        ctx.cfg = (geo1, geo2, geod, bn1[0], bn2[0], bnd[0] if bnd is not None else False, w1.shape[0])
+        ctx.cfg = (geo1, geo2, geod, bn1, bn2, bnd if bnd is not None else (False, None, None, None), w1.shape[0])
         return y
 
     @staticmethod
@@ -1958,20 +2052,20 @@ class _RNBasicBlock(torch.autograd.Function):
     @torch.autograd.function.once_differentiable
     def backward(ctx, dy):
         x, wd1, g1, b1, z1, m1, i1, wd2, g2, z2, m2, i2, wdd, gd, zd, md, idd, y = ctx.saved_tensors
-        geo1, geo2, geod, t1, t2, td, Co = ctx.cfg
+        geo1, geo2, geod, bn1, bn2, bnd, Co = ctx.cfg
         need = ctx.needs_input_grad
         dy = dy.float().contiguous()
-        dz2, gr, dg2, db2 = _rn_bn_bwd(dy, y, z2, m2, i2, g2, t2, want_g=zd is None)
+        dz2, gr, dg2, db2 = _rn_bn_bwd(dy, y, z2, m2, i2, g2, bn2[0], want_g=zd is None, sync=bn2[3])
         h = _rn_apply(z1, m1, i1, g1, b1)
         dw2 = _rn_wgrad(dz2, h, Co, geo2) if need[4] else None
         dh = _rn_dgrad(dz2, h.shape, wd2, geo2)
-        dz1, _, dg1, db1 = _rn_bn_bwd(dh, h, z1, m1, i1, g1, t1)
+        dz1, _, dg1, db1 = _rn_bn_bwd(dh, h, z1, m1, i1, g1, bn1[0], sync=bn1[3])
         del h, dh
         dw1 = _rn_wgrad(dz1, x, Co, geo1) if need[1] else None
         grads_ds = (None,) * 3
         dx = None
         if zd is not None:
-            dzd, _, dgd, dbd = _rn_bn_bwd(dy, y, zd, md, idd, gd, td)
+            dzd, _, dgd, dbd = _rn_bn_bwd(dy, y, zd, md, idd, gd, bnd[0], sync=bnd[3])
             grads_ds = (_rn_wgrad(dzd, x, Co, geod) if need[7] else None, dgd, dbd)
             if need[0]:
                 dx = _rn_dgrad(dzd, x.shape, wdd, geod)
@@ -2003,7 +2097,8 @@ class _RNMaxPool(torch.autograd.Function):
         B, H, W, C = x.shape
         y = torch.empty(B, rn_pool_out(H, padding), rn_pool_out(W, padding), C, dtype=torch.float32, device=x.device)
         arg = torch.empty(y.shape, dtype=torch.uint8, device=x.device)
-        launch("dva_resnet_maxpool_pad", x.device, x, B, H, W, C, padding, y, arg)
+        if B > 0:
+            launch("dva_resnet_maxpool_pad", x.device, x, B, H, W, C, padding, y, arg)
         ctx.save_for_backward(arg)
         ctx.cfg = (B, H, W, C, padding)
         ctx.mark_non_differentiable(arg)
@@ -2016,7 +2111,8 @@ class _RNMaxPool(torch.autograd.Function):
         (arg,) = ctx.saved_tensors
         B, H, W, C, padding = ctx.cfg
         dx = torch.empty(B, H, W, C, dtype=torch.float32, device=dy.device)
-        launch("dva_resnet_maxpool_pad_bwd", dy.device, dy.float().contiguous(), arg, B, H, W, C, padding, dx)
+        if B > 0:
+            launch("dva_resnet_maxpool_pad_bwd", dy.device, dy.float().contiguous(), arg, B, H, W, C, padding, dx)
         return dx.to(ctx.dtype), None
 
 
@@ -2044,7 +2140,8 @@ class _RNResize(torch.autograd.Function):
         col = 0
         for x, (sh, sw) in zip(xs, scales):
             _, H, W, C = x.shape
-            launch("dva_resnet_resize", x.device, x, B, H, W, C, Ho, Wo, sh, sw, y, ld, col)
+            if B > 0:
+                launch("dva_resnet_resize", x.device, x, B, H, W, C, Ho, Wo, sh, sw, y, ld, col)
             col += C
         ctx.shapes = [tuple(x.shape) for x in xs]
         ctx.cfg = (size, scales, ld)
@@ -2060,7 +2157,8 @@ class _RNResize(torch.autograd.Function):
         for (B, H, W, C), (sh, sw), need in zip(ctx.shapes, scales, ctx.needs_input_grad[2:]):
             if need:
                 dx = torch.empty(B, H, W, C, dtype=torch.float32, device=dy.device)
-                launch("dva_resnet_resize_bwd", dy.device, dy, ld, col, B, H, W, C, Ho, Wo, sh, sw, dx)
+                if B > 0:
+                    launch("dva_resnet_resize_bwd", dy.device, dy, ld, col, B, H, W, C, Ho, Wo, sh, sw, dx)
                 grads.append(dx)
             else:
                 grads.append(None)
@@ -2072,15 +2170,16 @@ def rn_conv_bn_relu(x, conv, bn):
     """relu(bn(conv(x))) for channels-last x [B, H, W, C_in] (conv an nn.Conv2d without bias, bn a BatchNorm2d):
     fp32 [B, H', W', C_out]; in training mode bn's running stats are updated."""
     geo = (conv.kernel_size[0], conv.stride[0], conv.dilation[0])
-    return _RNConvBNReLU.apply(x, conv.weight, bn.weight, bn.bias, bn.running_mean, bn.running_var, geo, _bn_cfg(bn))
+    return _RNConvBNReLU.apply(x, conv.weight, bn.weight, bn.bias, bn.running_mean, bn.running_var, geo,
+                               _rn_bn_cfg(bn))
 
 
 def rn_basic_block(x, block):
     """A BasicBlock (conv1, bn1, conv2, bn2, downsample) on channels-last x [B, H, W, C_in]: fp32 [B, H', W', C_out]."""
     ds = block.downsample
     cd, nd = (ds[0], ds[1]) if ds is not None else (None, None)
-    cfg = ((block.conv1.stride[0], block.conv1.dilation[0], block.conv2.dilation[0]), _bn_cfg(block.bn1),
-           _bn_cfg(block.bn2), _bn_cfg(nd) if nd is not None else None)
+    cfg = ((block.conv1.stride[0], block.conv1.dilation[0], block.conv2.dilation[0]), _rn_bn_cfg(block.bn1),
+           _rn_bn_cfg(block.bn2), _rn_bn_cfg(nd) if nd is not None else None)
     return _RNBasicBlock.apply(x, block.conv1.weight, block.bn1.weight, block.bn1.bias, block.conv2.weight,
                                block.bn2.weight, block.bn2.bias, cd.weight if cd is not None else None,
                                nd.weight if nd is not None else None, nd.bias if nd is not None else None,
@@ -2142,7 +2241,10 @@ def _ppm_index(B, h, w, scales, device):
 
 def ppm_branch_training(bn, B, s):
     """Whether a pyramid branch's BatchNorm uses batch statistics: PrudentSynchronizedBatchNorm2d runs in eval mode
-    for a (1, C, 1, 1) input, so the scale-1 branch at batch size 1 never does."""
+    for a (1, C, 1, 1) input, so the scale-1 branch at batch size 1 never does; an nn.SyncBatchNorm converted from
+    it has no such rule."""
+    if isinstance(bn, torch.nn.SyncBatchNorm):
+        return bool(bn.training)
     return bool(bn.training) and not (B == 1 and s == 1)
 
 
@@ -2168,43 +2270,44 @@ class _RNPPMHead(torch.autograd.Function):
         img, pix, aptr, offsets = _ppm_index(B, h, w, scales, dev)
         Vw, P = img.numel(), pix.shape[0]
         pooled = torch.empty(Vw, C, dtype=torch.float32, device=dev)
-        launch("dva_gather_pool_fwd", dev, x, 1, img, pix, 0, aptr, pooled, None, B, C, h, w, Vw, P,
-               REDUCE_CODES["mean"], dtype_code(x))
+        if B > 0:       # B == 0: a rank without images in synchronised BatchNorms
+            launch("dva_gather_pool_fwd", dev, x, 1, img, pix, 0, aptr, pooled, None, B, C, h, w, Vw, P,
+                   REDUCE_CODES["mean"], dtype_code(x))
         ld = C + sum(wk.shape[0] for wk in ws_)
         cat = torch.empty(B, h, w, ld, dtype=torch.float32, device=dev)
         cat[..., :C].copy_(x)
         saved, col = [], C
         for k, s in enumerate(scales):
-            training, momentum, eps = branch_cfg[k]
             xs = pooled[offsets[k]:offsets[k] + B * s * s].view(B, s, s, C)
             wf, wd = _rn_weights(ws_[k])
             Co = ws_[k].shape[0]
-            z, mean, invstd = _rn_conv_bn(xs, wf, Co, (1, 1, 1), (running[2 * k], running[2 * k + 1], training,
-                                                                 momentum, eps))
+            z, mean, invstd = _rn_conv_bn(xs, wf, Co, (1, 1, 1), (running[2 * k], running[2 * k + 1],
+                                                                 *branch_cfg[k][:3]), branch_cfg[k][3])
             y = _rn_apply(z, mean, invstd, gs[k], bs[k])
             sh, sw = resize_scale(s, h), resize_scale(s, w)
-            launch("dva_resnet_resize", dev, y, B, s, s, Co, h, w, sh, sw, cat, ld, col)
+            if B > 0:
+                launch("dva_resnet_resize", dev, y, B, s, s, Co, h, w, sh, sw, cat, ld, col)
             saved += [wd, z, mean, invstd, y]
             col += Co
         wf, wd = _rn_weights(w_last)
-        training, momentum, eps = last_cfg
         z, mean, invstd = _rn_conv_bn(cat, wf, w_last.shape[0], (3, 1, 1), (running[2 * n], running[2 * n + 1],
-                                                                           training, momentum, eps))
+                                                                           *last_cfg[:3]), last_cfg[3])
         y = _rn_apply(z, mean, invstd, g_last, b_last)
         out = y
         if out_size is not None:
             out = torch.empty(B, *out_size, y.shape[3], dtype=torch.float32, device=dev)
+        if out_size is not None and B > 0:
             launch("dva_resnet_resize", dev, y, B, h, w, y.shape[3], out_size[0], out_size[1],
                    resize_scale(h, out_size[0]), resize_scale(w, out_size[1]), out, y.shape[3], 0)
         ctx.save_for_backward(pooled, cat, *gs, g_last, wd, z, mean, invstd, y, *saved)
-        ctx.cfg = (B, h, w, C, tuple(scales), offsets, [c[0] for c in branch_cfg], last_cfg[0], out_size)
+        ctx.cfg = (B, h, w, C, tuple(scales), offsets, branch_cfg, last_cfg, out_size)
         return out
 
     @staticmethod
     @_bwd
     @torch.autograd.function.once_differentiable
     def backward(ctx, dy):
-        B, h, w, C, scales, offsets, branch_training, last_training, out_size = ctx.cfg
+        B, h, w, C, scales, offsets, branch_cfg, last_cfg, out_size = ctx.cfg
         n = len(scales)
         pooled, cat, *rest = ctx.saved_tensors
         gs, g_last, rest = rest[:n], rest[n], rest[n + 1:]
@@ -2216,10 +2319,11 @@ class _RNPPMHead(torch.autograd.Function):
         Co = y.shape[3]
         if out_size is not None:
             dyh = torch.empty_like(y)
-            launch("dva_resnet_resize_bwd", dev, dy, Co, 0, B, h, w, Co, out_size[0], out_size[1],
-                   resize_scale(h, out_size[0]), resize_scale(w, out_size[1]), dyh)
+            if B > 0:
+                launch("dva_resnet_resize_bwd", dev, dy, Co, 0, B, h, w, Co, out_size[0], out_size[1],
+                       resize_scale(h, out_size[0]), resize_scale(w, out_size[1]), dyh)
             dy = dyh
-        dz, _, dg_last, db_last = _rn_bn_bwd(dy, y, z, mean, invstd, g_last, last_training)
+        dz, _, dg_last, db_last = _rn_bn_bwd(dy, y, z, mean, invstd, g_last, last_cfg[0], sync=last_cfg[3])
         dw_last = _rn_wgrad(dz, cat, Co, (3, 1, 1)) if need[3 * n] else None
         dcat = _rn_dgrad(dz, cat.shape, wd, (3, 1, 1))
         del dz
@@ -2230,9 +2334,10 @@ class _RNPPMHead(torch.autograd.Function):
             wdk, zk, mk, ik, yk = branches[k]
             Ck = yk.shape[3]
             dyk = torch.empty_like(yk)
-            launch("dva_resnet_resize_bwd", dev, dcat, ld, col, B, s, s, Ck, h, w, resize_scale(s, h),
-                   resize_scale(s, w), dyk)
-            dzk, _, dgk, dbk = _rn_bn_bwd(dyk, yk, zk, mk, ik, gs[k], branch_training[k])
+            if B > 0:
+                launch("dva_resnet_resize_bwd", dev, dcat, ld, col, B, s, s, Ck, h, w, resize_scale(s, h),
+                       resize_scale(s, w), dyk)
+            dzk, _, dgk, dbk = _rn_bn_bwd(dyk, yk, zk, mk, ik, gs[k], branch_cfg[k][0], sync=branch_cfg[k][3])
             xs = pooled[offsets[k]:offsets[k] + B * s * s].view(B, s, s, C)
             dwk = _rn_wgrad(dzk, xs, Ck, (1, 1, 1)) if need[3 * k] else None
             if dpooled is not None:
@@ -2241,7 +2346,9 @@ class _RNPPMHead(torch.autograd.Function):
             grads += [dwk, dgk, dbk]
             col += Ck
         dx = None
-        if dpooled is not None:
+        if dpooled is not None and B == 0:
+            dx = dcat[..., :C].clone()
+        elif dpooled is not None:
             img, pix, aptr, _ = _ppm_index(B, h, w, scales, dev)
             Vw, P = img.numel(), pix.shape[0]
             dx = torch.empty(B, h, w, C, dtype=torch.float32, device=dev)
@@ -2268,11 +2375,11 @@ def rn_ppm_head(x, decoder, out_size=None):
     for m, s in zip(decoder.ppm, scales):
         params += [m[1].weight, m[2].weight, m[2].bias]
         running += [m[2].running_mean, m[2].running_var]
-        branch_cfg.append((ppm_branch_training(m[2], B, s), m[2].momentum, m[2].eps))
+        branch_cfg.append((ppm_branch_training(m[2], B, s), *_rn_bn_cfg(m[2])[1:]))
     params += [conv.weight, bn.weight, bn.bias]
     running += [bn.running_mean, bn.running_var]
     size = None if out_size is None else (int(out_size[0]), int(out_size[1]))
-    return _RNPPMHead.apply(x, size, scales, branch_cfg, _bn_cfg(bn), *params, *running)
+    return _RNPPMHead.apply(x, size, scales, branch_cfg, _rn_bn_cfg(bn), *params, *running)
 
 
 def rn_resize(xs, size, scale_factor=None):

@@ -2,8 +2,8 @@
  * dva_resnet.h -- C ABI of libdva_resnet.so: the ResNet-18 image encoders on the H100 (sm_90a) -- the dilated one
  * pretrained on ADE20K (mit_semseg's resnet18dilated behind the reference's ADE20KResNet18* wrappers), torchvision's
  * ImageNet one (ResNet18*) and the Cityscapes one (CityscapesResNet18*): zero-padded convolutions with the BatchNorm
- * statistics in their epilogue, train- and eval-mode BatchNorm, the 3x3 stride-2 max pools (padding 1 or 0) and the
- * bilinear resize of the wrappers (align_corners=False).
+ * statistics in their epilogue, train- and eval-mode BatchNorm (also synchronised over ranks), the 3x3 stride-2 max
+ * pools (padding 1 or 0) and the bilinear resize of the wrappers (align_corners=False).
  *
  * libdva_resnet.so links against libdva_b200.so (rpath $ORIGIN): it reports its errors through dva_last_error() and
  * counts its launches in dva_launch_count() of that library.
@@ -39,6 +39,19 @@ int dva_resnet_conv_bn_fwd(const float* x, int64_t B, int64_t H, int64_t W, int 
                            float* running_var, float* z, float* mean, float* invstd, void* ws, size_t ws_bytes,
                            void* stream);
 
+/* Training-mode BatchNorm synchronised over ranks (nn.SyncBatchNorm), the forward in two calls around one
+ * all-reduce of `sums` (fp64 [2 * C + 1]: per channel (sum z, sum z^2), then the count):
+ *   dva_resnet_conv_bn_fwd_sums: z = conv(x, wf) as dva_resnet_conv_bn_fwd does it, and this rank's sums, reduced in
+ *     tile order as there, with the count B*H'*W' (one value per channel is allowed here);
+ *   dva_resnet_bn_sync_stats: from the all-reduced sums and the global count n (>= 2, else DVA_EINVAL), mean, invstd
+ *     and the running-stat update with `momentum` (running_var with the unbiased variance of n values).
+ * Over the sums of one rank with its own count, the results are those of dva_resnet_conv_bn_fwd bit for bit. */
+int dva_resnet_conv_bn_fwd_sums(const float* x, int64_t B, int64_t H, int64_t W, int Ci, const float* wf, int Co,
+                                int T, int stride, int dil, float* z, double* sums, void* ws, size_t ws_bytes,
+                                void* stream);
+int dva_resnet_bn_sync_stats(const double* sums, int C, int64_t n, float momentum, float eps, float* running_mean,
+                             float* running_var, float* mean, float* invstd, void* stream);
+
 /* dx [B*H*W, Ci] = the data gradient of conv for dz [B*H'*W', Co] (+ add when add is not NULL; add may alias dx). */
 int dva_resnet_conv_dgrad(const float* dz, int64_t B, int64_t H, int64_t W, int Ci, int Co, const float* wd, int T,
                           int stride, int dil, const float* add, float* dx, void* stream);
@@ -63,6 +76,20 @@ size_t dva_resnet_bn_bwd_workspace_bytes(int64_t M, int C);
 int dva_resnet_bn_bwd(const float* dy, const float* y, const float* z, int64_t M, int C, const float* mean,
                       const float* invstd, const float* gamma, int training, float* dz, float* gout, float* dgamma,
                       float* dbeta, void* ws, size_t ws_bytes, void* stream);
+
+/* The backward of a synchronised BatchNorm in two calls around one all-reduce of `sums` (fp64 [2 * C + 1]: per
+ * channel (sum g, sum g * zhat), then the count):
+ *   dva_resnet_bn_bwd_sums: this rank's sums, reduced in chunk order as in dva_resnet_bn_bwd, with the count M, and
+ *     this rank's dbeta, dgamma (the gradient all-reduce sums them over ranks); ws as dva_resnet_bn_bwd's;
+ *   dva_resnet_bn_sync_bwd: from the all-reduced sums and the global count n (>= max(M, 2)), dz = gamma * invstd *
+ *     (g - sum g / n - zhat * sum (g * zhat) / n) and g to gout when it is not NULL; ws holds C * 16 bytes.
+ * Over the sums of one rank with its own count, the results are those of dva_resnet_bn_bwd bit for bit. */
+int dva_resnet_bn_bwd_sums(const float* dy, const float* y, const float* z, int64_t M, int C, const float* mean,
+                           const float* invstd, float* dgamma, float* dbeta, double* sums, void* ws, size_t ws_bytes,
+                           void* stream);
+int dva_resnet_bn_sync_bwd(const float* dy, const float* y, const float* z, int64_t M, int C, const float* mean,
+                           const float* invstd, const float* gamma, const double* sums, int64_t n, float* dz,
+                           float* gout, void* ws, size_t ws_bytes, void* stream);
 
 /* MaxPool2d(3, stride 2, padding pad), pad 0 or 1: y [B*H'*W', C], H' = (H + 2 pad - 3) / 2 + 1, and the window
  * position (r * 3 + s) of the max: the first valid tap starts as the max and a later one replaces it when greater or
